@@ -27,6 +27,9 @@
 // then per coset a forward network reading those coefficients through a bit-reversed row map and leaving the
 // evaluations in network order — which is exactly the bit-reversed row order the reference leaves in memory
 // (radix_2_dit_parallel.rs:245, fri/src/two_adic_pcs.rs:313-318).  No standalone bit-reversal or scaling pass exists.
+// With two equal passes on the cp.async kernel (2^20 rows by default) the LDE is three launches: inverse pass 1, ONE fused
+// pass (ntt_lde_mid_kernel: inverse pass 2 and every coset's forward pass 1, tile by tile through shared memory and registers)
+// and forward pass 2, so the coefficients are written and read once.  Every other LDE runs the four passes as separate launches.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -50,6 +53,17 @@ namespace p3 {
 static int env_int(const char *name, int dflt) {
     const char *s = getenv(name);
     return s ? atoi(s) : dflt;
+}
+
+// Profiling build: each launch gets its own 1 MiB window of the timeline buffer (8 windows, reused in turn).
+static unsigned long long *prof_window() {
+#ifdef P3GPU_NTT_PROFILE
+    static int launch_no = 0;
+    const char *pb = getenv("P3GPU_NTT_PROFBUF");
+    return pb ? reinterpret_cast<unsigned long long *>(strtoull(pb, nullptr, 0)) + (size_t)(launch_no++ % 8) * (1u << 17) : nullptr;
+#else
+    return nullptr;
+#endif
 }
 
 struct PassArgs {
@@ -433,6 +447,146 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
                 c += dc; g += dg;
                 if (c >= cw) { c -= cw; g++; }
             }
+        }
+        P3_STAMP(5);
+    }
+}
+
+// ---- fused middle passes of the two-pass coset LDE (2^(2r) rows, 7 <= r <= 10) ------------------------------------
+// The inverse network's second pass (layers [r, 2r)) and the forward networks' first pass (layers [0, r), read through the
+// bit-reversed row map) touch the same data tile by tile: inverse tile T holds coefficient rows T*2^r + rho, and forward tile
+// L = bitrev_r(T) reads exactly those rows, its local row rho' = bitrev_r(rho).  One kernel does both, so the coefficients
+// cross HBM once (read) instead of three times (write, re-read, scattered re-read):
+//   * the tile (2^r contiguous rows x ct columns) and its inverse twiddles stream in with cp.async, double-buffered as in
+//     ntt_pass_fast_kernel; the forward twiddles of every coset (layers [0, r): the same for every tile) are staged once;
+//   * inverse step 1: Q1 layers in place in shared memory; inverse step 2: Q2 layers into registers.  A step-2 item holds local
+//     rows g*E2 + m, i.e. forward rows bitrev_Q2(m)*E1 + bitrev_Q1(g): exactly one forward step-1 item (Q2 layers on rows
+//     gf + j*E1, gf = bitrev_Q1(g)), so the coefficients stay in that thread's registers for all cosets;
+//   * per coset: forward step 1 in registers, stored to the tile buffer in forward layout, then forward step 2 (Q1 layers) on
+//     consecutive local rows straight to that coset's output block, where the four-launch path's forward pass 1 stores it.
+// THREADS = E1 * CT_T (E1 * 12 for the runtime-width variant) gives every forward step-1 item (E1*cw of them) its own thread.
+template <int R_LOG, int CT_T> __host__ __device__ constexpr int lde_mid_threads() { return (1 << (R_LOG / 2)) * (CT_T ? CT_T : 12); }
+
+template <int F, int R_LOG, int CT_T>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
+__global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd) {
+    constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
+    constexpr u32 E1 = 1u << Q1, E2 = 1u << Q2, R = 1u << R_LOG;
+    constexpr u32 THREADS = lde_mid_threads<R_LOG, CT_T>();
+    const u32 CT = CT_T ? (u32)CT_T : a.ct;
+    const u32 gs1 = E2 * CT + ((CT + 32u - ((E2 * CT) & 31u)) & 31u);   // inverse layout: E1 groups of E2 local rows
+    const u32 gs2 = E1 * CT + ((CT + 32u - ((E1 * CT) & 31u)) & 31u);   // forward layout: E2 groups of E1 local rows
+    const u32 buf_words = (max(E1 * gs1, E2 * gs2) + 3u) & ~3u;
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
+    uint2 *twi0 = reinterpret_cast<uint2 *>(data0 + 2 * buf_words);    // the tile's inverse twiddles, double-buffered
+    uint2 *twf = twi0 + 2 * R;                                          // forward twiddles, R per coset
+
+    const u32 total = (1u << (a.log_n - R_LOG)) * a.n_ctiles;
+    auto issue = [&](u32 t, u32 buf) {
+        const u32 ctile = t % a.n_ctiles, T = t / a.n_ctiles;
+        const u32 col = ctile * CT, cw = min(CT, a.w - col);
+        uint2 *tws = twi0 + buf * R;
+        for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {   // tws[2^lam + q] = Z_inv[2^(r+lam) + T*2^lam + q]
+            const int lam = 31 - __clz(k);
+            cp_async8(tws + k, a.tw + ((size_t)1 << (R_LOG + lam)) + ((size_t)T << lam) + (k - (1u << lam)));
+        }
+        const u32 cpr = cw >> 2;                         // 16-byte chunks per row segment
+        const u32 rs = (THREADS / cpr) & ~(E2 - 1u);     // rows per sweep, >= E2 because THREADS >= 4 * E1 * cpr
+        if (threadIdx.x < rs * cpr) {
+            const u32 rho0 = threadIdx.x / cpr, e = 4u * (threadIdx.x - rho0 * cpr);
+            u32 *dst = data0 + buf * buf_words + (rho0 >> Q2) * gs1 + (rho0 & (E2 - 1u)) * CT + e;
+            const u32 *src = a.in + ((size_t)T * R + rho0) * a.w + col + e;
+            const u32 dstep = (rs >> Q2) * gs1;
+            const size_t sstep = (size_t)rs * a.w;
+            for (u32 rho = rho0; rho < R; rho += rs, dst += dstep, src += sstep) cp_async16(dst, src);
+        }
+        cp_async_commit();
+    };
+
+    u32 t = blockIdx.x;
+    if (t >= total) return;
+    for (u32 k = threadIdx.x; k < a.n_cosets * R; k += THREADS)   // heap entries 1..R-1 of every coset (entry 0 is unused)
+        if (k & (R - 1u)) cp_async8(twf + k, tw_fwd + (size_t)(k >> R_LOG) * a.tw_stride + (k & (R - 1u)));
+    issue(t, 0);   // the forward twiddles land with the first tile's group
+    for (u32 k = 0; t < total; t += gridDim.x, k++) {
+        const u32 buf = k & 1u;
+        __syncthreads();   // every warp is done with the buffer that is refilled next
+#ifdef P3GPU_NTT_PROFILE
+        if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
+#endif
+        P3_STAMP(1);
+        if (t + gridDim.x < total) { issue(t + gridDim.x, buf ^ 1u); P3_STAMP(2); cp_async_wait<1>(); }
+        else { P3_STAMP(2); cp_async_wait<0>(); }
+        __syncthreads();
+        P3_STAMP(3);
+        u32 *data = data0 + buf * buf_words;
+        const uint2 *twi = twi0 + buf * R;
+        const u32 ctile = t % a.n_ctiles, T = t / a.n_ctiles;
+        const u32 col = ctile * CT, cw = min(CT, a.w - col);
+        const u32 L = __brev(T) >> (32 - R_LOG);   // the forward tile this inverse tile feeds
+        const u32 dg = THREADS / cw, dc = THREADS - dg * cw;
+        // ---- inverse step 1 (in place): item (g, c) holds local rows g + m*E2
+        {
+            u32 g = threadIdx.x / cw, c = threadIdx.x - g * cw;
+            for (; g < E2; ) {
+                u32 *sp = data + g * CT + c;
+                u32 x[E1];
+#pragma unroll
+                for (u32 m = 0; m < E1; m++) x[m] = sp[m * gs1];
+                reg_network<F, Q1>(x, twi, 1u);
+#pragma unroll
+                for (u32 m = 0; m < E1; m++) sp[m * gs1] = x[m];
+                c += dc; g += dg;
+                if (c >= cw) { c -= cw; g++; }
+            }
+        }
+        __syncthreads();
+        P3_STAMP(4);
+        // ---- inverse step 2 into registers: thread (gf, c) takes inverse item g = bitrev_Q1(gf), local rows g*E2 + m.
+        // (gf, not g, is linear in the thread index so that the per-coset stores below are bank-conflict free.)
+        const u32 gf = threadIdx.x / cw, c = threadIdx.x - gf * cw;
+        const bool active = gf < E1;
+        u32 coef[E2];
+        if (active) {
+            const u32 g = __brev(gf) >> (32 - Q1);
+            const u32 *sp = data + g * gs1 + c;
+#pragma unroll
+            for (u32 m = 0; m < E2; m++) coef[m] = sp[m * CT];
+            reg_network<F, Q2>(coef, twi, E1 + g);
+        }
+        __syncthreads();   // the tile buffer now takes the forward layout
+        for (u32 cs = 0; cs < a.n_cosets; cs++) {
+            const uint2 *tf = twf + cs * R;
+            // ---- forward step 1: forward local rows gf + j*E1 = inverse local rows g*E2 + bitrev_Q2(j)
+            if (active) {
+                u32 y[E2];
+#pragma unroll
+                for (u32 j = 0; j < E2; j++) y[j] = coef[brev_const<Q2>(j)];
+                reg_network<F, Q2>(y, tf, 1u);
+                u32 *sp = data + gf * CT + c;
+#pragma unroll
+                for (u32 j = 0; j < E2; j++) sp[j * gs2] = y[j];
+            }
+            __syncthreads();
+            // ---- forward step 2: item (j, c2) holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
+            {
+                u32 *out = a.out + (size_t)cs * a.out_stride + col;
+                const size_t sstride = (size_t)R * a.w;
+                u32 j = threadIdx.x / cw, c2 = threadIdx.x - j * cw;
+                for (; j < E2; ) {
+                    const u32 *sp = data + j * gs2 + c2;
+                    u32 x[E1];
+#pragma unroll
+                    for (u32 b = 0; b < E1; b++) x[b] = sp[b * CT];
+                    reg_network<F, Q1>(x, tf, E2 + j);
+                    u32 *p = out + ((size_t)L + ((size_t)j << (Q1 + R_LOG))) * a.w + c2;
+#pragma unroll
+                    for (u32 b = 0; b < E1; b++) p[b * sstride] = x[b];
+                    c2 += dc; j += dg;
+                    if (c2 >= cw) { c2 -= cw; j++; }
+                }
+            }
+            if (cs + 1 < a.n_cosets) __syncthreads();   // the next coset overwrites the buffer
         }
         P3_STAMP(5);
     }
@@ -855,6 +1009,46 @@ static int32_t launch_fast(p3gpu_ctx *ctx, const PassArgs &a) {
     }
 }
 
+template <int F, int R_LOG, int CT_T>
+static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd) {
+    constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
+    constexpr int THREADS = lde_mid_threads<R_LOG, CT_T>();
+    const size_t ct = a.ct, e1 = (size_t)1 << Q1, e2 = (size_t)1 << Q2;
+    const size_t gs1 = e2 * ct + ((ct + 32 - ((e2 * ct) & 31)) & 31), gs2 = e1 * ct + ((ct + 32 - ((e1 * ct) & 31)) & 31);
+    const size_t buf_words = (std::max(e1 * gs1, e2 * gs2) + 3) & ~(size_t)3;
+    const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2);
+    P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: fused LDE tile does not fit shared memory");
+    auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T>;
+    static size_t smem_set[64] = {0};   // per instantiation and device
+    if (smem > 48 * 1024 && smem > smem_set[ctx->device & 63]) {
+        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        smem_set[ctx->device & 63] = smem;
+    }
+    const size_t tiles = ((size_t)1 << (a.log_n - R_LOG)) * a.n_ctiles;
+    // persistent grid: as many CTAs per SM as threads, registers and shared memory allow (one at 2^20 rows)
+    size_t per_sm = std::min<size_t>(2048 / THREADS, (227 * 1024) / (smem + 1024));
+    static int num_regs = 0;   // per instantiation; benign race (same value)
+    if (num_regs == 0) {
+        cudaFuncAttributes fa;
+        P3_CUDA(cudaFuncGetAttributes(&fa, kern));
+        num_regs = std::max(fa.numRegs, 16);
+    }
+    per_sm = std::max<size_t>(1, std::min<size_t>(per_sm, 65536 / ((size_t)THREADS * (size_t)num_regs)));
+    const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
+    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, tw_fwd);
+    ctx->launches++;
+    P3_CUDA(cudaGetLastError());
+    return P3GPU_OK;
+}
+template <int F, int R_LOG>
+static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd) {
+    switch (a.ct) {
+        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd);
+        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd);
+        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd);
+    }
+}
+
 // ---- pipelined kernel: host side -------------------------------------------------------------------------------
 typedef CUresult (*TensorMapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                       const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -902,7 +1096,8 @@ static int32_t make_pass_tensor_map(const PassArgs &a, bool perm, CUtensorMap *t
 // kernel, everything else eligible on the pipeline.  Measured on H100 (400 W), ms, cp.async kernel (512 threads) vs pipeline
 // (tiled intermediates for the LDE), blowup 2: LDE KoalaBear 2^20 x 100 3.3 vs 4.0, 2^20 x 1312 35.4 vs 36.5, BabyBear
 // 2^22 x 300 85 vs 62, 2^21 x 200 24.3 vs 24.1, KoalaBear 2^18 x 64 0.45 vs 0.37; DFT 2^20 x 100 1.39 vs 2.36, 2^21 x 200
-// 8.5 vs 6.6.  (2^22 and 2^21 run 8+7+7 and 7+7+7 layers, 2^18 9+9.)
+// 8.5 vs 6.6.  (2^22 and 2^21 run 8+7+7 and 7+7+7 layers, 2^18 9+9.)  Those LDE figures are for four launches; the cp.async
+// LDE now fuses its middle passes (coset_lde_impl), which made the 2^20 x 100 LDE 3.10 ms (DESIGN 4.1).
 static int pipe_mode() { return env_int("P3GPU_NTT_PIPE", -1); }
 static bool cp_async_pass(int r) { return r == 10; }
 
@@ -985,6 +1180,29 @@ static u32 choose_tile_width(u32 w) {
     return ct > 24 ? 24 : ct;
 }
 
+// Column tile width of the fused LDE middle pass: at most 20 columns (24-column tiles become two of 12); 0 = no 16-byte
+// aligned width (w % 4 != 0), which the fused pass does not take.
+static u32 lde_mid_tile_width(u32 w) {
+    const u32 ct = choose_tile_width(w);
+    if (w % 4 != 0 || ct % 4 != 0 || ct > 24) return 0;
+    return ct == 24 ? 12 : ct;
+}
+
+// a: the inverse network's second pass (l0 = r, l1 = 2r) over the coefficient buffer, writing the forward networks' first-pass
+// results of a.n_cosets cosets to a.out (blocks a.out_stride apart); tw_fwd: the cosets' forward heaps, a.tw_stride apart.
+template <int F>
+static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd) {
+    a.ct = lde_mid_tile_width(a.w);
+    a.n_ctiles = (a.w + a.ct - 1) / a.ct;
+    a.prof = prof_window();
+    switch (a.l1 - a.l0) {
+        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd);
+        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd);
+        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd);
+        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd);
+    }
+}
+
 // One pass over all columns.
 //   fast path (7 <= r <= 10): ONE launch, tiles of choose_tile_width(w) columns (16/20/24; ragged last tile allowed).
 //   generic path: columns are split greedily into power-of-two tiles of main_ct, main_ct/2, ... columns.
@@ -992,13 +1210,7 @@ template <int F>
 static int32_t launch_pass(p3gpu_ctx *ctx, PassArgs a, unsigned n_cosets, int main_log_ct) {
     a.n_cosets = n_cosets;
     const int r = a.l1 - a.l0;
-#ifdef P3GPU_NTT_PROFILE
-    {   // each launch gets its own 1 MiB window of the timeline buffer
-        static int launch_no = 0;
-        const char *pb = getenv("P3GPU_NTT_PROFBUF");
-        a.prof = pb ? reinterpret_cast<unsigned long long *>(strtoull(pb, nullptr, 0)) + (size_t)(launch_no++ % 8) * (1u << 17) : nullptr;
-    }
-#endif
+    a.prof = prof_window();
     if (!env_int("P3GPU_NTT_GENERIC", 0) && pipe_eligible(a)) return launch_pipe<F>(ctx, a);
     if (r >= 6 && r <= 10 && !env_int("P3GPU_NTT_GENERIC", 0)) {
         const u32 ct = choose_tile_width(a.w);
@@ -1054,6 +1266,7 @@ static NetworkPlan plan_passes(int log_n, int max_r) {
     for (int k = 0; k < p.n_passes; k++) p.bounds[k + 1] = p.bounds[k] + base + (k < extra ? 1 : 0);
     return p;
 }
+static int network_max_r() { return std::min(12, std::max(4, env_int("P3GPU_NTT_MAXR", 10))); }
 
 // Runs the size-2^log_n network on n_cosets (input, output, twiddle heap) triples laid out at fixed strides.
 //   src: input rows, natural order unless in_bitrev (then element i of the network is read from row bitrev(i))
@@ -1064,9 +1277,8 @@ template <int F>
 static int32_t run_network(p3gpu_ctx *ctx, int log_n, size_t w, const uint2 *tw, size_t tw_stride, unsigned n_cosets,
                            const u32 *src, size_t src_stride, int in_bitrev, u32 *dst, size_t dst_stride, int out_bitrev,
                            int out_sh, u32 out_add, u32 *tmp, bool has_scale, uint2 scale, bool final_reduce) {
-    const int max_r = std::min(12, std::max(4, env_int("P3GPU_NTT_MAXR", 10)));
     const int main_log_ct = std::min(5, std::max(0, env_int("P3GPU_NTT_LOGCT", 4)));
-    const NetworkPlan plan = plan_passes(log_n, max_r);
+    const NetworkPlan plan = plan_passes(log_n, network_max_r());
     const bool remap = out_bitrev || out_sh != 0 || out_add != 0;
     const size_t hw = ((size_t)1 << log_n) * w;
     if (remap && plan.n_passes > 1) P3_CHECK(tmp != nullptr, P3GPU_EINVAL, "ntt: scratch missing");
@@ -1233,17 +1445,36 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
     P3_CHECK((in_pitch == 0 || in_pitch == w) && (out_pitch == 0 || out_pitch == w), P3GPU_EUNSUPPORTED,
              "column-block LDE (pitch != width) needs the pipelined tiled path: bit-reversed rows, width %% 4 == 0, width >= 8, height >= 2^12");
     // 1) inverse network: evaluations on H (natural) -> coefficients in network (bit-reversed) order, scaled by 1/h
-    const uint2 *tw_inv = nullptr;
-    P3_TRY(get_twiddles<F>(ctx, log_n, 0, Fp<F>::ONE, 1, &tw_inv));
-    void *coef = nullptr;
-    P3_TRY(ctx_scratch(ctx, h * w * 4, &coef));
-    P3_TRY(run_network<F>(ctx, log_n, w, tw_inv, 0, 1, d_in, 0, 0, (u32 *)coef, 0, 0, 0, 0, nullptr, true, inv_height_scale<F>(h), false));
-
     // 2) forward networks, one per coset.  Memory block cb (h rows) holds the coset with natural index c = bitrev(cb):
     //    points shift * g_big^c * H  (radix_2_dit_parallel.rs:226-239).  The heaps of all cosets are one allocation
     //    (block cb at offset cb*h) so that the cosets run as grid.y of a single launch and share the coefficient reads in L2.
-    const uint2 *tw = nullptr;
+    const uint2 *tw_inv = nullptr, *tw = nullptr;
+    P3_TRY(get_twiddles<F>(ctx, log_n, 0, Fp<F>::ONE, 1, &tw_inv));
     P3_TRY(get_twiddles<F>(ctx, log_n, (int)added_bits, shift, 0, &tw));
+    void *coef = nullptr;
+    P3_TRY(ctx_scratch(ctx, h * w * 4, &coef));
+    // Two equal passes on the cp.async kernel: three launches (inverse pass 1, ntt_lde_mid_kernel, forward pass 2 of every coset)
+    // instead of four, so the coefficients are written once and read once.
+    const NetworkPlan run_plan = plan_passes(log_n, network_max_r());
+    const int r = run_plan.bounds[1];
+    if (bitrev_rows && (cp_async || pipe_mode() == 0) && run_plan.n_passes == 2 && 2 * r == log_n && r >= 7 && r <= 10 && n_cosets <= 4 &&
+        lde_mid_tile_width((u32)w) != 0 && ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) % 16) == 0 &&
+        !env_int("P3GPU_NTT_GENERIC", 0)) {
+        PassArgs a;
+        memset(&a, 0, sizeof a);
+        a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = r;
+        a.tw = tw_inv; a.in = d_in; a.out = (u32 *)coef; a.has_scale = 1; a.scale = inv_height_scale<F>(h);
+        P3_TRY(launch_pass<F>(ctx, a, 1, 4));
+        memset(&a, 0, sizeof a);
+        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
+        a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;
+        P3_TRY(launch_lde_mid<F>(ctx, a, tw));
+        memset(&a, 0, sizeof a);
+        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n;
+        a.tw = tw; a.tw_stride = h; a.in = d_out; a.in_stride = h * w; a.out = d_out; a.out_stride = h * w; a.final_reduce = 1;
+        return launch_pass<F>(ctx, a, (unsigned)n_cosets, 4);
+    }
+    P3_TRY(run_network<F>(ctx, log_n, w, tw_inv, 0, 1, d_in, 0, 0, (u32 *)coef, 0, 0, 0, 0, nullptr, true, inv_height_scale<F>(h), false));
     if (bitrev_rows) {
         P3_TRY(run_network<F>(ctx, log_n, w, tw, h, (unsigned)n_cosets, (const u32 *)coef, 0, 1, d_out, h * w, 0, 0, 0, nullptr, false,
                               make_uint2(0, 0), true));

@@ -1,10 +1,10 @@
 #!/usr/bin/env python3
 """Regenerate profiles/ncu_traffic.json (read by bench.py for `roofline.traffic`) from an ncu capture of ONE 2^20 x 100 LDE step.
 
-    ncu --set full --clock-control none -k regex:ntt_pass_ -s 4 -c 4 -o ntt python tools/run_lde_once.py 2 100
+    ncu --set full --clock-control none -k regex:'ntt_(pass|lde_mid)_' -s 3 -c 3 -o ntt python tools/run_lde_once.py 2 100
     python tools/ncu_traffic.py ntt.ncu-rep profiles/ntt_pass_kernels.txt
 
-dram__bytes_read.sum + dram__bytes_write.sum per launch, summed over the 4 launches of the step.  Also writes the per-launch
+dram__bytes_read.sum + dram__bytes_write.sum per launch, summed over the 3 launches of the step.  Also writes the per-launch
 summary table (tools/ncu_summary.py) next to it."""
 import csv
 import json

@@ -2,7 +2,9 @@
    P3GPU_OUT=$PWD/build/libp3gpu_prof.so P3GPU_OBJ=$PWD/build/obj_prof plonky3_b200/csrc/build.sh -DP3GPU_NTT_PROFILE
    P3GPU_LIB=$PWD/build/libp3gpu_prof.so python tools/ntt_timeline.py [w]).
 Prints, per launch of one 2^20 x w LDE, the mean duration (us) of: wait for the previous tile's readers, cp.async issue,
-load wait, step 1, step 2 (+stores), and the co-residency of CTAs on an SM."""
+load wait, step 1, step 2 (+stores), and the co-residency of CTAs on an SM.  The cp.async LDE is three launches: inverse layers
+0-9, the fused pass (inverse layers 10-19 + forward layers 0-9 of every coset; its "step1" is inverse step 1 and its "step2" all
+the rest) and forward layers 10-19; the pipeline (P3GPU_NTT_PIPE=1) is four."""
 import os, sys, pathlib
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
 import torch
@@ -15,7 +17,7 @@ from plonky3_b200.field import KoalaBear as KB
 from plonky3_b200.gpu import default_gpu
 gpu = default_gpu(0)
 x = torch.randint(0, KB.P, (1 << 20, w), device="cuda", dtype=torch.int32)
-for _ in range(2):   # 2 LDEs = 8 launches = the 8 windows; the second LDE (warm) overwrites windows 4..7
+for _ in range(2):   # the launches of 2 LDEs take the 8 windows in turn; the second LDE is the warm one
     y = gpu.coset_lde_batch(KB.id, x, 1, KB.generator)
 torch.cuda.synchronize()
 raw = buf.cpu().numpy().reshape(8, -1)
@@ -31,14 +33,14 @@ if os.environ.get("P3GPU_NTT_PIPE") == "1":   # dense LDEs take the cp.async ker
               f"step2+stores {np.mean(rows[:, 4] - rows[:, 3]) / 1e3:6.2f} | total {np.mean(rows[:, 4] - rows[:, 1]) / 1e3:6.2f}")
     sys.exit(0)
 b = raw.reshape(8, -1, 16, 8)
-names = ["inverse 0-9", "inverse 10-19", "forward 0-9", "forward 10-19"]
-for li in range(4, 8):
+names = ["inverse 0-9", "inverse 10-19 + forward 0-9 (fused)", "forward 10-19"]
+for li in range(3, 6):
     d = b[li]
     valid = d[:, :, 5] != 0
     n_cta = int(valid[:, 0].sum())
     rows = d[valid]
     start, issued, loaded, s1, s2 = (rows[:, i].astype(np.float64) for i in (1, 2, 3, 4, 5))
-    print(f"launch {names[li - 4]}: {n_cta} CTAs, {len(rows)} stamped tiles")
+    print(f"launch {names[li - 3]}: {n_cta} CTAs, {len(rows)} stamped tiles")
     print(f"   issue {np.mean(issued - start) / 1e3:7.2f} us | load wait {np.mean(loaded - issued) / 1e3:7.2f} | step1 {np.mean(s1 - loaded) / 1e3:7.2f} | "
           f"step2+stores {np.mean(s2 - s1) / 1e3:7.2f} | tile total {np.mean(s2 - start) / 1e3:7.2f}")
     # per CTA: gap between consecutive tiles (includes the leading barrier)

@@ -75,6 +75,7 @@ struct PassArgs {
     u32 ct;        // tile width of the generic-width kernel variant
     u32 n_cosets;  // cosets batched in this launch (fastest-varying part of blockIdx.x)
     u32 vec16;     // fast kernel: row segments are 16-byte aligned (cp.async 16)
+    u32 tma_store; // fast kernel (inverse pass 1 of the three-launch LDE): step 2 writes the tile back to shared memory and ONE tensor copy stores it
     u32 skip_load, skip_store;  // profiling experiments only
     u32 skip_bfly; // profiling experiment only (P3GPU_NTT_NOBFLY=1): move the data, skip the butterflies
     u32 wc;                    // pipelined kernel: columns of this launch (<= w = row pitch of the dense layout)
@@ -269,16 +270,32 @@ __device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
+// Tile stores through the tensor copy engine: the tile's writers make their shared-memory writes visible to the async proxy,
+// meet at a barrier, and one thread stores the whole tile with ONE 5-D tensor copy (box = the padded tile layout: see
+// make_pass_tensor_map).  The copy drains to HBM while the SM computes; a buffer is rewritten only after
+// bulk_wait_read says the copy has read it out of shared memory.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_tile(const CUtensorMap *map, const void *smem, int c0, int c3, int c4) {
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                 ::"l"(reinterpret_cast<unsigned long long>(map)), "r"((u32)__cvta_generic_to_shared(smem)), "r"(c0), "r"(0), "r"(0), "r"(c3), "r"(c4)
+                 : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // Persistent, double-buffered pass kernel.  A CTA (one per SM) walks over tiles of 2^R_LOG rows x `ct` columns:
 //   * tile k+1 (rows as 16-byte cp.async/LDGSTS copies, plus its 2^R_LOG - 1 twiddles) streams into the second shared
 //     buffer while tile k is computed, so HBM latency overlaps the integer work;
-//   * step 1 runs Q1 layers in registers IN PLACE in shared memory, step 2 runs Q2 layers and streams the results to
-//     global memory (per-row TMA bulk stores were tried and rejected: UBLKCP is a warp-uniform instruction, so one
-//     copy per lane serialises into a 32-iteration R2UR/PLOP3 loop per warp);
+//   * step 1 runs Q1 layers in registers IN PLACE in shared memory, step 2 runs Q2 layers and either streams the results to
+//     global memory from registers or (a.tma_store: inverse pass 1 of the three-launch LDE) writes them back in place and
+//     the tile leaves as ONE tensor copy that drains while the next tile computes.  (One 1-D bulk copy per row segment was
+//     rejected: UBLKCP is a warp-uniform instruction, so one copy per lane serialises into a 32-iteration loop per warp.)
 //   * all tiles of a pass have the same runtime width ct (16/20/24 columns; w = 100 -> 5 x 20) so that ONE launch covers
 //     every column and neighbouring tiles share DRAM bursts through L2.
 template <int F, int R_LOG, int CT_T, int THREADS, int NBUF>   // CT_T: compile-time tile width (16/20/24) or 0 = runtime a.ct
-__global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREADS == 256) ? 3 : 2) ntt_pass_fast_kernel(const __grid_constant__ PassArgs a) {
+__global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREADS == 256) ? 3 : 2)
+ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__ CUtensorMap omap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     constexpr u32 E1 = 1u << Q1, E2 = 1u << Q2, R = 1u << R_LOG;
     const u32 CT = CT_T ? (u32)CT_T : a.ct;
@@ -295,6 +312,7 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
     const u32 total = n_row_tiles * a.n_ctiles * a.n_cosets;
     const bool vec16 = a.vec16 != 0;       // row segments 16-byte aligned in global memory (loads AND stores)
     const bool shared_tw = (a.l0 == 0);    // first pass of a network: every tile uses the same twiddles
+    const bool tma_store = NBUF == 2 && a.tma_store;   // the output map omap is set up (launch_fast_rct)
 
     auto decode = [&](u32 t, u32 &coset, u32 &col, u32 &cw, u32 &T, u32 &ibase) {
         coset = t % a.n_cosets;
@@ -370,6 +388,7 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
     if (NBUF == 2) issue(t, 0);
     for (u32 k = 0; t < total; t += gridDim.x, k++) {
         const u32 buf = NBUF == 2 ? (k & 1u) : 0u;
+        if (tma_store && threadIdx.x == 0) bulk_wait_read();   // the previous tile's store has left the buffer refilled next
         __syncthreads();   // every warp is done reading the buffer that is refilled next
 #ifdef P3GPU_NTT_PROFILE
         if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
@@ -428,7 +447,12 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
 #pragma unroll
                     for (u32 m = 0; m < E2; m++) x[m] = fp_reduce<F>(x[m]);
                 }
-                {
+                if (tma_store) {
+                    if (!P3_SKIP(a.skip_store)) {
+#pragma unroll
+                        for (u32 m = 0; m < E2; m++) sp[m * CT] = x[m];
+                    }
+                } else {
                     const u32 i0 = ibase | (g << (lowbits + Q2));
                     const u32 row0 = ((a.out_bitrev ? (__brev(i0) >> brsh) : i0) << a.out_sh) + a.out_add;
                     u32 *p = out + (size_t)row0 * a.w + c;
@@ -447,9 +471,16 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
                 c += dc; g += dg;
                 if (c >= cw) { c -= cw; g++; }
             }
+            if (tma_store && !P3_SKIP(a.skip_store)) {
+                fence_proxy_async_smem();
+                __syncthreads();
+                // tensor coordinates (column, 0, 0, L, T + coset block): see make_pass_tensor_map
+                if (threadIdx.x == 0) tma_store_tile(&omap, data, (int)col, (int)(ibase & ((1u << lowbits) - 1u)), (int)(T + (coset << a.l0)));
+            }
         }
         P3_STAMP(5);
     }
+    if (tma_store && threadIdx.x == 0) bulk_wait_all();
 }
 
 // ---- fused middle passes of the two-pass coset LDE (2^(2r) rows, 7 <= r <= 10) ------------------------------------
@@ -463,12 +494,18 @@ __global__ void __launch_bounds__(THREADS, NBUF == 2 ? 1 : (CT_T == 16 && THREAD
 //     rows g*E2 + m, i.e. forward rows bitrev_Q2(m)*E1 + bitrev_Q1(g): exactly one forward step-1 item (Q2 layers on rows
 //     gf + j*E1, gf = bitrev_Q1(g)), so the coefficients stay in that thread's registers for all cosets;
 //   * per coset: forward step 1 in registers, stored to the tile buffer in forward layout, then forward step 2 (Q1 layers) on
-//     consecutive local rows straight to that coset's output block, where the four-launch path's forward pass 1 stores it.
+//     consecutive local rows, in place; ONE tensor copy (omap) stores the tile to that coset's output block, where the
+//     four-launch path's forward pass 1 stores it; the next coset rewrites the buffer once the copy has read it out, and the
+//     HBM writes drain while the CTA computes;
+//   * work items go in forward-tile order (L, column tile), T = bitrev_r(L): the CTAs resident at once store neighbouring
+//     output rows (runs of ~26 rows per 2^r-row group at 132 SMs) instead of rows 2^r / 32 apart, while each tile's
+//     reads stay one contiguous block of 2^r rows.
 // THREADS = E1 * CT_T (E1 * 12 for the runtime-width variant) gives every forward step-1 item (E1*cw of them) its own thread.
 template <int R_LOG, int CT_T> __host__ __device__ constexpr int lde_mid_threads() { return (1 << (R_LOG / 2)) * (CT_T ? CT_T : 12); }
 
 template <int F, int R_LOG, int CT_T>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
-__global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd) {
+__global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1)
+ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, const __grid_constant__ CUtensorMap omap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     constexpr u32 E1 = 1u << Q1, E2 = 1u << Q2, R = 1u << R_LOG;
     constexpr u32 THREADS = lde_mid_threads<R_LOG, CT_T>();
@@ -483,7 +520,7 @@ __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid
 
     const u32 total = (1u << (a.log_n - R_LOG)) * a.n_ctiles;
     auto issue = [&](u32 t, u32 buf) {
-        const u32 ctile = t % a.n_ctiles, T = t / a.n_ctiles;
+        const u32 ctile = t % a.n_ctiles, T = __brev(t / a.n_ctiles) >> (32 - R_LOG);
         const u32 col = ctile * CT, cw = min(CT, a.w - col);
         uint2 *tws = twi0 + buf * R;
         for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {   // tws[2^lam + q] = Z_inv[2^(r+lam) + T*2^lam + q]
@@ -510,6 +547,7 @@ __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid
     issue(t, 0);   // the forward twiddles land with the first tile's group
     for (u32 k = 0; t < total; t += gridDim.x, k++) {
         const u32 buf = k & 1u;
+        if (threadIdx.x == 0) bulk_wait_read();   // the previous tile's last store has left the buffer refilled next
         __syncthreads();   // every warp is done with the buffer that is refilled next
 #ifdef P3GPU_NTT_PROFILE
         if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
@@ -521,9 +559,8 @@ __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid
         P3_STAMP(3);
         u32 *data = data0 + buf * buf_words;
         const uint2 *twi = twi0 + buf * R;
-        const u32 ctile = t % a.n_ctiles, T = t / a.n_ctiles;
+        const u32 ctile = t % a.n_ctiles, L = t / a.n_ctiles;
         const u32 col = ctile * CT, cw = min(CT, a.w - col);
-        const u32 L = __brev(T) >> (32 - R_LOG);   // the forward tile this inverse tile feeds
         const u32 dg = THREADS / cw, dc = THREADS - dg * cw;
         // ---- inverse step 1 (in place): item (g, c) holds local rows g + m*E2
         {
@@ -533,7 +570,7 @@ __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid
                 u32 x[E1];
 #pragma unroll
                 for (u32 m = 0; m < E1; m++) x[m] = sp[m * gs1];
-                reg_network<F, Q1>(x, twi, 1u);
+                if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q1>(x, twi, 1u);
 #pragma unroll
                 for (u32 m = 0; m < E1; m++) sp[m * gs1] = x[m];
                 c += dc; g += dg;
@@ -552,44 +589,67 @@ __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1) ntt_lde_mid
             const u32 *sp = data + g * gs1 + c;
 #pragma unroll
             for (u32 m = 0; m < E2; m++) coef[m] = sp[m * CT];
-            reg_network<F, Q2>(coef, twi, E1 + g);
+            if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q2>(coef, twi, E1 + g);
         }
-        __syncthreads();   // the tile buffer now takes the forward layout
+#ifdef P3GPU_NTT_PROFILE
+        unsigned long long store_wait = 0;   // slot 6: time thread 0 waits for the previous coset's store to leave the buffer
+#endif
         for (u32 cs = 0; cs < a.n_cosets; cs++) {
             const uint2 *tf = twf + cs * R;
+            // (Running forward step 1 before this wait keeps y[] live next to coef[] across it: 80 bytes of spills at r = 10, ct = 20.)
+            if (cs > 0 && threadIdx.x == 0) {   // the previous coset's store has left the buffer
+#ifdef P3GPU_NTT_PROFILE
+                unsigned long long w0_, w1_;
+                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
+                bulk_wait_read();
+                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
+                store_wait += w1_ - w0_;
+#else
+                bulk_wait_read();
+#endif
+            }
+            __syncthreads();   // the tile buffer takes the forward layout (cs = 0: every warp is done with inverse step 2)
             // ---- forward step 1: forward local rows gf + j*E1 = inverse local rows g*E2 + bitrev_Q2(j)
             if (active) {
                 u32 y[E2];
 #pragma unroll
                 for (u32 j = 0; j < E2; j++) y[j] = coef[brev_const<Q2>(j)];
-                reg_network<F, Q2>(y, tf, 1u);
+                if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q2>(y, tf, 1u);
                 u32 *sp = data + gf * CT + c;
 #pragma unroll
                 for (u32 j = 0; j < E2; j++) sp[j * gs2] = y[j];
             }
             __syncthreads();
-            // ---- forward step 2: item (j, c2) holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
+            // ---- forward step 2 (in place): item (j, c2) holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
             {
-                u32 *out = a.out + (size_t)cs * a.out_stride + col;
-                const size_t sstride = (size_t)R * a.w;
                 u32 j = threadIdx.x / cw, c2 = threadIdx.x - j * cw;
                 for (; j < E2; ) {
-                    const u32 *sp = data + j * gs2 + c2;
+                    u32 *sp = data + j * gs2 + c2;
                     u32 x[E1];
 #pragma unroll
                     for (u32 b = 0; b < E1; b++) x[b] = sp[b * CT];
-                    reg_network<F, Q1>(x, tf, E2 + j);
-                    u32 *p = out + ((size_t)L + ((size_t)j << (Q1 + R_LOG))) * a.w + c2;
+                    if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q1>(x, tf, E2 + j);
+                    if (!P3_SKIP(a.skip_store)) {
 #pragma unroll
-                    for (u32 b = 0; b < E1; b++) p[b * sstride] = x[b];
+                        for (u32 b = 0; b < E1; b++) sp[b * CT] = x[b];
+                    }
                     c2 += dc; j += dg;
                     if (c2 >= cw) { c2 -= cw; j++; }
                 }
             }
-            if (cs + 1 < a.n_cosets) __syncthreads();   // the next coset overwrites the buffer
+            if (!P3_SKIP(a.skip_store)) {
+                fence_proxy_async_smem();
+                __syncthreads();
+                // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
+                if (threadIdx.x == 0) tma_store_tile(&omap, data, (int)col, (int)L, (int)cs);
+            }
         }
+#ifdef P3GPU_NTT_PROFILE
+        if (a.prof && threadIdx.x == 0 && k < 16) a.prof[((size_t)blockIdx.x * 16 + k) * 8 + 6] = store_wait;
+#endif
         P3_STAMP(5);
     }
+    if (threadIdx.x == 0) bulk_wait_all();
 }
 
 // ---- pipelined path: TMA tile loads + warp-specialised consumer groups -------------------------------------------
@@ -947,13 +1007,23 @@ static int32_t launch_pass_ct(p3gpu_ctx *ctx, const PassArgs &a) {
     return P3GPU_OK;
 }
 
+static int32_t make_pass_tensor_map(const PassArgs &a, const u32 *base, bool tiled, size_t blk_stride, u32 box_w, bool perm, int gs_log,
+                                    CUtensorMap *tm);
+
 template <int F, int R_LOG, int CT_T, int THREADS, int NBUF>
-static int32_t launch_fast_rct(p3gpu_ctx *ctx, const PassArgs &a) {
+static int32_t launch_fast_rct(p3gpu_ctx *ctx, PassArgs a) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     const u32 ct = a.ct;
     const u32 e2 = 1u << Q2, e1 = 1u << Q1;
     const u32 padw = (ct + 32u - ((e2 * ct) & 31u)) & 31u;
     const size_t buf_words = ((size_t)e1 * (e2 * ct + padw) + 3) & ~(size_t)3;
+    CUtensorMap omap;
+    memset(&omap, 0, sizeof omap);
+    a.tma_store = a.tma_store && NBUF == 2 && a.vec16;
+    if (a.tma_store) {   // the padded tile is the store box: group stride (2^Q2 + 1) * ct words (always so for ct % 4 == 0)
+        P3_CHECK(e2 * ct + padw == (e2 + 1) * ct && !a.out_bitrev && a.out_sh == 0 && a.out_add == 0, P3GPU_EINVAL, "ntt: tile layout is no TMA box");
+        P3_TRY(make_pass_tensor_map(a, a.out, false, a.out_stride, ct, false, Q2, &omap));
+    }
     const size_t smem = NBUF * buf_words * 4 + NBUF * ((size_t)1 << R_LOG) * sizeof(uint2);
     auto kern = ntt_pass_fast_kernel<F, R_LOG, CT_T, THREADS, NBUF>;
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: tile does not fit shared memory");
@@ -976,7 +1046,7 @@ static int32_t launch_fast_rct(p3gpu_ctx *ctx, const PassArgs &a) {
     if (per_sm > by_regs) per_sm = by_regs;
     if (per_sm < 1) per_sm = 1;
     const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
-    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a);
+    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, omap);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
@@ -1010,7 +1080,7 @@ static int32_t launch_fast(p3gpu_ctx *ctx, const PassArgs &a) {
 }
 
 template <int F, int R_LOG, int CT_T>
-static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd) {
+static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     constexpr int THREADS = lde_mid_threads<R_LOG, CT_T>();
     const size_t ct = a.ct, e1 = (size_t)1 << Q1, e2 = (size_t)1 << Q2;
@@ -1018,6 +1088,7 @@ static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 
     const size_t buf_words = (std::max(e1 * gs1, e2 * gs2) + 3) & ~(size_t)3;
     const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2);
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: fused LDE tile does not fit shared memory");
+    P3_CHECK(gs2 == (e1 + 1) * ct, P3GPU_EINVAL, "ntt: fused LDE tile layout is no TMA box");
     auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T>;
     static size_t smem_set[64] = {0};   // per instantiation and device
     if (smem > 48 * 1024 && smem > smem_set[ctx->device & 63]) {
@@ -1035,17 +1106,17 @@ static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 
     }
     per_sm = std::max<size_t>(1, std::min<size_t>(per_sm, 65536 / ((size_t)THREADS * (size_t)num_regs)));
     const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
-    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, tw_fwd);
+    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, tw_fwd, omap);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
 template <int F, int R_LOG>
-static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd) {
+static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap) {
     switch (a.ct) {
-        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd);
-        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd);
-        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd);
+        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd, omap);
+        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd, omap);
+        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd, omap);
     }
 }
 
@@ -1064,28 +1135,34 @@ static TensorMapEncodeFn tensor_map_encoder() {
     return fn;
 }
 
-// 5-D view of the pass input for ntt_pass_pipe_kernel: (column, row-in-group, group, L, T) with the tile's local row
-// rho = group * GS + row-in-group at global row  T * 2^(n-l0) + rho * 2^lowbits + L   (PERM: block * 2^r + position).
-static int32_t make_pass_tensor_map(const PassArgs &a, bool perm, CUtensorMap *tm) {
+// 5-D view of a pass's input or output over `base` for tensor copies of whole tiles: (column, row-in-group, group, L, T) with
+// the tile's local row rho = group * 2^gs_log + row-in-group at global row  T * 2^(n-l0) + rho * 2^lowbits + L   (PERM: block * 2^r
+// + position).  The box is (box_w, 2^gs_log + 1, 2^(r - gs_log), 1, 1): one row more per group than the tensor has, which a load
+// zero-fills and a store skips, so the box is exactly the padded shared-memory tile (group stride (2^gs_log + 1) * box_w words).
+// box_w * 4 must be a multiple of 16 bytes; columns past the width are skipped by stores (a ragged last column tile).
+// Dense layout (tiled = 0): pitch w; blk_stride != 0 (= w * 2^n) stacks the n_cosets blocks in the last dimension, whose
+// coordinate is then T + (block << l0).  Tiled layout (ntt_pass_pipe_kernel only): 8-column matrices of 2^n rows.
+static int32_t make_pass_tensor_map(const PassArgs &a, const u32 *base, bool tiled, size_t blk_stride, u32 box_w, bool perm, int gs_log,
+                                    CUtensorMap *tm) {
     TensorMapEncodeFn enc = tensor_map_encoder();
     P3_CHECK(enc != nullptr, P3GPU_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const int r = a.l1 - a.l0, q2 = (r + 1) / 2, q1 = r - q2, lowbits = a.log_n - a.l1;
-    const cuuint64_t pitch = a.in_tiled ? 32 : (cuuint64_t)a.w * 4;
-    const cuuint64_t n_ctiles = (a.wc + 7) / 8;
+    const int r = a.l1 - a.l0, lowbits = a.log_n - a.l1;
+    const u32 wc = a.wc ? a.wc : a.w;
+    const cuuint64_t pitch = tiled ? 32 : (cuuint64_t)a.w * 4;
+    const cuuint64_t n_ctiles = (wc + 7) / 8;
     cuuint64_t dims[5], strides[4];
-    cuuint32_t box[5] = {8, 0, 0, 1, 1}, es[5] = {1, 1, 1, 1, 1};
-    dims[0] = a.in_tiled ? 8 : a.wc;
-    const cuuint64_t in_blocks = a.in_tiled ? n_ctiles * a.in_blocks : (a.in_stride ? a.n_cosets : 1);
+    cuuint32_t box[5] = {box_w, (1u << gs_log) + 1, 1u << (r - gs_log), 1, 1}, es[5] = {1, 1, 1, 1, 1};
+    dims[0] = tiled ? 8 : wc;
+    dims[1] = 1ull << gs_log; dims[2] = 1ull << (r - gs_log);
+    const cuuint64_t blocks = tiled ? n_ctiles * a.in_blocks : (blk_stride ? a.n_cosets : 1);
     if (!perm) {
-        dims[1] = 1ull << q2; dims[2] = 1ull << q1; dims[3] = 1ull << lowbits; dims[4] = in_blocks << a.l0;
-        strides[0] = pitch << lowbits; strides[1] = pitch << (lowbits + q2); strides[2] = pitch; strides[3] = pitch << (a.log_n - a.l0);
-        box[1] = (1u << q2) + 1; box[2] = 1u << q1;
+        dims[3] = 1ull << lowbits; dims[4] = blocks << a.l0;
+        strides[0] = pitch << lowbits; strides[1] = pitch << (lowbits + gs_log); strides[2] = pitch; strides[3] = pitch << (a.log_n - a.l0);
     } else {
-        dims[1] = 1ull << q1; dims[2] = 1ull << q2; dims[3] = 1; dims[4] = in_blocks << (a.log_n - r);
-        strides[0] = pitch; strides[1] = pitch << q1; strides[2] = pitch; strides[3] = pitch << r;
-        box[1] = (1u << q1) + 1; box[2] = 1u << q2;
+        dims[3] = 1; dims[4] = blocks << (a.log_n - r);
+        strides[0] = pitch; strides[1] = pitch << gs_log; strides[2] = pitch; strides[3] = pitch << r;
     }
-    const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(a.in), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
     return P3GPU_OK;
@@ -1097,7 +1174,7 @@ static int32_t make_pass_tensor_map(const PassArgs &a, bool perm, CUtensorMap *t
 // (tiled intermediates for the LDE), blowup 2: LDE KoalaBear 2^20 x 100 3.3 vs 4.0, 2^20 x 1312 35.4 vs 36.5, BabyBear
 // 2^22 x 300 85 vs 62, 2^21 x 200 24.3 vs 24.1, KoalaBear 2^18 x 64 0.45 vs 0.37; DFT 2^20 x 100 1.39 vs 2.36, 2^21 x 200
 // 8.5 vs 6.6.  (2^22 and 2^21 run 8+7+7 and 7+7+7 layers, 2^18 9+9.)  Those LDE figures are for four launches; the cp.async
-// LDE now fuses its middle passes (coset_lde_impl), which made the 2^20 x 100 LDE 3.10 ms (DESIGN 4.1).
+// LDE now fuses its middle passes and stores tiles with tensor copies (coset_lde_impl): 2.72 ms for 2^20 x 100 (DESIGN 4.1).
 static int pipe_mode() { return env_int("P3GPU_NTT_PIPE", -1); }
 static bool cp_async_pass(int r) { return r == 10; }
 
@@ -1127,7 +1204,7 @@ static int32_t launch_pipe_r(p3gpu_ctx *ctx, PassArgs a) {
     CUtensorMap tm;
     if (a.wc == 0) a.wc = a.w;
     if (a.in_blocks == 0) a.in_blocks = 1;
-    P3_TRY(make_pass_tensor_map(a, PERM, &tm));
+    P3_TRY(make_pass_tensor_map(a, a.in, a.in_tiled, a.in_stride, 8, PERM, PERM ? Q1 : Q2, &tm));
     a.n_ctiles = (a.wc + 7) / 8;
     const size_t units = ((size_t)1 << (a.log_n - R_LOG)) * a.n_cosets;
     // few units (small transforms): split a unit's column tiles over several CTAs so that every SM has work
@@ -1195,11 +1272,19 @@ static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd) {
     a.ct = lde_mid_tile_width(a.w);
     a.n_ctiles = (a.w + a.ct - 1) / a.ct;
     a.prof = prof_window();
-    switch (a.l1 - a.l0) {
-        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd);
-        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd);
-        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd);
-        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd);
+    a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
+    // output = the forward networks' first pass (layers [0, r)) over the cosets' blocks: tile L, local row j*2^Q1 + b at row
+    // L + 2^r * (j*2^Q1 + b), i.e. the pass map with groups of 2^Q1 rows (the forward layout gs2 = (2^Q1 + 1) * ct words)
+    const int r = a.l1 - a.l0;
+    PassArgs o = a;
+    o.l0 = 0; o.l1 = r;
+    CUtensorMap omap;
+    P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
+    switch (r) {
+        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd, omap);
+        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd, omap);
+        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd, omap);
+        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd, omap);
     }
 }
 
@@ -1459,10 +1544,12 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
     const int r = run_plan.bounds[1];
     if (bitrev_rows && (cp_async || pipe_mode() == 0) && run_plan.n_passes == 2 && 2 * r == log_n && r >= 7 && r <= 10 && n_cosets <= 4 &&
         lde_mid_tile_width((u32)w) != 0 && ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) % 16) == 0 &&
-        !env_int("P3GPU_NTT_GENERIC", 0)) {
+        tensor_map_encoder() != nullptr && !env_int("P3GPU_NTT_GENERIC", 0)) {
+        // inverse pass 1 and the fused pass store whole tiles with tensor copies.  Forward pass 2 keeps its register stores: its
+        // rows are contiguous already, and the tensor copies measured 3 % slower there (DESIGN 4.1)
         PassArgs a;
         memset(&a, 0, sizeof a);
-        a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = r;
+        a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = r; a.tma_store = 1;
         a.tw = tw_inv; a.in = d_in; a.out = (u32 *)coef; a.has_scale = 1; a.scale = inv_height_scale<F>(h);
         P3_TRY(launch_pass<F>(ctx, a, 1, 4));
         memset(&a, 0, sizeof a);

@@ -1,10 +1,12 @@
 """Per-CTA phase timeline of the NTT pass kernel (needs the instrumented build:
    P3GPU_OUT=$PWD/build/libp3gpu_prof.so P3GPU_OBJ=$PWD/build/obj_prof plonky3_b200/csrc/build.sh -DP3GPU_NTT_PROFILE
    P3GPU_LIB=$PWD/build/libp3gpu_prof.so python tools/ntt_timeline.py [w]).
-Prints, per launch of one 2^20 x w LDE, the mean duration (us) of: wait for the previous tile's readers, cp.async issue,
-load wait, step 1, step 2 (+stores), and the co-residency of CTAs on an SM.  The cp.async LDE is three launches: inverse layers
-0-9, the fused pass (inverse layers 10-19 + forward layers 0-9 of every coset; its "step1" is inverse step 1 and its "step2" all
-the rest) and forward layers 10-19; the pipeline (P3GPU_NTT_PIPE=1) is four."""
+Prints, per launch of one 2^20 x w LDE, the mean duration (us) of: cp.async issue, load wait, step 1, step 2 (+stores), and
+the gap between a CTA's tiles.  The cp.async LDE is three launches: inverse layers 0-9, the fused pass (inverse layers 10-19 +
+forward layers 0-9 of every coset; its "step1" is inverse step 1 and its "step2" all the rest) and forward layers 10-19; the
+pipeline (P3GPU_NTT_PIPE=1) is four.  The first two store their tiles with tensor copies: their gap between tiles includes the
+wait for the previous tile's store to leave the buffer that is refilled next, and the fused pass also reports the time it waits
+for one coset's store before the next coset rewrites the tile buffer."""
 import os, sys, pathlib
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parent.parent))
 import torch
@@ -43,7 +45,9 @@ for li in range(3, 6):
     print(f"launch {names[li - 3]}: {n_cta} CTAs, {len(rows)} stamped tiles")
     print(f"   issue {np.mean(issued - start) / 1e3:7.2f} us | load wait {np.mean(loaded - issued) / 1e3:7.2f} | step1 {np.mean(s1 - loaded) / 1e3:7.2f} | "
           f"step2+stores {np.mean(s2 - s1) / 1e3:7.2f} | tile total {np.mean(s2 - start) / 1e3:7.2f}")
-    # per CTA: gap between consecutive tiles (includes the leading barrier)
+    if li == 4:   # slot 6: the fused pass's waits for a coset's store to leave the tile buffer, summed over the tile's cosets
+        print(f"   wait for the previous coset's store {np.mean(rows[:, 6].astype(np.float64)) / 1e3:7.2f} us per tile")
+    # per CTA: gap between consecutive tiles (the wait for the store of the buffer refilled next, and the leading barrier)
     gaps = []
     for c in range(d.shape[0]):
         k = int(valid[c].sum())

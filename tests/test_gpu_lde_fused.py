@@ -3,8 +3,8 @@ and every coset's forward layers [0, r), csrc/ntt.cu ntt_lde_mid_kernel) and for
 takes it by default; P3GPU_NTT_PIPE=0 puts every two-pass height on it, so the whole output can be checked against the CPU
 oracle at 2^14-2^18 (7 to 9 layers per pass).  Widths: 20-column tiles (100), ragged 16-column tiles (44 = 16 + 16 + 12),
 one 16-column tile, narrow runtime-width tiles (8; 24 = 12 + 12) and a width without 16-byte row segments (6), which keeps the
-four-launch path."""
-import numpy as np
+four-launch path.  Each case asserts its launch count and writes into a poisoned, guarded buffer after a dirty call on other
+data (test_gpu_lde_paths.run_lde_checked)."""
 import pytest
 import torch
 
@@ -13,6 +13,7 @@ from oracle import p3_oracle as O
 from plonky3_b200 import _lib
 from plonky3_b200.field import BabyBear, KoalaBear
 from plonky3_b200.gpu import default_gpu
+from test_gpu_lde_paths import run_lde_checked
 
 pytestmark = pytest.mark.gpu
 
@@ -31,6 +32,4 @@ def gpu():
 def test_two_pass_lde_on_cp_async_kernel_matches_oracle(gpu, f, log_h, w, added_bits, monkeypatch):
     monkeypatch.setenv("P3GPU_NTT_PIPE", "0")
     m = O.random_matrix(f.id, 1 << log_h, w, seed=1000 * log_h + 10 * w + added_bits)
-    x = torch.from_numpy(m.view(np.int32)).cuda()
-    got = gpu.coset_lde_batch(f.id, x, added_bits, f.generator).cpu().numpy().view(np.uint32)
-    assert np.array_equal(got, O.coset_lde_batch(f.id, m, added_bits, f.generator, bitrev_out=True))
+    run_lde_checked(gpu, f, m, added_bits, f.generator, launches=4 if w % 4 else 3)   # w = 6: no 16-byte rows, four launches

@@ -100,6 +100,11 @@ unsafe extern "C" {
     pub fn p3gpu_peer_allgather_dev(ctx: *mut P3GpuCtx, grp: *const P3GpuPeerGroup, table_offset_bytes: usize, d_src: *const u32, words: usize) -> i32;
     pub fn p3gpu_coset_lde_batch_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, grp: *const P3GpuPeerGroup, d_in: *const u32, h: usize,
                                              w_local: usize, added_bits: c_uint, shift: u32, w_total: usize, col_off: usize) -> i32;
+    pub fn p3gpu_shard_col_segments(world: u32, col_starts: *const usize, rows: usize, segs: *mut usize, max_segs: usize, n_segs: *mut usize) -> i32;
+    pub fn p3gpu_peer_exchange_dev(ctx: *mut P3GpuCtx, grp: *const P3GpuPeerGroup, epoch: *mut u32, bufs: *const *mut c_void, d_src: *const u32,
+                                   words: usize) -> i32;
+    pub fn p3gpu_p2air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
+                                            log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
 
     // streams, counters
     pub fn p3gpu_ctx_set_stream(ctx: *mut P3GpuCtx, cuda_stream: *mut c_void) -> i32;
@@ -122,6 +127,8 @@ unsafe extern "C" {
     pub fn p3gpu_p2air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_perms: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_p2air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_lde: *const u32, log_lde_height: c_uint,
                                     log_trace_height: c_uint, alpha: *const u32, d_quotient: *mut u32) -> i32;
+    pub fn p3gpu_p2air_generate_trace_cols_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_inputs: *const u32, n_perms: usize,
+                                               col0: usize, col1: usize, d_out: *mut u32) -> i32;
 
     // DuplexChallenger with device-resident state
     pub fn p3gpu_challenger_new(ctx: *mut P3GpuCtx, field: c_int, width: c_int, rate: c_int, out: *mut *mut P3GpuChallenger) -> i32;

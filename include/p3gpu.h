@@ -220,6 +220,11 @@ int32_t p3gpu_p2air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t
  * d_quotient: 2^log_lde_height EF4 values in NATURAL order (what commit_quotient / split_evals consume). */
 int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_lde, unsigned log_lde_height,
                                  unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient);
+/* Columns [col0, col1) of the trace p3gpu_p2air_generate_trace_dev writes for the same inputs (n_perms a multiple of
+ * vector_len): d_out is the dense (n_perms / vector_len) x (col1 - col0) matrix — one rank's column block of a sharded prove,
+ * built without the full trace.  The window may cut a permutation. */
+int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms,
+                                            size_t col0, size_t col1, uint32_t *d_out);
 
 /* ---- transcript and query phase of the prove driver (SURVEY.md 8f rank 4 / N1) ----------------------------------------
  * DuplexChallenger<F, Poseidon2<width>, width, rate> (challenger/src/duplex_challenger.rs:60-300) with its state resident on the
@@ -297,6 +302,26 @@ int32_t p3gpu_commit_sharded_dev(p3gpu_ctx *ctx, int field, int hash, const p3gp
                                  size_t *n_layers, uint32_t *h_cap, size_t *cap_len, float *phase_ms);
 /* the column chunk boundaries (0 = first, w_local = last) a block of w_local columns is exchanged in; returns their number */
 size_t p3gpu_shard_chunk_bounds(size_t w_local, size_t *bounds, size_t max_bounds);
+/* The column segments of a row block of `rows` rows as p3gpu_commit_sharded_dev leaves it: segs[3k .. 3k+2] = (first column,
+ * end column, element offset of its rows x width row-major matrix in the block), in column order; one dense segment when
+ * world == 1.  P3GPU_EINVAL when a segment bound is not a multiple of 4 columns (a 16-byte load would cross two chunks). */
+int32_t p3gpu_shard_col_segments(uint32_t world, const size_t *col_starts, size_t rows, size_t *segs, size_t max_segs, size_t *n_segs);
+
+/* All-gather over caller-owned exchange buffers: bufs[q] is rank q's buffer (p3gpu_malloc'ed, IPC-mapped; own pointer at
+ * [rank]), at least world * words u32.  Barrier, then copy-engine peer copies of d_src into slot `rank` (u32 offset
+ * rank * words) of every rank's buffer, then barrier: afterwards bufs[rank] holds every rank's `words` in rank order.  Uses
+ * two epochs of *epoch (the same counter as p3gpu_commit_sharded_dev). */
+int32_t p3gpu_peer_exchange_dev(p3gpu_ctx *ctx, const p3gpu_peer_group *grp, uint32_t *epoch, void *const *bufs, const uint32_t *d_src,
+                                size_t words);
+
+/* The Poseidon2 AIR's quotient values (as p3gpu_p2air_quotient_dev) over MY row block after p3gpu_commit_sharded_dev with the same
+ * col_starts: rows [rank * R, (rank + 1) * R) of the bit-reversed LDE, R = 2^log_lde_height / world, read in place from
+ * grp->rows[rank].  d_quotient_slice (R EF4 values) receives the same rows of the quotient in BIT-REVERSED order: entry m is the
+ * value at natural index bitrev(rank * R + m).  The concatenation over the ranks, un-bit-reversed, is p3gpu_p2air_quotient_dev's
+ * output. */
+int32_t p3gpu_p2air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                         unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                         uint32_t *d_quotient_slice);
 
 #ifdef __cplusplus
 }

@@ -28,6 +28,7 @@ EXPORTS = [
     "p3gpu_challenger_sample", "p3gpu_challenger_grind", "p3gpu_gather_rows_dev", "p3gpu_merkle_paths_dev",
     "p3gpu_ipc_export", "p3gpu_ipc_import", "p3gpu_ipc_close", "p3gpu_memset_dev", "p3gpu_peer_barrier_dev",
     "p3gpu_peer_allgather_dev", "p3gpu_coset_lde_batch_sharded_dev", "p3gpu_commit_sharded_dev", "p3gpu_shard_chunk_bounds",
+    "p3gpu_p2air_generate_trace_cols_dev", "p3gpu_shard_col_segments", "p3gpu_peer_exchange_dev", "p3gpu_p2air_quotient_sharded_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -112,6 +113,10 @@ def load():
         "p3gpu_coset_lde_batch_sharded_dev": (i32, [vp, ci, vp, vp, sz, sz, cu, u32, sz, sz]),
         "p3gpu_commit_sharded_dev": (i32, [vp, ci, ci, vp, vp, vp, sz, vp, cu, cu, vp, vp, vp, vp, vp, vp]),
         "p3gpu_shard_chunk_bounds": (sz, [sz, vp, sz]),
+        "p3gpu_p2air_generate_trace_cols_dev": (i32, [vp, ci, ci, vp, sz, sz, sz, vp]),
+        "p3gpu_shard_col_segments": (i32, [u32, vp, sz, vp, sz, vp]),
+        "p3gpu_peer_exchange_dev": (i32, [vp, vp, vp, vp, vp, sz]),
+        "p3gpu_p2air_quotient_sharded_dev": (i32, [vp, ci, ci, vp, vp, cu, cu, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -41,8 +41,15 @@ template <int F> __device__ __forceinline__ void air_internal_layer(u32 (&s)[AIR
 // instruction touches 32 different rows 16 bytes each — partial sectors, and ncu shows the kernel stuck on the store queue
 // (lg_throttle).  Instead every group of n values per permutation goes through a [32][n + 1] tile per warp and is
 // written back with consecutive lanes on consecutive words of a row: whole 64/80-byte row segments per instruction.
-template <int F>
-__global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, size_t n_perms, u32 *trace, const __grid_constant__ AirConsts k) {
+//
+// WINDOW: only columns [col0, col1) of the vectorised trace (rows of vec_len permutations) are stored, as a dense
+// (n_perms / vec_len) x (col1 - col0) matrix — the column block one rank of the sharded prover commits.  Every permutation is
+// still evaluated (its later columns depend on all earlier rounds); only the stores are filtered.
+struct GenWindow { size_t col0, col1; unsigned vec_len; };
+
+template <int F, bool WINDOW>
+__global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, size_t n_perms, u32 *trace, const __grid_constant__ AirConsts k,
+                                                             const GenWindow win) {
     __shared__ u32 tiles[4][32 * 33];
     u32 *tile = tiles[threadIdx.x >> 5];
     const unsigned lane = threadIdx.x & 31u;
@@ -57,7 +64,12 @@ __global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, 
         __syncwarp();
         for (unsigned idx = lane; idx < n_warp * n; idx += 32) {
             const unsigned perm = idx / n, i = idx - perm * n;
-            trace[(p0 + perm) * cols + off + i] = tile[perm * (n + 1) + i];
+            if constexpr (WINDOW) {
+                const size_t pp = p0 + perm, c = (pp % win.vec_len) * cols + off + i;
+                if (c >= win.col0 && c < win.col1) trace[(pp / win.vec_len) * (win.col1 - win.col0) + (c - win.col0)] = tile[perm * (n + 1) + i];
+            } else {
+                trace[(p0 + perm) * cols + off + i] = tile[perm * (n + 1) + i];
+            }
         }
         __syncwarp();
     };
@@ -116,16 +128,30 @@ template <int F> __device__ __forceinline__ void qmac(u64 (&acc)[4], u32 c, cons
     }
 }
 
+// One column segment of a sharded row block: columns [c0, c1) of the trace are a (rows x (c1 - c0)) row-major matrix at element
+// offset `off` of the block.  c0 and c1 are multiples of 4, so a 16-byte load never straddles two segments.
+struct QSeg { u32 c0, c1; u64 off; };
+static_assert(sizeof(QSeg) == 16, "QSeg is one 16-byte shared-memory entry");
+constexpr int QSEG_MAX = 512;
+
 struct QuotArgs {
-    const u32 *lde;      // H x (vec_len * cols), bit-reversed rows
-    u32 *q;              // H x 4, natural order over the quotient domain
+    const u32 *lde;      // H x (vec_len * cols), bit-reversed rows (SHARDED: this rank's row block, laid out by `segs`)
+    u32 *q;              // H x 4, natural order over the quotient domain (SHARDED: rows x 4, the block's bit-reversed slice)
     const u32 *apow;     // (vec_len * n_constraints) EF4: alpha^j
     const u32 *invz;     // 2^rate_bits inverse vanishing values
     unsigned log_h, rate_mask;
     int vec_len;
+    // SHARDED only
+    const QSeg *segs;    // n_segs segments in column order, tiling [0, vec_len * cols)
+    int n_segs;
+    size_t row0, rows;   // the block is memory rows [row0, row0 + rows) of the bit-reversed LDE
 };
 
-template <int F>
+// SHARDED = false: the whole LDE, one thread per (natural index i, permutation v), reads memory row bitrev(i), writes q[i].
+// SHARDED = true: one rank's row block of the row-sharded commit, one thread per (block row m, permutation v); memory row
+// row0 + m is natural index i = bitrev(row0 + m), so it takes 1/Z_H entry i & rate_mask and writes q[m].  The block is read in
+// place through the segment table (the chunk-major layout p3gpu_commit_sharded_dev leaves), never copied into a dense matrix.
+template <int F, bool SHARDED>
 __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, const __grid_constant__ AirConsts k) {
     // alpha powers, one padded row per permutation of the vector: constraint kk of permutation v (global index j = v * nc + kk,
     // multiplied by alpha^(n_all - 1 - j)) sits at ap[v * (nc + 1) + kk].  The row stride of nc + 1 = 149 entries (596 words = 20
@@ -136,25 +162,53 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
         const int j = n_all - 1 - t;
         ap[(j / nc) * (nc + 1) + (j % nc)] = __ldg(reinterpret_cast<const uint4 *>(a.apow) + t);
     }
+    QSeg *sg = reinterpret_cast<QSeg *>(ap + a.vec_len * (nc + 1));   // SHARDED: the segment table behind the alpha powers
+    if constexpr (SHARDED)
+        for (int t = threadIdx.x; t < a.n_segs; t += blockDim.x) sg[t] = a.segs[t];
     __syncthreads();
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int lanes = a.vec_len;                                    // power of two <= 32 (checked by the host)
-    const size_t i = t / lanes;
+    const size_t i = t / lanes;                                     // SHARDED: the block row m
     const int v = (int)(t % lanes);
-    const bool live = i < ((size_t)1 << a.log_h);
+    const bool live = SHARDED ? i < a.rows : i < ((size_t)1 << a.log_h);
     u64 acc[4] = {0, 0, 0, 0};
     if (live) {
         const size_t cols = 144 + (size_t)k.rounds_p;
-        const size_t m = (size_t)(__brevll((unsigned long long)i) >> (64 - a.log_h));
+        const size_t m = SHARDED ? i : (size_t)(__brevll((unsigned long long)i) >> (64 - a.log_h));
         const u32 *c = a.lde + (m * lanes + v) * cols;
         const uint4 *apv = ap + v * (nc + 1);
         // a permutation's 164 columns start 16-byte aligned (656 = 41 x 16 bytes): 16-byte loads throughout
         const uint4 *c4 = reinterpret_cast<const uint4 *>(c);
+        // SHARDED: the permutation's columns are read in order; `c4` walks the current segment, `rem` columns are left in it
+        int si = 0;
+        u32 rem = 0;
+        if constexpr (SHARDED) {
+            const u32 col = (u32)(v * cols);
+            int hi = a.n_segs - 1;
+            while (si < hi) { const int mid = (si + hi) >> 1; if (sg[mid].c1 <= col) si = mid + 1; else hi = mid; }
+            const QSeg s0 = sg[si];
+            c4 = reinterpret_cast<const uint4 *>(a.lde + s0.off + m * (s0.c1 - s0.c0) + (col - s0.c0));
+            rem = s0.c1 - col;
+        }
+        auto ldc = [&]() -> uint4 {                                 // SHARDED: next 4 columns of this permutation
+            if (rem == 0) {
+                const QSeg s1 = sg[++si];
+                c4 = reinterpret_cast<const uint4 *>(a.lde + s1.off + m * (s1.c1 - s1.c0));
+                rem = s1.c1 - s1.c0;
+            }
+            rem -= 4;
+            return __ldg(c4++);
+        };
         u32 s[AIR_W];
         auto ld16 = [&](u32 (&dst)[AIR_W]) {
+            if constexpr (SHARDED) {
 #pragma unroll
-            for (int x = 0; x < 4; x++) { const uint4 v4 = __ldg(c4 + x); dst[4 * x] = v4.x; dst[4 * x + 1] = v4.y; dst[4 * x + 2] = v4.z; dst[4 * x + 3] = v4.w; }
-            c4 += 4;
+                for (int x = 0; x < 4; x++) { const uint4 v4 = ldc(); dst[4 * x] = v4.x; dst[4 * x + 1] = v4.y; dst[4 * x + 2] = v4.z; dst[4 * x + 3] = v4.w; }
+            } else {
+#pragma unroll
+                for (int x = 0; x < 4; x++) { const uint4 v4 = __ldg(c4 + x); dst[4 * x] = v4.x; dst[4 * x + 1] = v4.y; dst[4 * x + 2] = v4.z; dst[4 * x + 3] = v4.w; }
+                c4 += 4;
+            }
         };
         ld16(s);
         mds_light<F, AIR_W>(s);
@@ -173,7 +227,9 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
             const u32 *cp = reinterpret_cast<const u32 *>(c4);
 #pragma unroll 1
             for (int r = 0; r < k.rounds_p; r += 4) {           // rounds_p % 4 == 0 is checked by the host (20 for KoalaBear width 16)
-                const uint4 v4 = __ldg(reinterpret_cast<const uint4 *>(cp + r));
+                uint4 v4;
+                if constexpr (SHARDED) v4 = ldc();
+                else v4 = __ldg(reinterpret_cast<const uint4 *>(cp + r));
                 const u32 pv[4] = {v4.x, v4.y, v4.z, v4.w};
 #pragma unroll
                 for (int t2 = 0; t2 < 4; t2++) {
@@ -183,7 +239,7 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
                     air_internal_layer<F>(s);
                 }
             }
-            c4 = reinterpret_cast<const uint4 *>(cp + k.rounds_p);
+            if constexpr (!SHARDED) c4 = reinterpret_cast<const uint4 *>(cp + k.rounds_p);
         }
 #pragma unroll 1
         for (int r = 0; r < 4; r++) {
@@ -204,7 +260,8 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
 #pragma unroll
         for (int d = 0; d < 4; d++) r[d] = fp_add<F>(r[d], __shfl_xor_sync(0xffffffffu, r[d], off));
     if (live && v == 0) {
-        const u32 z = __ldg(a.invz + (i & a.rate_mask));
+        const size_t nat = SHARDED ? (size_t)(__brevll((unsigned long long)(a.row0 + i)) >> (64 - a.log_h)) : i;
+        const u32 z = __ldg(a.invz + (nat & a.rate_mask));
         reinterpret_cast<uint4 *>(a.q)[i] = make_uint4(mont_mul<F>(r[0], z), mont_mul<F>(r[1], z), mont_mul<F>(r[2], z), mont_mul<F>(r[3], z));
     }
 }
@@ -251,13 +308,58 @@ int32_t air_generate_trace(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_
     const AirConsts *k;
     P3_TRY(air_consts(ctx, field, &k));
     if (n_perms == 0) return P3GPU_OK;
-    p2air_generate_kernel<KOALA_BEAR><<<(unsigned)((n_perms + 127) / 128), 128, 0, ctx->stream>>>(d_inputs, n_perms, d_trace, *k);
+    p2air_generate_kernel<KOALA_BEAR, false><<<(unsigned)((n_perms + 127) / 128), 128, 0, ctx->stream>>>(d_inputs, n_perms, d_trace, *k, GenWindow{});
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
 
-int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q) {
+int32_t air_generate_trace_cols(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_inputs, size_t n_perms, size_t col0, size_t col1, u32 *d_out) {
+    const AirConsts *k;
+    P3_TRY(air_consts(ctx, field, &k));
+    P3_CHECK(vec_len >= 1 && n_perms % (size_t)vec_len == 0, P3GPU_EINVAL, "%zu permutations do not fill rows of %d", n_perms, vec_len);
+    const size_t width = (size_t)vec_len * (144 + (size_t)k->rounds_p);
+    P3_CHECK(col0 <= col1 && col1 <= width, P3GPU_EINVAL, "column window [%zu, %zu) outside the trace width %zu", col0, col1, width);
+    if (n_perms == 0 || col0 == col1) return P3GPU_OK;
+    const GenWindow win{col0, col1, (unsigned)vec_len};
+    p2air_generate_kernel<KOALA_BEAR, true><<<(unsigned)((n_perms + 127) / 128), 128, 0, ctx->stream>>>(d_inputs, n_perms, d_out, *k, win);
+    ctx->launches++;
+    P3_CUDA(cudaGetLastError());
+    return P3GPU_OK;
+}
+
+// The column segments of a row block as p3gpu_commit_sharded_dev leaves it: dense (one segment) with one rank, chunk-major
+// otherwise — for every source rank g and every chunk [b, b') of shard_chunk_bounds(its block width), columns
+// [col_starts[g] + b, col_starts[g] + b') at element offset rows * (col_starts[g] + b).
+int32_t shard_col_segments(unsigned world, const size_t *col_starts, size_t rows, std::vector<size_t> &segs) {
+    P3_CHECK(world >= 1 && world <= 16, P3GPU_EINVAL, "bad world %u", world);
+    P3_CHECK(col_starts[0] == 0, P3GPU_EINVAL, "column blocks must start at 0");
+    for (unsigned g = 0; g < world; g++) P3_CHECK(col_starts[g] <= col_starts[g + 1], P3GPU_EINVAL, "column blocks must be ordered");
+    segs.clear();
+    auto add = [&](size_t c0, size_t c1, size_t off) -> int32_t {
+        P3_CHECK(c0 % 4 == 0 && c1 % 4 == 0, P3GPU_EINVAL,
+                 "column segment [%zu, %zu) does not start and end on a multiple of 4 columns: a 16-byte load would straddle two chunks", c0, c1);
+        P3_CHECK(c1 < (1ull << 32), P3GPU_EINVAL, "trace too wide");
+        segs.insert(segs.end(), {c0, c1, off});
+        return P3GPU_OK;
+    };
+    if (world == 1) {
+        if (col_starts[1] > 0) P3_TRY(add(0, col_starts[1], 0));
+    } else {
+        for (unsigned g = 0; g < world; g++) {
+            const std::vector<size_t> cb = shard_chunk_bounds(col_starts[g + 1] - col_starts[g]);
+            for (size_t c = 0; c + 1 < cb.size(); c++)
+                if (cb[c + 1] > cb[c]) P3_TRY(add(col_starts[g] + cb[c], col_starts[g] + cb[c + 1], rows * (col_starts[g] + cb[c])));
+        }
+    }
+    P3_CHECK(segs.size() / 3 <= (size_t)QSEG_MAX, P3GPU_EUNSUPPORTED, "%zu column segments (at most %d)", segs.size() / 3, QSEG_MAX);
+    return P3GPU_OK;
+}
+
+// alpha powers + 1/Z_H tables into scratch2, then one quotient launch (the whole LDE, or one row block with its segment table)
+template <bool SHARDED>
+static int32_t quotient_launch(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q,
+                               const std::vector<size_t> *segs, size_t row0, size_t rows) {
     constexpr int F = KOALA_BEAR;
     const AirConsts *k;
     P3_TRY(air_consts(ctx, field, &k));
@@ -267,9 +369,16 @@ int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, u
     const int nc = 128 + k->rounds_p, n_all = nc * vec_len;
     const unsigned rate_bits = log_h - log_n;
     const size_t nz = (size_t)1 << rate_bits;
+    const size_t n_segs = SHARDED ? segs->size() / 3 : 0;
+    if constexpr (SHARDED) {
+        const size_t width = (size_t)vec_len * (144 + (size_t)k->rounds_p);
+        P3_CHECK(n_segs > 0 && (*segs)[1 + 3 * (n_segs - 1)] == width, P3GPU_EINVAL, "the column blocks do not cover the trace width %zu", width);
+        P3_CHECK(rows > 0 && row0 + rows <= ((size_t)1 << log_h), P3GPU_EINVAL, "row block [%zu, %zu) outside the LDE height 2^%u", row0, row0 + rows, log_h);
+    }
     void *tab = nullptr;
-    P3_TRY(ctx_scratch2(ctx, (size_t)n_all * 16 + nz * 4, &tab));
+    P3_TRY(ctx_scratch2(ctx, SHARDED ? (size_t)n_all * 16 + 256 * 4 + n_segs * sizeof(QSeg) : (size_t)n_all * 16 + nz * 4, &tab));
     u32 *apow = (u32 *)tab, *invz = apow + (size_t)n_all * 4;
+    QSeg *dsegs = reinterpret_cast<QSeg *>(invz + 256);         // SHARDED: behind the largest 1/Z_H table, 16-byte aligned
     Ef4<F> al; for (int d = 0; d < 4; d++) al.c[d] = alpha[d];
     ef_powers_kernel<F><<<(unsigned)(((n_all + 31) / 32 + 63) / 64), 64, 0, ctx->stream>>>(apow, (size_t)n_all, al);
     // 1 / Z_H on the coset GENERATOR * K (domain.rs:326-360): Z_H(x_i) = g^N * w^(i mod 2^rate_bits) - 1, w of order 2^rate_bits
@@ -280,14 +389,34 @@ int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, u
     P3_CUDA(cudaMemcpyAsync(invz, hz, nz * 4, cudaMemcpyHostToDevice, ctx->stream));
     QuotArgs qa;
     qa.lde = d_lde; qa.q = d_q; qa.apow = apow; qa.invz = invz; qa.log_h = log_h; qa.rate_mask = (unsigned)(nz - 1); qa.vec_len = vec_len;
-    const size_t threads = ((size_t)1 << log_h) * vec_len;
-    const size_t smem = (size_t)vec_len * (nc + 1) * 16;
-    auto kern = p2air_quotient_kernel<F>;
+    qa.segs = nullptr; qa.n_segs = 0; qa.row0 = row0; qa.rows = rows;
+    if constexpr (SHARDED) {
+        std::vector<QSeg> hs(n_segs);
+        for (size_t s = 0; s < n_segs; s++) hs[s] = QSeg{(u32)(*segs)[3 * s], (u32)(*segs)[3 * s + 1], (u64)(*segs)[3 * s + 2]};
+        P3_CUDA(cudaMemcpyAsync(dsegs, hs.data(), n_segs * sizeof(QSeg), cudaMemcpyHostToDevice, ctx->stream));
+        qa.segs = dsegs; qa.n_segs = (int)n_segs;
+    }
+    const size_t threads = (SHARDED ? rows : (size_t)1 << log_h) * vec_len;
+    const size_t smem = (size_t)vec_len * (nc + 1) * 16 + n_segs * sizeof(QSeg);
+    auto kern = p2air_quotient_kernel<F, SHARDED>;
     if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<(unsigned)((threads + 127) / 128), 128, smem, ctx->stream>>>(qa, *k);
     ctx->launches += 2;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
+}
+
+int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q) {
+    return quotient_launch<false>(ctx, field, vec_len, d_lde, log_h, log_n, alpha, d_q, nullptr, 0, 0);
+}
+
+int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned world, unsigned rank, const u32 *d_block, const size_t *col_starts,
+                             unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q) {
+    const size_t H = (size_t)1 << log_h, rows = H / world;
+    P3_CHECK(world >= 1 && rank < world && rows * world == H, P3GPU_EINVAL, "LDE height 2^%u does not split over %u ranks", log_h, world);
+    std::vector<size_t> segs;
+    P3_TRY(shard_col_segments(world, col_starts, rows, segs));
+    return quotient_launch<true>(ctx, field, vec_len, d_block, log_h, log_n, alpha, d_q, &segs, (size_t)rank * rows, rows);
 }
 
 }  // namespace p3

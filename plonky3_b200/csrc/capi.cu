@@ -490,6 +490,12 @@ int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, cons
     P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
     return air_quotient(ctx, field, vector_len, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
 }
+int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms, size_t col0,
+                                            size_t col1, uint32_t *d_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && (d_out || col0 == col1), P3GPU_EINVAL, "null argument");
+    return air_generate_trace_cols(ctx, field, vector_len, d_inputs, n_perms, col0, col1, d_out);
+}
 
 // ---- transcript + query phase (prove driver) ---------------------------------------------------------
 int32_t p3gpu_challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out) {
@@ -611,6 +617,39 @@ size_t p3gpu_shard_chunk_bounds(size_t w_local, size_t *bounds, size_t max_bound
     const std::vector<size_t> cb = shard_chunk_bounds(w_local);
     for (size_t i = 0; i < cb.size() && i < max_bounds; i++) bounds[i] = cb[i];
     return cb.size();
+}
+
+int32_t p3gpu_shard_col_segments(uint32_t world, const size_t *col_starts, size_t rows, size_t *segs, size_t max_segs, size_t *n_segs) {
+    P3_CHECK(col_starts && n_segs && (segs || max_segs == 0), P3GPU_EINVAL, "null argument");
+    std::vector<size_t> s;
+    P3_TRY(shard_col_segments(world, col_starts, rows, s));
+    *n_segs = s.size() / 3;
+    P3_CHECK(*n_segs <= max_segs, P3GPU_EINVAL, "%zu column segments, room for %zu", *n_segs, max_segs);
+    for (size_t i = 0; i < s.size(); i++) segs[i] = s[i];
+    return P3GPU_OK;
+}
+
+int32_t p3gpu_peer_exchange_dev(p3gpu_ctx *ctx, const p3gpu_peer_group *grp, uint32_t *epoch, void *const *bufs, const uint32_t *d_src, size_t words) {
+    P3_ENTER(ctx);
+    P3_TRY(check_group(grp, false));
+    P3_CHECK(epoch && bufs && (d_src || words == 0), P3GPU_EINVAL, "null argument");
+    for (uint32_t q = 0; q < grp->world; q++) P3_CHECK(bufs[q] != nullptr, P3GPU_EINVAL, "null exchange buffer of rank %u", q);
+    const double tmo = grp->timeout_s > 0 ? grp->timeout_s : 20.0;
+    // nobody overwrites a slot before every rank has finished reading the previous exchange out of its buffer
+    P3_TRY(peer_barrier(ctx, grp->world, grp->rank, grp->ctrl, ++*epoch, tmo));
+    if (words)
+        for (uint32_t q = 0; q < grp->world; q++)     // copy-engine peer copies, stream-ordered before the closing barrier
+            P3_CUDA(cudaMemcpyAsync((u32 *)bufs[q] + (size_t)grp->rank * words, d_src, words * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    return peer_barrier(ctx, grp->world, grp->rank, grp->ctrl, ++*epoch, tmo);
+}
+
+int32_t p3gpu_p2air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                         unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient_slice) {
+    P3_ENTER(ctx);
+    P3_TRY(check_group(grp, true));
+    P3_CHECK(col_starts && alpha && d_quotient_slice, P3GPU_EINVAL, "null argument");
+    return air_quotient_sharded(ctx, field, vector_len, grp->world, grp->rank, grp->rows[grp->rank], col_starts, log_lde_height, log_trace_height,
+                                alpha, d_quotient_slice);
 }
 
 // TwoAdicFriPcs::commit of ONE trace whose columns are sharded over the ranks, bit-identical to the single-GPU commitment.

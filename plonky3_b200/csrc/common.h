@@ -148,6 +148,10 @@ int32_t peer_allgather(p3gpu_ctx *ctx, unsigned world, unsigned rank, void *cons
 int32_t air_set_constants(p3gpu_ctx *ctx, int field, const u32 *beg, const u32 *part, int rounds_p, const u32 *end);
 int32_t air_generate_trace(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_perms, u32 *d_trace);
 int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q);
+int32_t air_generate_trace_cols(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_inputs, size_t n_perms, size_t col0, size_t col1, u32 *d_out);
+int32_t shard_col_segments(unsigned world, const size_t *col_starts, size_t rows, std::vector<size_t> &segs);   // (c0, c1, offset) triples
+int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned world, unsigned rank, const u32 *d_block, const size_t *col_starts,
+                             unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q);
 
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);

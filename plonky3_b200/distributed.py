@@ -165,6 +165,8 @@ class PeerGroup:
         self.gpu, self.rows_per_rank, self.w_total = gpu, int(rows_per_rank), int(w_total)
         self.epoch = C.c_uint32(0)
         self._imported = []
+        self.group, self._simulated = group, _sim is not None
+        self.xchg, self.xchg_ptrs, self._xchg_imported = None, None, []
         if _sim is not None:                       # single-process simulation (tests): all blocks live on this device
             self.world, self.rank, self.ctrl, self.rows, peers = _sim
         else:
@@ -279,7 +281,289 @@ class PeerGroup:
                     out[:, c0:c0 + (b - a)] = flat[R * c0: R * (c0 + b - a)].reshape(R, b - a)
         return out
 
+    def column_segments(self, col_starts=None):
+        """[(first column, end column, element offset)] of my row block as the last commit left it (p3gpu_shard_col_segments)."""
+        return column_segments(self.world, col_starts if col_starts is not None else self.col_starts, self.rows_per_rank)
+
+    def ensure_exchange(self, nbytes: int):
+        """Collective: every rank's exchange buffer holds at least `nbytes`, mapped on every rank through CUDA IPC.  A smaller
+        buffer from an earlier call is closed and replaced; every rank must call this with the same size."""
+        if self.xchg is not None and self.xchg.nbytes >= nbytes:
+            return
+        if self._simulated:
+            raise NotImplementedError("exchange buffers need one process per rank")
+        self._close_exchange()
+        self.xchg = RawBuffer(self.gpu, nbytes)
+        ptrs = [self.xchg.ptr] * self.world
+        if self.world > 1:
+            h = (C.c_uint8 * 64)()
+            check(self.gpu.L.p3gpu_ipc_export(self.gpu.h, C.c_void_p(self.xchg.ptr), h))
+            handles = [None] * self.world
+            dist.all_gather_object(handles, bytes(h), group=self.group)
+            for q, b in enumerate(handles):
+                if q != self.rank:
+                    p = C.c_void_p()
+                    check(self.gpu.L.p3gpu_ipc_import(self.gpu.h, (C.c_uint8 * 64).from_buffer_copy(b), C.byref(p)))
+                    self._xchg_imported.append(p.value)
+                    ptrs[q] = p.value
+        self.xchg_ptrs = (C.c_void_p * 16)(*ptrs)
+
+    def exchange(self, src):
+        """p3gpu_peer_exchange_dev: all-gather of `src` (contiguous CUDA int32) over the exchange buffers.  Returns a
+        (world, src.numel()) view of MY exchange buffer, valid until the next exchange."""
+        s = self.gpu._dev(src)
+        words = int(s.numel())
+        assert self.xchg is not None and self.world * words * 4 <= self.xchg.nbytes, "exchange buffer too small (ensure_exchange)"
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_peer_exchange_dev(self.gpu.h, C.byref(self.struct), C.byref(self.epoch), self.xchg_ptrs, s.data_ptr(), words))
+        return self.xchg.tensor((self.world, words))
+
+    def p2air_quotient(self, field, vector_len: int, log_lde_height: int, log_trace_height: int, alpha):
+        """p3gpu_p2air_quotient_sharded_dev on my row block: (rows_per_rank, 4) quotient values, bit-reversed slice `rank`."""
+        gpu = self.gpu
+        gpu._use_torch_stream()
+        cs = (C.c_size_t * (self.world + 1))(*self.col_starts)
+        q = gpu._empty((self.rows_per_rank, 4))
+        check(gpu.L.p3gpu_p2air_quotient_sharded_dev(gpu.h, field.id, vector_len, C.byref(self.struct), cs, log_lde_height, log_trace_height,
+                                                     gpu._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
+
+    def _close_exchange(self):
+        if self.xchg is None:
+            return
+        if self.world > 1 and not self._simulated:
+            dist.barrier(group=self.group)         # no peer still copies into the buffer being freed
+        for p in self._xchg_imported:
+            self.gpu.L.p3gpu_ipc_close(self.gpu.h, C.c_void_p(p))
+        self._xchg_imported = []
+        self.xchg.free()
+        self.xchg, self.xchg_ptrs = None, None
+
     def close(self):
+        self._close_exchange()
         for p in self._imported:
             self.gpu.L.p3gpu_ipc_close(self.gpu.h, C.c_void_p(p))
         self._imported = []
+
+
+def column_segments(world: int, col_starts, rows: int):
+    """p3gpu_shard_col_segments: the (first column, end column, element offset) segments of a row block of `rows` rows after
+    p3gpu_commit_sharded_dev with these column blocks.  Raises P3GpuError for a layout whose segment bounds are not multiples
+    of 4 columns."""
+    L = _lib.load()
+    starts = (C.c_size_t * (world + 1))(*[int(x) for x in col_starts])
+    cap = 3 * (int(col_starts[-1]) // 4 + world + 2)
+    buf = (C.c_size_t * cap)(); n = C.c_size_t()
+    check(L.p3gpu_shard_col_segments(world, starts, rows, buf, cap // 3, C.byref(n)))
+    return [(int(buf[3 * k]), int(buf[3 * k + 1]), int(buf[3 * k + 2])) for k in range(n.value)]
+
+
+def query_owner(index: int, rows_per_rank: int):
+    """(rank, local row) holding row `index` of the bit-reversed LDE after the row-sharded commit."""
+    return index // rows_per_rank, index % rows_per_rank
+
+
+def quotient_slice_natural_indices(rank: int, rows_per_rank: int, log_height: int):
+    """Natural quotient-domain index of every entry of rank `rank`'s sharded quotient slice: bitrev(rank * R + m)."""
+    m = np.arange(rank * rows_per_rank, (rank + 1) * rows_per_rank, dtype=np.int64)
+    return _bitrev(m, log_height)
+
+
+def _bitrev(x, bits: int):
+    """Bit reversal of `bits`-bit indices: numpy int64 arrays or CUDA int64 tensors."""
+    r = x * 0
+    for b in range(bits):
+        r = r | (((x >> b) & 1) << (bits - 1 - b))
+    return r
+
+
+class _ShardedTraceMmcs:
+    """The trace batch's Mmcs::open_multi_batch when its rows are spread over the ranks: every rank gathers the rows and
+    authentication paths of the queries it owns (rank idx // R, local row idx % R), the tables are all-gathered over peer
+    memory, and every rank takes each answer from its owner's slot.  The path's levels inside a sub-tree come from the owner's
+    sub-tree; the levels above it (cap_height < log2(world)) from the tree over the sub-tree roots that the commit left in the
+    control block."""
+
+    def __init__(self, grp: "PeerGroup", sub_layers, top_layers, log_height: int, cap_height: int):
+        self.grp, self.sub_layers, self.top_layers = grp, sub_layers, top_layers
+        self.log_height, self.height = log_height, 1 << log_height
+        self.path_len = log_height - min(cap_height, log_height)
+
+    def get_max_height(self, _data):
+        return self.height
+
+    def open_multi_batch(self, indices, _data):
+        grp, gpu = self.grp, self.grp.gpu
+        R, W, rank = grp.rows_per_rank, grp.w_total, grp.rank
+        log_r = R.bit_length() - 1
+        idx = np.asarray(indices, dtype=np.int64)
+        n, plen = int(idx.size), self.path_len
+        sub_len = min(log_r, plen)
+        owner, local = idx // R, idx % R
+        mine = np.nonzero(owner == rank)[0]
+        rec = W + plen * 8
+        table = torch.zeros((n, rec), dtype=torch.int32, device=f"cuda:{gpu.device}")
+        if mine.size:
+            li = np.ascontiguousarray(local[mine], dtype=np.uint32)
+            mine = torch.from_numpy(mine).to(table.device)
+            k = int(li.size)
+            flat = grp.rows_tensor().reshape(-1)
+            gpu._use_torch_stream()
+            for c0, c1, off in grp.column_segments():
+                piece = gpu._empty((k, c1 - c0))
+                check(gpu.L.p3gpu_gather_rows_dev(gpu.h, flat[off:].data_ptr(), R, c1 - c0, li.ctypes.data, k, 0, piece.data_ptr()))
+                table[mine, c0:c1] = piece
+            if sub_len:
+                lay = self.sub_layers
+                lens = (C.c_size_t * len(lay))(*[int(l.shape[0]) for l in lay])
+                paths = gpu._empty((k, sub_len, 8))
+                check(gpu.L.p3gpu_merkle_paths_dev(gpu.h, lay[0].data_ptr(), lens, len(lay), sub_len, li.ctypes.data, k, 0, paths.data_ptr()))
+                table[mine, W:W + sub_len * 8] = paths.reshape(k, -1)
+            for lvl in range(plen - sub_len):          # levels above the sub-tree roots: the same siblings for all my queries
+                sib = self.top_layers[lvl][(rank >> lvl) ^ 1]
+                table[mine, W + (sub_len + lvl) * 8: W + (sub_len + lvl + 1) * 8] = torch.from_numpy(sib.view(np.int32)).to(table.device)
+        got = grp.exchange(table.reshape(-1)).reshape(grp.world, n, rec)
+        ans = got[torch.from_numpy(owner).to(table.device), torch.arange(n, device=table.device)].cpu().numpy().view(np.uint32)
+        return [np.ascontiguousarray(ans[:, :W])], np.ascontiguousarray(ans[:, W:]).reshape(n, plen, 8)
+
+
+def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
+    """uni_stark.prove of the Poseidon2 AIR with the trace sharded by column block over the ranks of `grp` (rank g holds columns
+    [col_starts[g], col_starts[g+1]) of the 2^n-row trace).  Every rank returns the same Proof, byte for byte the one
+    `uni_stark.prove` writes for the whole trace on one GPU.
+
+    Each rank runs its own device challenger; ranks exchange data (over peer memory, no collective library) only where a
+    value depends on rows they do not own, and after every exchange all ranks hold identical bytes, so the transcripts stay
+    identical.  trace commit: PeerGroup.commit (rank g keeps LDE rows [g R, (g+1) R), R = 2N / world); quotient: evaluated
+    on the own row block in place, slices all-gathered, committed redundantly; opened values at zeta: partial column-wise dots
+    over the first coset's rows, all-gathered and summed; reduced openings of the trace: over the own rows, all-gathered;
+    FRI: redundantly on every rank; trace query openings: answered by the owner rank and all-gathered."""
+    import time
+    from . import extension as X
+    from .dft import _log2_strict
+    from .uni_stark import Proof, get_log_num_quotient_chunks, prove_fri
+    pcs, mmcs = config.pcs, config.pcs.mmcs
+    f, gpu = pcs.dft.field, grp.gpu
+    assert gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
+    assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
+    starts = [int(x) for x in col_starts]
+    world, rank, R, W = grp.world, grp.rank, grp.rows_per_rank, grp.w_total
+    assert starts[-1] == W == air.width(), "column blocks must cover the AIR's width"
+    degree = int(trace_block.shape[0])
+    log_degree = _log2_strict(degree)
+    log_blowup = pcs.fri.log_blowup
+    log_num_quotient_chunks = get_log_num_quotient_chunks(air)
+    num_quotient_chunks = 1 << log_num_quotient_chunks
+    assert log_num_quotient_chunks == log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
+    H, log_h = degree << log_blowup, log_degree + log_blowup
+    assert R * world == H
+    dev = f"cuda:{gpu.device}"
+    sync = torch.cuda.synchronize
+    T = {}
+
+    def span(name, t0):
+        sync(); T[name] = (time.perf_counter() - t0) * 1e3
+
+    for p in mmcs.perms:
+        p.upload(gpu)
+    nq = pcs.fri.num_queries
+    grp.ensure_exchange(4 * max(H * 4, world * W * 4, world * nq * (W + 8 * log_h)))
+    challenger = config.initialise_challenger()
+    trace_domain = pcs.natural_domain_for_degree(degree)
+
+    t0 = time.perf_counter()
+    trace_commit, sub_layers, _ = grp.commit(f, mmcs.hash_kind, trace_block, starts, log_blowup, mmcs.cap_height)
+    span("commit to trace data", t0)
+    log_g = world.bit_length() - 1
+    top_layers = []
+    if mmcs.cap_height < log_g:                      # the tree over the sub-tree roots, as the commit left it in the control block
+        user = grp.ctrl.tensor((_lib.PEER_CTRL_BYTES // 4,))[_lib.PEER_CTRL_USER // 4:].cpu().numpy().view(np.uint32)
+        off = world * 8
+        for lvl in range(log_g):
+            n = world >> lvl
+            top_layers.append(user[off:off + n * 8].reshape(n, 8).copy()); off += n * 8
+
+    challenger.observe_canonical(log_degree)
+    challenger.observe_canonical(log_degree)
+    challenger.observe_canonical(0)
+    challenger.observe_cap(trace_commit)
+    alpha = challenger.sample_algebra_element()
+
+    t0 = time.perf_counter()
+    quotient_domain = (f.mul(trace_domain[0], f.generator), log_h)
+    q_slice = grp.p2air_quotient(f, air.vector_len, log_h, log_degree, alpha)
+    q_bitrev = grp.exchange(q_slice).reshape(H, 4)
+    perm = _bitrev(torch.arange(H, device=dev, dtype=torch.int64), log_h)
+    quotient_flat = q_bitrev[perm].contiguous()      # natural order
+    span("compute quotient polynomial", t0)
+
+    t0 = time.perf_counter()
+    quotient_commit, quotient_data = pcs.commit_quotient(quotient_domain, quotient_flat, num_quotient_chunks)
+    span("commit to quotient poly chunks", t0)
+    challenger.observe_cap(quotient_commit)
+    zeta = challenger.sample_algebra_element()
+
+    t0 = time.perf_counter()
+    z = np.asarray([int(v) for v in zeta], dtype=np.uint32)
+    inv_denoms, adjusted = gpu.open_inv_denoms(f.id, log_h, z, X.ef_inv(f, z))
+    g_pow_n = f.pow(f.generator, degree)
+    denom_inv = f.inv(f.mul(g_pow_n, f.to_monty(degree)))
+    scal = X.ef_scale(f, X.ef_mul(f, z, X.ef_sub(f, X.ef_pow(f, z, degree), X.ef_from_base(f, g_pow_n))), denom_inv)
+    one = X.ef_one(f)
+    flat = grp.rows_tensor().reshape(-1)
+    segs = grp.column_segments()
+    chunk = lambda c0, c1, off: flat[off:off + R * (c1 - c0)].reshape(R, c1 - c0)
+    row0 = rank * R
+    # trace values at zeta: barycentric sum over the first coset's rows (memory rows [0, N)), split by owner
+    partial = torch.zeros((W, 4), dtype=torch.int32, device=dev)
+    used = min(R, degree - row0)
+    if used > 0:
+        for c0, c1, off in segs:
+            partial[c0:c1] = gpu.columnwise_dot(f.id, chunk(c0, c1, off)[:used], adjusted[row0:row0 + used])
+    parts = grp.exchange(partial.reshape(-1)).reshape(world, W, 4)
+    acc = torch.zeros((W, 4), dtype=torch.int32, device=dev)
+    for q in range(world):
+        gpu.ef_axpy(f.id, acc, parts[q], one)
+    trace_ys = torch.zeros((W, 4), dtype=torch.int32, device=dev)
+    gpu.ef_axpy(f.id, trace_ys, acc, scal)
+    challenger.observe_algebra_slice(trace_ys)
+    q_mats = mmcs.get_matrices(quotient_data)
+    q_ys = []
+    for m in q_mats:
+        ys = gpu.columnwise_dot(f.id, m[:int(m.shape[0]) >> log_blowup], adjusted, scal)
+        challenger.observe_algebra_slice(ys)
+        q_ys.append(ys)
+    alpha2 = np.asarray(challenger.sample_algebra_element(), dtype=np.uint32)
+
+    def yred_of(ys):
+        return X.ef_from_basis_rows(f, gpu.rowwise_dot(f.id, ys.t().contiguous(), alpha2).cpu().numpy().view(np.uint32))
+    # reduced openings: the trace's term over my rows (row-wise dot per column segment, shifted by alpha^(first column)) ...
+    r_local = torch.zeros((R, 4), dtype=torch.int32, device=dev)
+    for c0, c1, off in segs:
+        gpu.ef_axpy(f.id, r_local, gpu.rowwise_dot(f.id, chunk(c0, c1, off), alpha2), X.ef_pow(f, alpha2, c0))
+    red_local = torch.zeros((R, 4), dtype=torch.int32, device=dev)
+    gpu.open_reduce(f.id, red_local, r_local, inv_denoms[row0:row0 + R], X.ef_pow(f, alpha2, 0), yred_of(trace_ys))
+    reduced = grp.exchange(red_local).reshape(H, 4).clone()
+    # ... and the quotient chunks' terms, locally on the full height
+    num_reduced = W
+    for m, ys in zip(q_mats, q_ys):
+        gpu.open_reduce(f.id, reduced, gpu.rowwise_dot(f.id, m, alpha2), inv_denoms, X.ef_pow(f, alpha2, num_reduced), yred_of(ys))
+        num_reduced += int(m.shape[1])
+    span("open: evaluate + reduce", t0)
+
+    t0 = time.perf_counter()
+    trace_view = _ShardedTraceMmcs(grp, sub_layers, top_layers, log_h, mmcs.cap_height)
+    rounds = [(None, [[zeta]]), (quotient_data, [[zeta]] * num_quotient_chunks)]
+    fri = prove_fri(pcs, [reduced], challenger, rounds, input_mmcs=[trace_view, mmcs])
+    span("open: FRI", t0)
+
+    if world > 1 and dist.is_initialized():
+        every = [None] * world
+        dist.all_gather_object(every, T, group=grp.group)
+        T = {k: max(t[k] for t in every) for k in T}
+    return Proof(trace_commit=trace_commit, quotient_commit=quotient_commit, trace_local=trace_ys.cpu().numpy().view(np.uint32),
+                 quotient_chunks=[ys.cpu().numpy().view(np.uint32) for ys in q_ys], commit_phase_commits=fri["commits"],
+                 commit_pow_witnesses=fri["pow_witnesses"], final_poly=fri["final_poly"], query_pow_witness=fri["query_pow_witness"],
+                 query_indices=fri["indices"], input_openings=fri["input_openings"], commit_phase_openings=fri["commit_phase_openings"],
+                 degree_bits=log_degree, timings_ms=T, input_opening_indices=fri["input_opening_indices"],
+                 commit_phase_indices=fri["commit_phase_indices"])

@@ -278,6 +278,14 @@ class Gpu:
         check(self.L.p3gpu_p2air_generate_trace_dev(self.h, field, x.data_ptr(), n, out.data_ptr()))
         return out
 
+    def p2air_generate_trace_cols(self, field, inputs_dev, col0, col1, vector_len=8):
+        """Columns [col0, col1) of `p2air_generate_trace`'s output: (n_perms / vector_len, col1 - col0)."""
+        x = self._dev(inputs_dev); self._use_torch_stream()
+        n = int(x.shape[0])
+        out = self._empty((n // vector_len, col1 - col0))
+        check(self.L.p3gpu_p2air_generate_trace_cols_dev(self.h, field, vector_len, x.data_ptr(), n, col0, col1, out.data_ptr()))
+        return out
+
     def p2air_quotient(self, field, lde_dev, log_trace_height, alpha, vector_len=8):
         """quotient values (H, 4) in natural order over GENERATOR * K, |K| = H = LDE height."""
         m = self._dev(lde_dev); self._use_torch_stream()

@@ -121,6 +121,14 @@ class VectorizedPoseidon2Air:
         self._upload()
         return self.gpu.p2air_generate_trace(self.field.id, inputs_dev, self.vector_len)
 
+    def generate_trace_cols(self, inputs_dev, col0: int, col1: int):
+        """Columns [col0, col1) of `generate_trace_rows(inputs_dev)` without building the full trace: one rank's column block
+        for `distributed.prove_sharded`."""
+        if self.gpu is None:
+            raise _lib.P3GpuError("trace generation needs a GPU context (no CPU fallback)")
+        self._upload()
+        return self.gpu.p2air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1), self.vector_len)
+
     def quotient_values(self, trace_lde_dev, log_degree: int, alpha):
         """uni-stark/src/prover.rs:462-827 on the committed LDE (natural order over the quotient domain)."""
         if self.gpu is None:
@@ -236,8 +244,10 @@ def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values
                  commit_phase_indices=fri["commit_phase_indices"])
 
 
-def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list) -> dict:
-    """fri/src/prover.rs:43-160."""
+def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list,
+              input_mmcs: Optional[list] = None) -> dict:
+    """fri/src/prover.rs:43-160.  `input_mmcs[k]` (default pcs.mmcs) opens input batch k: anything with get_max_height(data) and
+    open_multi_batch(indices, data), such as the row-sharded trace of distributed.prove_sharded."""
     import torch
     params: FriParameters = pcs.fri
     f, gpu = pcs.dft.field, pcs.dft.gpu
@@ -256,10 +266,11 @@ def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, pr
     t0 = time.perf_counter()
     # open_inputs (:380-417): every committed batch at the (height-reduced) query indices
     input_openings, input_opening_indices, commit_phase_indices = [], [], []
-    for data, _ in prover_data_with_opening_points:
-        log_max_height = _log2_strict(pcs.mmcs.get_max_height(data))
+    openers = input_mmcs or [pcs.mmcs] * len(prover_data_with_opening_points)
+    for (data, _), mmcs in zip(prover_data_with_opening_points, openers):
+        log_max_height = _log2_strict(mmcs.get_max_height(data))
         reduced = [i >> (log_global_max_height - log_max_height) for i in indices]
-        input_openings.append(pcs.mmcs.open_multi_batch(reduced, data))
+        input_openings.append(mmcs.open_multi_batch(reduced, data))
         input_opening_indices.append(reduced)
     # answer_queries (:308-378)
     commit_phase_openings, cur = [], list(indices)

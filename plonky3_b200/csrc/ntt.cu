@@ -30,6 +30,8 @@
 // With two equal passes on the cp.async kernel (2^20 rows by default) the LDE is three launches: inverse pass 1, ONE fused
 // pass (ntt_lde_mid_kernel: inverse pass 2 and every coset's forward pass 1, tile by tile through shared memory and registers)
 // and forward pass 2, so the coefficients are written and read once.  Every other LDE runs the four passes as separate launches.
+// The fused pass runs warp-specialised where its registers allow (all instances but the runtime-width one at r = 10): a producer
+// lane loads each tile with one tensor copy and owns the tile stores and their read-out waits (DESIGN 4.1).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -284,6 +286,54 @@ __device__ __forceinline__ void tma_store_tile(const CUtensorMap *map, const voi
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// mbarriers and bulk loads (the producer-warp form of ntt_lde_mid_kernel, and ntt_pass_pipe_kernel)
+__device__ __forceinline__ void mbar_init(u32 bar, u32 count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
+__device__ __forceinline__ void mbar_wait(u32 bar, u32 parity) {
+    u32 done = 0, spins = 0;
+    unsigned long long t0 = 0;
+    while (true) {
+        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+        if (done) break;
+        // watchdog: a pass takes milliseconds; a wait of 20 s can only be a protocol error.  Trap (the launch fails with an error the
+        // host reports) instead of leaving a hung kernel on the device.
+        if ((++spins & 0xfffu) == 0) {
+            unsigned long long now;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+            if (t0 == 0) t0 = now;
+            else if (now - t0 > 20000000000ull) __trap();
+        }
+    }
+}
+// The same wait without a watchdog, for a barrier that only a thread whose own waits have one arrives on (it then cannot hang
+// unless that thread traps): no registers beyond its operands, for waits at a kernel's register cap.
+__device__ __forceinline__ void mbar_wait_plain(u32 bar, u32 parity) {
+    asm volatile("{ .reg .pred p; WAIT_%=: mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1; @!p bra WAIT_%=; }" ::"r"(bar), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(u32 bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_arrive_n(u32 bar, u32 n) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(u32 bar, u32 bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
+__device__ __forceinline__ void bulk_load(void *smem, const void *gmem, u32 bytes, u32 bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"((u32)__cvta_generic_to_shared(smem)), "l"(gmem), "r"(bytes), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tma_load_tile(const CUtensorMap *map, void *smem, int c0, int c3, int c4, u32 bar) {
+    asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
+                 ::"r"((u32)__cvta_generic_to_shared(smem)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(0), "r"(0), "r"(c3), "r"(c4),
+                   "r"(bar) : "memory");
+}
+// a tile's twiddles tws[2^lam + q] = Z[2^(l0+lam) + T*2^lam + q], 1 <= lam < r: one bulk copy per layer on `bar`, 8 * (2^r - 2)
+// bytes.  Layer 0's single 8-byte entry tws[1] = Z[2^l0 + T] is too small for a bulk copy: the producer writes it itself, before
+// its arrive on bar.
+__device__ __forceinline__ void load_tile_twiddles(uint2 *tws, const uint2 *tw, int l0, u32 T, int r, u32 bar) {
+#pragma unroll 1
+    for (int lam = 1; lam < r; lam++) bulk_load(tws + (1u << lam), tw + ((size_t)1 << (l0 + lam)) + ((size_t)T << lam), 8u << lam, bar);
+}
+// Consumer-only barrier of a producer-warp kernel (the producer warp never joins it); the plain kernels use __syncthreads.
+template <bool PROD, u32 THREADS> __device__ __forceinline__ void consumer_sync() {
+    if constexpr (PROD) asm volatile("bar.sync 1, %0;" ::"n"(THREADS) : "memory");
+    else __syncthreads();
+}
+
 // Persistent, double-buffered pass kernel.  A CTA (one per SM) walks over tiles of 2^R_LOG rows x `ct` columns:
 //   * tile k+1 (rows as 16-byte cp.async/LDGSTS copies, plus its 2^R_LOG - 1 twiddles) streams into the second shared
 //     buffer while tile k is computed, so HBM latency overlaps the integer work;
@@ -501,11 +551,19 @@ ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
 //     output rows (runs of ~26 rows per 2^r-row group at 132 SMs) instead of rows 2^r / 32 apart, while each tile's
 //     reads stay one contiguous block of 2^r rows.
 // THREADS = E1 * CT_T (E1 * 12 for the runtime-width variant) gives every forward step-1 item (E1*cw of them) its own thread.
+// PROD (producer-warp form, every instance whose registers allow it: lde_mid_producer): one more warp, lane 0 of which loads the
+// tile (ONE tensor copy, imap over the coefficients in the inverse layout; the zero-filled pad row per group is the shared layout)
+// and its inverse twiddles (one bulk copy per layer) on full[b], stages the forward twiddles with the first tile, and owns the
+// stores: the consumers write a coset's forward step 2 back, fence and arrive on ready[b]; the producer stores the tile, waits
+// until the copy has read the buffer out (the thread that commits a bulk group is the one that can wait for it) and arrives on
+// `freed`, which the consumers wait on before the next coset's forward step 1 rewrites the buffer.  After a tile's last coset
+// the producer refills the buffer with tile k + 2 instead: the consumers' only other wait is full[b].
 template <int R_LOG, int CT_T> __host__ __device__ constexpr int lde_mid_threads() { return (1 << (R_LOG / 2)) * (CT_T ? CT_T : 12); }
 
-template <int F, int R_LOG, int CT_T>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
-__global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>(), 1)
-ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, const __grid_constant__ CUtensorMap omap) {
+template <int F, int R_LOG, int CT_T, bool PROD>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
+__global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>() + (PROD ? 32 : 0), 1)
+ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, const __grid_constant__ CUtensorMap omap,
+                   const __grid_constant__ CUtensorMap imap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     constexpr u32 E1 = 1u << Q1, E2 = 1u << Q2, R = 1u << R_LOG;
     constexpr u32 THREADS = lde_mid_threads<R_LOG, CT_T>();
@@ -517,6 +575,11 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
     u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
     uint2 *twi0 = reinterpret_cast<uint2 *>(data0 + 2 * buf_words);    // the tile's inverse twiddles, double-buffered
     uint2 *twf = twi0 + 2 * R;                                          // forward twiddles, R per coset
+    // PROD: mbarriers full[b] (producer arrive + transaction bytes), ready[b] (every consumer thread, per coset), freed (producer)
+    const u32 bar0 = (u32)__cvta_generic_to_shared(twf + a.n_cosets * R);
+    auto full_bar = [&](u32 b) { return bar0 + 8u * b; };
+    auto ready_bar = [&](u32 b) { return bar0 + 16u + 8u * b; };
+    const u32 freed_bar = bar0 + 32u;
 
     const u32 total = (1u << (a.log_n - R_LOG)) * a.n_ctiles;
     auto issue = [&](u32 t, u32 buf) {
@@ -542,20 +605,98 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
 
     u32 t = blockIdx.x;
     if (t >= total) return;
-    for (u32 k = threadIdx.x; k < a.n_cosets * R; k += THREADS)   // heap entries 1..R-1 of every coset (entry 0 is unused)
-        if (k & (R - 1u)) cp_async8(twf + k, tw_fwd + (size_t)(k >> R_LOG) * a.tw_stride + (k & (R - 1u)));
-    issue(t, 0);   // the forward twiddles land with the first tile's group
+#ifdef P3GPU_NTT_PROFILE
+    // PROD: the producer stamps slot 2 (load issue) and slot 6 (its wait for the tile's stores to be read out, summed over cosets)
+#define P3_PSTAMP(kk, slot, v) do { if (a.prof && (kk) < 16) a.prof[((size_t)blockIdx.x * 16 + (kk)) * 8 + (slot)] = (v); } while (0)
+#else
+#define P3_PSTAMP(kk, slot, v) do { } while (0)
+#endif
+    if constexpr (PROD) {
+        if (threadIdx.x == 0) {
+            for (u32 b = 0; b < 2; b++) { mbar_init(full_bar(b), 1); mbar_init(ready_bar(b), THREADS); }
+            mbar_init(freed_bar, 1);
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        }
+        __syncthreads();
+        if (threadIdx.x >= THREADS) {
+            // ---------------- producer ----------------
+            if (threadIdx.x != THREADS) return;
+            const u32 n_mine = (total - blockIdx.x + gridDim.x - 1) / gridDim.x;   // tiles of this CTA
+            auto load = [&](u32 k) {
+                const u32 b = k & 1u, tt = blockIdx.x + k * gridDim.x;
+                const u32 col = (tt % a.n_ctiles) * CT, T = __brev(tt / a.n_ctiles) >> (32 - R_LOG);
+                uint2 *tws = twi0 + b * R;
+                tws[1] = a.tw[((size_t)1 << R_LOG) + T];
+                // the box counts its zero-filled pad rows: E1 groups of gs1 = (E2 + 1) * CT words; the first tile brings the forward
+                // twiddles of every coset (whole heaps of R entries: entry 0 is unused, but keeps the copy a multiple of 16 bytes)
+                mbar_expect_tx(full_bar(b), E1 * gs1 * 4u + 8u * (R - 2u) + (k == 0 ? a.n_cosets * R * 8u : 0u));
+#ifdef P3GPU_NTT_PROFILE
+                { unsigned long long ts_; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ts_)); P3_PSTAMP(k, 2, ts_); }
+#endif
+                if (k == 0)
+                    for (u32 cs = 0; cs < a.n_cosets; cs++) bulk_load(twf + cs * R, tw_fwd + (size_t)cs * a.tw_stride, R * 8u, full_bar(b));
+                load_tile_twiddles(tws, a.tw, R_LOG, T, R_LOG, full_bar(b));
+                // tensor coordinates (column, 0, 0, 0, T): coefficient rows T * 2^r + rho (see launch_lde_mid)
+                tma_load_tile(&imap, data0 + b * buf_words, (int)col, 0, (int)T, full_bar(b));
+            };
+            load(0);
+            if (n_mine > 1) load(1);
+            for (u32 k = 0; k < n_mine; k++) {
+                const u32 b = k & 1u, tt = blockIdx.x + k * gridDim.x;
+                const u32 col = (tt % a.n_ctiles) * CT, L = tt / a.n_ctiles;
+#ifdef P3GPU_NTT_PROFILE
+                unsigned long long read_wait = 0;
+#endif
+                for (u32 cs = 0; cs < a.n_cosets; cs++) {
+                    // ready[b] completes once per coset of every tile in buffer b
+                    mbar_wait(ready_bar(b), ((k >> 1) * a.n_cosets + cs) & 1u);
+                    if (!P3_SKIP(a.skip_store)) {
+#ifdef P3GPU_NTT_PROFILE
+                        unsigned long long w0_, w1_;
+                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
+#endif
+                        // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
+                        tma_store_tile(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
+                        bulk_wait_read();   // the copy has read the buffer out: the next coset (or tile) may rewrite it
+#ifdef P3GPU_NTT_PROFILE
+                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
+                        read_wait += w1_ - w0_;
+#endif
+                    }
+                    if (cs + 1 < a.n_cosets) mbar_arrive(freed_bar);
+                }
+#ifdef P3GPU_NTT_PROFILE
+                P3_PSTAMP(k, 6, read_wait);
+#endif
+                if (k + 2 < n_mine) load(k + 2);
+            }
+            bulk_wait_all();
+            return;
+        }
+    } else {
+        for (u32 k = threadIdx.x; k < a.n_cosets * R; k += THREADS)   // heap entries 1..R-1 of every coset (entry 0 is unused)
+            if (k & (R - 1u)) cp_async8(twf + k, tw_fwd + (size_t)(k >> R_LOG) * a.tw_stride + (k & (R - 1u)));
+        issue(t, 0);   // the forward twiddles land with the first tile's group
+    }
     for (u32 k = 0; t < total; t += gridDim.x, k++) {
         const u32 buf = k & 1u;
-        if (threadIdx.x == 0) bulk_wait_read();   // the previous tile's last store has left the buffer refilled next
-        __syncthreads();   // every warp is done with the buffer that is refilled next
+        if constexpr (PROD) {
 #ifdef P3GPU_NTT_PROFILE
-        if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
+            if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
 #endif
-        P3_STAMP(1);
-        if (t + gridDim.x < total) { issue(t + gridDim.x, buf ^ 1u); P3_STAMP(2); cp_async_wait<1>(); }
-        else { P3_STAMP(2); cp_async_wait<0>(); }
-        __syncthreads();
+            P3_STAMP(1);
+            mbar_wait(full_bar(buf), (k >> 1) & 1u);   // every consumer thread waits for every tile, in order
+        } else {
+            if (threadIdx.x == 0) bulk_wait_read();   // the previous tile's last store has left the buffer refilled next
+            __syncthreads();   // every warp is done with the buffer that is refilled next
+#ifdef P3GPU_NTT_PROFILE
+            if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
+#endif
+            P3_STAMP(1);
+            if (t + gridDim.x < total) { issue(t + gridDim.x, buf ^ 1u); P3_STAMP(2); cp_async_wait<1>(); }
+            else { P3_STAMP(2); cp_async_wait<0>(); }
+            __syncthreads();
+        }
         P3_STAMP(3);
         u32 *data = data0 + buf * buf_words;
         const uint2 *twi = twi0 + buf * R;
@@ -577,7 +718,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                 if (c >= cw) { c -= cw; g++; }
             }
         }
-        __syncthreads();
+        consumer_sync<PROD, THREADS>();
         P3_STAMP(4);
         // ---- inverse step 2 into registers: thread (gf, c) takes inverse item g = bitrev_Q1(gf), local rows g*E2 + m.
         // (gf, not g, is linear in the thread index so that the per-coset stores below are bank-conflict free.)
@@ -592,23 +733,27 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q2>(coef, twi, E1 + g);
         }
 #ifdef P3GPU_NTT_PROFILE
-        unsigned long long store_wait = 0;   // slot 6: time thread 0 waits for the previous coset's store to leave the buffer
+        // slot 6 (PROD: 7): time thread 0 waits for the previous coset's store to leave the buffer (PROD: for the producer's `freed`)
+        unsigned long long store_wait = 0;
 #endif
         for (u32 cs = 0; cs < a.n_cosets; cs++) {
             const uint2 *tf = twf + cs * R;
             // (Running forward step 1 before this wait keeps y[] live next to coef[] across it: 80 bytes of spills at r = 10, ct = 20.)
-            if (cs > 0 && threadIdx.x == 0) {   // the previous coset's store has left the buffer
 #ifdef P3GPU_NTT_PROFILE
-                unsigned long long w0_, w1_;
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
-                bulk_wait_read();
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
-                store_wait += w1_ - w0_;
-#else
-                bulk_wait_read();
+            unsigned long long w0_ = 0, w1_ = 0;
+            if (cs > 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
 #endif
+            if (PROD && cs > 0) {
+                // the producer has seen the previous coset's store leave the buffer: `freed` completes n_cosets - 1 times per tile.
+                // coef[] is live here: at r = 10, ct = 20 a phase counter or the watchdog's registers would spill.
+                mbar_wait_plain(freed_bar, (k * (a.n_cosets - 1u) + cs - 1u) & 1u);
+            } else {
+                if (cs > 0 && threadIdx.x == 0) bulk_wait_read();   // the previous coset's store has left the buffer
+                consumer_sync<PROD, THREADS>();   // the tile buffer takes the forward layout (cs = 0: every warp is done with inverse step 2)
             }
-            __syncthreads();   // the tile buffer takes the forward layout (cs = 0: every warp is done with inverse step 2)
+#ifdef P3GPU_NTT_PROFILE
+            if (cs > 0) { asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_)); store_wait += w1_ - w0_; }
+#endif
             // ---- forward step 1: forward local rows gf + j*E1 = inverse local rows g*E2 + bitrev_Q2(j)
             if (active) {
                 u32 y[E2];
@@ -619,7 +764,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
 #pragma unroll
                 for (u32 j = 0; j < E2; j++) sp[j * gs2] = y[j];
             }
-            __syncthreads();
+            consumer_sync<PROD, THREADS>();
             // ---- forward step 2 (in place): item (j, c2) holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
             {
                 u32 j = threadIdx.x / cw, c2 = threadIdx.x - j * cw;
@@ -637,7 +782,12 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                     if (c2 >= cw) { c2 -= cw; j++; }
                 }
             }
-            if (!P3_SKIP(a.skip_store)) {
+            if constexpr (PROD) {
+                // this thread's shared-memory writes are ordered before the producer's tensor copies (the store of this coset, and
+                // after the last coset the next load into this buffer); then the producer may take the buffer
+                fence_proxy_async_smem();
+                mbar_arrive(ready_bar(buf));
+            } else if (!P3_SKIP(a.skip_store)) {
                 fence_proxy_async_smem();
                 __syncthreads();
                 // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
@@ -645,11 +795,11 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             }
         }
 #ifdef P3GPU_NTT_PROFILE
-        if (a.prof && threadIdx.x == 0 && k < 16) a.prof[((size_t)blockIdx.x * 16 + k) * 8 + 6] = store_wait;
+        if (a.prof && threadIdx.x == 0 && k < 16) a.prof[((size_t)blockIdx.x * 16 + k) * 8 + (PROD ? 7 : 6)] = store_wait;
 #endif
         P3_STAMP(5);
     }
-    if (threadIdx.x == 0) bulk_wait_all();
+    if (!PROD && threadIdx.x == 0) bulk_wait_all();
 }
 
 // ---- pipelined path: TMA tile loads + warp-specialised consumer groups -------------------------------------------
@@ -669,27 +819,6 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
 // neighbouring 32-byte segments of the same rows are requested within microseconds of each other (L2/DRAM page locality).
 // PERM = the pass reads its rows through the bit-reversal map (first forward pass of the LDE): the tile is then a CONTIGUOUS
 // block of rows holding local row rho at position bitrev_r(rho); the two steps simply swap their shared-memory access shapes.
-__device__ __forceinline__ void mbar_init(u32 bar, u32 count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_wait(u32 bar, u32 parity) {
-    u32 done = 0, spins = 0;
-    unsigned long long t0 = 0;
-    while (true) {
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (done) break;
-        // watchdog: a pass takes milliseconds; a wait of 20 s can only be a protocol error.  Trap (the launch fails with an error the
-        // host reports) instead of leaving a hung kernel on the device.
-        if ((++spins & 0xfffu) == 0) {
-            unsigned long long now;
-            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 20000000000ull) __trap();
-        }
-    }
-}
-__device__ __forceinline__ void mbar_arrive(u32 bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_arrive_n(u32 bar, u32 n) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(u32 bar, u32 bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory"); }
-
 template <int F, int R_LOG, bool PERM, int NSTAGE, int NGROUP, int GTHREADS>
 __global__ void __launch_bounds__(NGROUP * GTHREADS + 32, 1) ntt_pass_pipe_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ PassArgs a) {
     constexpr u32 CT = 8;
@@ -1079,17 +1208,21 @@ static int32_t launch_fast(p3gpu_ctx *ctx, const PassArgs &a) {
     }
 }
 
-template <int F, int R_LOG, int CT_T>
-static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap) {
+// Instances of the fused kernel that have a producer-warp form: every one but the runtime-width instance at r = 10, whose 384
+// consumer threads need 168 registers against the 152 that 416 threads leave them.
+template <int R_LOG, int CT_T> constexpr bool lde_mid_producer() { return R_LOG < 10 || CT_T != 0; }
+
+template <int F, int R_LOG, int CT_T, bool PROD>
+static int32_t launch_lde_mid_rcp(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
-    constexpr int THREADS = lde_mid_threads<R_LOG, CT_T>();
+    constexpr int THREADS = lde_mid_threads<R_LOG, CT_T>(), BLOCK = THREADS + (PROD ? 32 : 0);
     const size_t ct = a.ct, e1 = (size_t)1 << Q1, e2 = (size_t)1 << Q2;
     const size_t gs1 = e2 * ct + ((ct + 32 - ((e2 * ct) & 31)) & 31), gs2 = e1 * ct + ((ct + 32 - ((e1 * ct) & 31)) & 31);
     const size_t buf_words = (std::max(e1 * gs1, e2 * gs2) + 3) & ~(size_t)3;
-    const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2);
+    const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2) + (PROD ? 5 * 8 : 0);
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: fused LDE tile does not fit shared memory");
-    P3_CHECK(gs2 == (e1 + 1) * ct, P3GPU_EINVAL, "ntt: fused LDE tile layout is no TMA box");
-    auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T>;
+    P3_CHECK(gs2 == (e1 + 1) * ct && gs1 == (e2 + 1) * ct, P3GPU_EINVAL, "ntt: fused LDE tile layout is no TMA box");
+    auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T, PROD>;
     static size_t smem_set[64] = {0};   // per instantiation and device
     if (smem > 48 * 1024 && smem > smem_set[ctx->device & 63]) {
         P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1097,26 +1230,31 @@ static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 
     }
     const size_t tiles = ((size_t)1 << (a.log_n - R_LOG)) * a.n_ctiles;
     // persistent grid: as many CTAs per SM as threads, registers and shared memory allow (one at 2^20 rows)
-    size_t per_sm = std::min<size_t>(2048 / THREADS, (227 * 1024) / (smem + 1024));
+    size_t per_sm = std::min<size_t>(2048 / BLOCK, (227 * 1024) / (smem + 1024));
     static int num_regs = 0;   // per instantiation; benign race (same value)
     if (num_regs == 0) {
         cudaFuncAttributes fa;
         P3_CUDA(cudaFuncGetAttributes(&fa, kern));
         num_regs = std::max(fa.numRegs, 16);
     }
-    per_sm = std::max<size_t>(1, std::min<size_t>(per_sm, 65536 / ((size_t)THREADS * (size_t)num_regs)));
+    per_sm = std::max<size_t>(1, std::min<size_t>(per_sm, 65536 / ((size_t)BLOCK * (size_t)num_regs)));
     const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
-    kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, tw_fwd, omap);
+    kern<<<(unsigned)grid, BLOCK, smem, ctx->stream>>>(a, tw_fwd, omap, imap);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
+template <int F, int R_LOG, int CT_T>
+static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
+    if constexpr (lde_mid_producer<R_LOG, CT_T>()) return launch_lde_mid_rcp<F, R_LOG, CT_T, true>(ctx, a, tw_fwd, omap, imap);
+    else return launch_lde_mid_rcp<F, R_LOG, CT_T, false>(ctx, a, tw_fwd, omap, imap);
+}
 template <int F, int R_LOG>
-static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap) {
+static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
     switch (a.ct) {
-        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd, omap);
-        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd, omap);
-        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd, omap);
+        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd, omap, imap);
+        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd, omap, imap);
+        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd, omap, imap);
     }
 }
 
@@ -1278,13 +1416,15 @@ static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd) {
     const int r = a.l1 - a.l0;
     PassArgs o = a;
     o.l0 = 0; o.l1 = r;
-    CUtensorMap omap;
+    CUtensorMap omap, imap;
     P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
+    // input (producer-warp form): inverse tile T = coefficient rows T * 2^r + rho in the inverse layout, groups of 2^ceil(r/2) rows
+    P3_TRY(make_pass_tensor_map(a, a.in, false, 0, a.ct, false, (r + 1) / 2, &imap));
     switch (r) {
-        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd, omap);
-        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd, omap);
-        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd, omap);
-        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd, omap);
+        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd, omap, imap);
+        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd, omap, imap);
+        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd, omap, imap);
+        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd, omap, imap);
     }
 }
 

@@ -45,8 +45,13 @@ for li in range(3, 6):
     print(f"launch {names[li - 3]}: {n_cta} CTAs, {len(rows)} stamped tiles")
     print(f"   issue {np.mean(issued - start) / 1e3:7.2f} us | load wait {np.mean(loaded - issued) / 1e3:7.2f} | step1 {np.mean(s1 - loaded) / 1e3:7.2f} | "
           f"step2+stores {np.mean(s2 - s1) / 1e3:7.2f} | tile total {np.mean(s2 - start) / 1e3:7.2f}")
-    if li == 4:   # slot 6: the fused pass's waits for a coset's store to leave the tile buffer, summed over the tile's cosets
-        print(f"   wait for the previous coset's store {np.mean(rows[:, 6].astype(np.float64)) / 1e3:7.2f} us per tile")
+    if li == 4:
+        # slot 6: the waits for a coset's store to leave the tile buffer, summed over the tile's cosets (producer-warp form: the
+        # producer's read-out waits, off the consumers' path); slot 7 (producer-warp form only): the consumers' waits for the
+        # producer's `freed` before the next coset, and slot 2 is the producer's load issue
+        print(f"   wait for the stores to be read out {np.mean(rows[:, 6].astype(np.float64)) / 1e3:7.2f} us per tile")
+        if rows[:, 7].any():
+            print(f"   consumers' wait for the buffer between cosets {np.mean(rows[:, 7].astype(np.float64)) / 1e3:7.2f} us per tile")
     # per CTA: gap between consecutive tiles (the wait for the store of the buffer refilled next, and the leading barrier)
     gaps = []
     for c in range(d.shape[0]):

@@ -11,6 +11,33 @@ pub struct P3GpuChallenger {
     _private: [u8; 0],
 }
 
+#[repr(C)]
+pub struct P3GpuAirProgram {
+    _private: [u8; 0],
+}
+
+/// `p3gpu_air_node`: op is one of the `P3GPU_AIR_*` codes below; operands refer only to earlier nodes.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct P3GpuAirNode {
+    pub op: u32,
+    pub a: u32,
+    pub b: u32,
+    pub imm: u32,
+}
+
+pub const P3GPU_AIR_CONST: u32 = 0;
+pub const P3GPU_AIR_MAIN_LOCAL: u32 = 1;
+pub const P3GPU_AIR_MAIN_NEXT: u32 = 2;
+pub const P3GPU_AIR_PUBLIC: u32 = 3;
+pub const P3GPU_AIR_IS_FIRST_ROW: u32 = 4;
+pub const P3GPU_AIR_IS_LAST_ROW: u32 = 5;
+pub const P3GPU_AIR_IS_TRANSITION: u32 = 6;
+pub const P3GPU_AIR_ADD: u32 = 7;
+pub const P3GPU_AIR_SUB: u32 = 8;
+pub const P3GPU_AIR_NEG: u32 = 9;
+pub const P3GPU_AIR_MUL: u32 = 10;
+
 pub const P3GPU_BABY_BEAR: i32 = 0;
 pub const P3GPU_KOALA_BEAR: i32 = 1;
 pub const P3GPU_DFT: i32 = 0;
@@ -129,6 +156,15 @@ unsafe extern "C" {
                                     log_trace_height: c_uint, alpha: *const u32, d_quotient: *mut u32) -> i32;
     pub fn p3gpu_p2air_generate_trace_cols_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_inputs: *const u32, n_perms: usize,
                                                col0: usize, col1: usize, d_out: *mut u32) -> i32;
+
+    // any AIR as a constraint program (symbolic expression DAG -> register program -> quotient kernel)
+    pub fn p3gpu_air_program_create(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize, constraints: *const u32,
+                                    n_constraints: usize, width: u32, n_public: u32, out: *mut *mut P3GpuAirProgram) -> i32;
+    pub fn p3gpu_air_program_destroy(prog: *mut P3GpuAirProgram);
+    pub fn p3gpu_air_program_info(prog: *const P3GpuAirProgram, n_instructions: *mut usize, n_slots: *mut usize, n_constraints: *mut usize) -> i32;
+    pub fn p3gpu_air_quotient_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, d_lde: *const u32, log_lde_height: c_uint,
+                                  log_quotient_size: c_uint, log_trace_height: c_uint, public_values: *const u32, alpha: *const u32,
+                                  d_quotient: *mut u32) -> i32;
 
     // DuplexChallenger with device-resident state
     pub fn p3gpu_challenger_new(ctx: *mut P3GpuCtx, field: c_int, width: c_int, rate: c_int, out: *mut *mut P3GpuChallenger) -> i32;

@@ -226,6 +226,44 @@ int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, cons
 int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms,
                                             size_t col0, size_t col1, uint32_t *d_out);
 
+/* ---- any AIR as a constraint program (DESIGN.md section 4.7) ----------------------------------------------------------------
+ * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
+ * (operands refer only to earlier nodes) plus the list of constrained nodes in assertion order.  The library compiles it once
+ * into a register program; p3gpu_air_quotient_dev runs that program over the quotient domain (uni-stark/src/prover.rs:462-827).
+ * Not supported: periodic or preprocessed columns, extension-field constraints, ZK. */
+enum {
+    P3GPU_AIR_CONST = 0,          /* imm: the constant, Montgomery word */
+    P3GPU_AIR_MAIN_LOCAL = 1,     /* a: column of the current row */
+    P3GPU_AIR_MAIN_NEXT = 2,      /* a: column of the next row (wraps at the end of the domain) */
+    P3GPU_AIR_PUBLIC = 3,         /* a: public value index */
+    P3GPU_AIR_IS_FIRST_ROW = 4,   /* selectors as selectors_on_coset (commit/src/domain.rs:321-361), unnormalised */
+    P3GPU_AIR_IS_LAST_ROW = 5,
+    P3GPU_AIR_IS_TRANSITION = 6,
+    P3GPU_AIR_ADD = 7,            /* a + b */
+    P3GPU_AIR_SUB = 8,            /* a - b */
+    P3GPU_AIR_NEG = 9,            /* -a */
+    P3GPU_AIR_MUL = 10            /* a * b */
+};
+typedef struct { uint32_t op, a, b, imm; } p3gpu_air_node;
+typedef struct p3gpu_air_program p3gpu_air_program;
+
+/* Validates and compiles.  P3GPU_EINVAL: a column >= width, a public index >= n_public, an operand that is not an earlier node, a
+ * constraint that names no node, an unknown op, a constant >= p.  P3GPU_EUNSUPPORTED: a field other than BabyBear / KoalaBear, more
+ * than 2048 constraints or more than 384 simultaneously live values (the message states the limit). */
+int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                 size_t n_constraints, uint32_t width, uint32_t n_public, p3gpu_air_program **out);
+void p3gpu_air_program_destroy(p3gpu_air_program *prog);
+/* instruction count (computes + folds), slot count (the most values live at once) and constraint count; NULL outputs are skipped */
+int32_t p3gpu_air_program_info(const p3gpu_air_program *prog, size_t *n_instructions, size_t *n_slots, size_t *n_constraints);
+/* Quotient values of the AIR over the quotient domain GENERATOR * K, |K| = 2^log_quotient_size, from the first 2^log_quotient_size rows
+ * of the committed bit-reversed trace LDE d_lde (2^log_lde_height rows, `width` columns): the fast path of get_evaluations_on_domain
+ * (two_adic_pcs.rs:376-385).  log_trace_height <= log_quotient_size <= log_lde_height, log_quotient_size - log_trace_height <= 8.
+ * public_values: n_public Montgomery words (host).  d_quotient: 2^log_quotient_size EF4 values in NATURAL order (what
+ * p3gpu_p2air_quotient_dev writes). */
+int32_t p3gpu_air_quotient_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_lde, unsigned log_lde_height,
+                               unsigned log_quotient_size, unsigned log_trace_height, const uint32_t *public_values, const uint32_t alpha[4],
+                               uint32_t *d_quotient);
+
 /* ---- transcript and query phase of the prove driver (SURVEY.md 8f rank 4 / N1) ----------------------------------------
  * DuplexChallenger<F, Poseidon2<width>, width, rate> (challenger/src/duplex_challenger.rs:60-300) with its state resident on the
  * device, so that caps and opened values produced on the GPU are absorbed without a PCIe round trip per duplexing.  The

@@ -11,6 +11,7 @@ _HERE = pathlib.Path(__file__).resolve().parent
 LIB_PATH = pathlib.Path(os.environ["P3GPU_LIB"]) if os.environ.get("P3GPU_LIB") else _HERE / "libp3gpu.so"
 
 BABY_BEAR, KOALA_BEAR = 0, 1
+EOK, EINVAL, EUNSUPPORTED, ECUDA, ENOMEM, ESTATE = 0, -1, -2, -3, -4, -5
 DFT, IDFT, COSET_DFT, COSET_IDFT = 0, 1, 2, 3
 HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_KECCAK = 0, 1, 2
 
@@ -29,6 +30,7 @@ EXPORTS = [
     "p3gpu_ipc_export", "p3gpu_ipc_import", "p3gpu_ipc_close", "p3gpu_memset_dev", "p3gpu_peer_barrier_dev",
     "p3gpu_peer_allgather_dev", "p3gpu_coset_lde_batch_sharded_dev", "p3gpu_commit_sharded_dev", "p3gpu_shard_chunk_bounds",
     "p3gpu_p2air_generate_trace_cols_dev", "p3gpu_shard_col_segments", "p3gpu_peer_exchange_dev", "p3gpu_p2air_quotient_sharded_dev",
+    "p3gpu_air_program_create", "p3gpu_air_program_destroy", "p3gpu_air_program_info", "p3gpu_air_quotient_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -41,7 +43,11 @@ class PeerGroupStruct(C.Structure):
 
 
 class P3GpuError(RuntimeError):
-    pass
+    """A non-zero return code of the library; `code` is the P3GPU_E* value (0 for errors raised before any call)."""
+
+    def __init__(self, msg, code=0):
+        super().__init__(msg)
+        self.code = code
 
 
 _lib = None
@@ -117,6 +123,10 @@ def load():
         "p3gpu_shard_col_segments": (i32, [u32, vp, sz, vp, sz, vp]),
         "p3gpu_peer_exchange_dev": (i32, [vp, vp, vp, vp, vp, sz]),
         "p3gpu_p2air_quotient_sharded_dev": (i32, [vp, ci, ci, vp, vp, cu, cu, vp, vp]),
+        "p3gpu_air_program_create": (i32, [vp, ci, vp, sz, vp, sz, u32, u32, C.POINTER(vp)]),
+        "p3gpu_air_program_destroy": (None, [vp]),
+        "p3gpu_air_program_info": (i32, [vp, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]),
+        "p3gpu_air_quotient_dev": (i32, [vp, vp, vp, cu, cu, cu, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -127,4 +137,4 @@ def load():
 
 def check(rc: int):
     if rc != 0:
-        raise P3GpuError(f"libp3gpu error {rc}: {load().p3gpu_last_error().decode()}")
+        raise P3GpuError(f"libp3gpu error {rc}: {load().p3gpu_last_error().decode()}", rc)

@@ -1,0 +1,263 @@
+"""Any AIR as symbolic constraints: a builder that mirrors the reference's `AirBuilder` / `SymbolicAirBuilder`
+(air/src/air.rs, air/src/symbolic/{builder,expression}.rs) and `SymbolicAir`, which gives `uni_stark.prove` / `verify` everything they
+read from an AIR.
+
+    def fib(b):                                   # uni-stark/tests/fib_air.rs:33-75
+        m, pis = b.main(), b.public_values()
+        l, r, nl, nr = m.local[0], m.local[1], m.next[0], m.next[1]
+        b.when_first_row().assert_eq(l, pis[0]); b.when_first_row().assert_eq(r, pis[1])
+        t = b.when_transition(); t.assert_eq(r, nl); t.assert_eq(l + r, nr)
+        b.when_last_row().assert_eq(r, pis[2])
+    air = SymbolicAir(BabyBear, 2, fib, num_public_values=3, gpu=gpu)
+
+`eval` runs once, on the host, and records an expression DAG: identical subexpressions are one node (hash-consed), and every node
+carries the reference's `degree_multiple` (expression.rs:44-48).  The prover compiles the DAG into a register program on the device
+(p3gpu_air_program_create) and evaluates the quotient there (p3gpu_air_quotient_dev); there is no CPU evaluation of the quotient.
+The verifier's constraint folder evaluates the same DAG at the out-of-domain point.
+
+Not offered: periodic and preprocessed columns, extension-field constraints (assert_zero_ext), ZK.
+"""
+from __future__ import annotations
+
+from typing import Callable, Optional, Sequence
+
+import numpy as np
+
+from . import _lib
+from .field import Field
+
+# node ops (include/p3gpu.h P3GPU_AIR_*)
+CONST, MAIN_LOCAL, MAIN_NEXT, PUBLIC, IS_FIRST_ROW, IS_LAST_ROW, IS_TRANSITION, ADD, SUB, NEG, MUL = range(11)
+BINARY = (ADD, SUB, MUL)
+
+
+class Expr:
+    """A node of the expression DAG.  +, -, * and unary - with other expressions or Python integers; `x ** k` by squaring."""
+    __slots__ = ("g", "i")
+
+    def __init__(self, g: "SymbolicAirBuilder", i: int):
+        self.g, self.i = g, i
+
+    def _e(self, x) -> "Expr":
+        return x if isinstance(x, Expr) else self.g.constant(x)
+
+    def __add__(self, o): return self.g._node(ADD, self.i, self._e(o).i)
+    def __radd__(self, o): return self.g._node(ADD, self._e(o).i, self.i)
+    def __sub__(self, o): return self.g._node(SUB, self.i, self._e(o).i)
+    def __rsub__(self, o): return self.g._node(SUB, self._e(o).i, self.i)
+    def __mul__(self, o): return self.g._node(MUL, self.i, self._e(o).i)
+    def __rmul__(self, o): return self.g._node(MUL, self._e(o).i, self.i)
+    def __neg__(self): return self.g._node(NEG, self.i)
+
+    def __pow__(self, e: int):
+        """exp_u64: square and multiply (e >= 1)."""
+        if e < 1:
+            return self.g.constant(1)
+        acc, base = None, self
+        while e:
+            if e & 1:
+                acc = base if acc is None else acc * base
+            e >>= 1
+            if e:
+                base = base * base
+        return acc
+
+    def degree(self) -> int:
+        return self.g.degrees[self.i]
+
+
+class _Row:
+    def __init__(self, g, op, width):
+        self.g, self.op, self.width = g, op, width
+
+    def __len__(self): return self.width
+
+    def __getitem__(self, c):
+        if isinstance(c, slice):
+            return [self[k] for k in range(*c.indices(self.width))]
+        if not 0 <= c < self.width:
+            raise IndexError(f"column {c} outside the trace width {self.width}")
+        return self.g._node(self.op, c)
+
+
+class _Main:
+    """builder.main(): `local[c]` (current row) and `next[c]` (next row)."""
+
+    def __init__(self, g, width):
+        self.local, self.next = _Row(g, MAIN_LOCAL, width), _Row(g, MAIN_NEXT, width)
+
+
+class _Ops:
+    """AirBuilder's provided methods (air/src/air.rs) on top of assert_zero."""
+
+    def assert_zero(self, x):
+        raise NotImplementedError
+
+    def assert_eq(self, x, y): self.assert_zero(self._root._e(x) - y)
+    def assert_one(self, x): self.assert_zero(self._root._e(x) - 1)
+
+    def assert_bool(self, x):
+        x = self._root._e(x)
+        self.assert_zero(x * (x - 1))
+
+    def when(self, cond): return _Filtered(self, self._root._e(cond))
+    def when_first_row(self): return self.when(self._root.is_first_row())
+    def when_last_row(self): return self.when(self._root.is_last_row())
+    def when_transition(self): return self.when(self._root.is_transition())
+
+    def main(self): return self._root.main()
+    def public_values(self): return self._root.public_values()
+    def is_first_row(self): return self._root.is_first_row()
+    def is_last_row(self): return self._root.is_last_row()
+    def is_transition(self): return self._root.is_transition()
+
+
+class _Filtered(_Ops):
+    """FilteredAirBuilder: every assertion is multiplied by the condition."""
+
+    def __init__(self, inner, cond: Expr):
+        self._inner, self._cond, self._root = inner, cond, inner._root
+
+    def assert_zero(self, x): self._inner.assert_zero(self._cond * self._root._e(x))
+
+
+class SymbolicAirBuilder(_Ops):
+    """Records an AIR's constraints as a hash-consed expression DAG (nodes in topological order)."""
+
+    def __init__(self, field: Field, width: int, num_public_values: int = 0):
+        self.field, self.width, self.num_public = field, int(width), int(num_public_values)
+        self._root = self
+        self.nodes: list = []          # (op, a, b, imm)
+        self.degrees: list = []
+        self.constraints: list = []    # node indices in assertion order
+        self._memo: dict = {}
+
+    def _e(self, x) -> Expr:
+        return x if isinstance(x, Expr) else self.constant(x)
+
+    def _node(self, op, a=0, b=0, imm=0) -> Expr:
+        key = (op, a, b, imm)
+        i = self._memo.get(key)
+        if i is None:
+            d = self.degrees
+            deg = {MAIN_LOCAL: 1, MAIN_NEXT: 1, IS_FIRST_ROW: 1, IS_LAST_ROW: 1}.get(op, 0)      # degree_multiple
+            if op in (ADD, SUB):
+                deg = max(d[a], d[b])
+            elif op == NEG:
+                deg = d[a]
+            elif op == MUL:
+                deg = d[a] + d[b]
+            i = len(self.nodes)
+            self.nodes.append(key); d.append(deg); self._memo[key] = i
+        return Expr(self, i)
+
+    def constant(self, v: int) -> Expr:
+        if isinstance(v, Expr):
+            return v
+        if not isinstance(v, (int, np.integer)):
+            raise TypeError(f"constants are integers, got {type(v).__name__}")
+        return self._node(CONST, imm=self.field.to_monty(int(v) % self.field.P))
+
+    def main(self): return _Main(self, self.width)
+
+    def public_values(self):
+        return [self._node(PUBLIC, k) for k in range(self.num_public)]
+
+    def is_first_row(self): return self._node(IS_FIRST_ROW)
+    def is_last_row(self): return self._node(IS_LAST_ROW)
+    def is_transition(self): return self._node(IS_TRANSITION)
+
+    def assert_zero(self, x):
+        x = self._e(x)
+        if x.g is not self:
+            raise ValueError("expression built by another builder")
+        self.constraints.append(x.i)
+
+    def node_array(self) -> np.ndarray:
+        return np.array(self.nodes, dtype=np.uint32).reshape(-1, 4)
+
+
+class SymbolicAir:
+    """An AIR given by `eval_fn(builder)`, in the surface uni_stark.prove and verifier.verify read."""
+
+    def __init__(self, field: Field, width: int, eval_fn: Callable, num_public_values: int = 0,
+                 main_next_row_columns: Optional[Sequence[int]] = None, max_constraint_degree: Optional[int] = None, gpu=None):
+        self.field, self.gpu = field, gpu
+        b = SymbolicAirBuilder(field, width, num_public_values)
+        eval_fn(b)
+        self.builder = b
+        self.nodes = b.node_array()
+        self.constraints = np.array(b.constraints, dtype=np.uint32)
+        # BaseAir::main_next_row_columns defaults to every column; it decides whether the proof carries the next-row opening
+        self._next_cols = list(range(b.width)) if main_next_row_columns is None else [int(c) for c in main_next_row_columns]
+        if not self._next_cols and any(n[0] == MAIN_NEXT for n in b.nodes):
+            raise ValueError("the constraints read the next row but main_next_row_columns() is empty")
+        self._degree_hint = max_constraint_degree
+        self._program = None
+
+    # ---- BaseAir / the degree the quotient is split by
+    def width(self) -> int: return self.builder.width
+    def num_public_values(self) -> int: return self.builder.num_public
+    def main_next_row_columns(self): return list(self._next_cols)
+
+    def constraint_degrees(self):
+        return [self.builder.degrees[c] for c in self.builder.constraints]
+
+    def max_constraint_degree(self) -> int:
+        """The hint if given (uni-stark/src/symbolic.rs), otherwise the largest degree_multiple of a constraint."""
+        if self._degree_hint is not None:
+            return int(self._degree_hint)
+        return max(self.constraint_degrees(), default=0)
+
+    # ---- prover: the quotient on the device
+    def program(self):
+        if self.gpu is None:
+            raise _lib.P3GpuError("quotient evaluation needs a GPU context (no CPU fallback)")
+        if self._program is None:
+            self._program = self.gpu.air_program_create(self.field.id, self.nodes, self.constraints, self.width(), self.num_public_values())
+        return self._program
+
+    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=()):
+        """uni-stark/src/prover.rs:462-827: `trace_lde_dev` holds the trace on the quotient domain GENERATOR * K, |K| = its height, in
+        bit-reversed row order (the committed LDE or its prefix).  Returns (|K|, 4) in natural order.  `public_values`: canonical."""
+        if len(public_values) != self.num_public_values():
+            raise ValueError(f"{len(public_values)} public values given, the AIR has {self.num_public_values()}")
+        prog = self.program()
+        H = int(trace_lde_dev.shape[0])
+        pv = [self.field.to_monty(int(v) % self.field.P) for v in public_values]
+        return self.gpu.air_quotient(prog, trace_lde_dev, H.bit_length() - 1, log_degree, pv, alpha)
+
+    # ---- verifier: the constraint folder on the same DAG
+    def eval_folded_constraints(self, e, local, nxt, public_values, is_first_row, is_last_row, is_transition, alpha):
+        """VerifierConstraintFolder (uni-stark/src/folder.rs): acc = acc * alpha + c per constraint, on canonical EF4 values (`e`:
+        verifier.Ext), every node evaluated once."""
+        f = self.field
+        vals = []
+        for op, a, b, imm in self.builder.nodes:
+            if op == CONST:
+                v = e.base(f.from_monty(imm))
+            elif op == MAIN_LOCAL:
+                v = local[a]
+            elif op == MAIN_NEXT:
+                v = nxt[a]
+            elif op == PUBLIC:
+                v = e.base(int(public_values[a]))
+            elif op == IS_FIRST_ROW:
+                v = is_first_row
+            elif op == IS_LAST_ROW:
+                v = is_last_row
+            elif op == IS_TRANSITION:
+                v = is_transition
+            elif op == ADD:
+                v = e.add(vals[a], vals[b])
+            elif op == SUB:
+                v = e.sub(vals[a], vals[b])
+            elif op == NEG:
+                v = e.sub(e.ZERO, vals[a])
+            else:
+                v = e.mul(vals[a], vals[b])
+            vals.append(v)
+        acc = [0, 0, 0, 0]
+        for c in self.builder.constraints:
+            acc = e.add(e.mul(acc, alpha), vals[c])
+        return acc

@@ -1,0 +1,271 @@
+// Constraint programs: an AIR given as a symbolic expression DAG (the reference's SymbolicExpression, air/src/symbolic/expression.rs),
+// compiled once into a register program that air_program.cu's quotient kernel interprets over the quotient domain.
+//
+// This header holds everything that is not a CUDA launch — the node validation, the compiler, the per-instruction semantics and
+// the per-row quotient evaluation — so host C++ can include it (tests/cpp/air_program_check.cpp runs it against the oracle on the
+// CPU) exactly as the kernel does.
+//
+//   nodes        p3gpu_air_node {op, a, b, imm} in topological order (operands refer only to earlier nodes)
+//   compile      drop dead nodes; per constraint in assertion order emit its not yet emitted cone (post-order), then FOLD it;
+//                slots by liveness (an operand's slot is released at its last use, before the result is allocated), so the slot
+//                count is the maximum number of simultaneously live values
+//   instruction  2 words: op_dst = op | dst << 4, arg = operand (binary: a | b << 16; leaf: column / public index / Montgomery
+//                constant; FOLD: dst is the constraint index, arg the slot)
+//   fold         acc += c_k * alpha^(K - 1 - k) (the first constraint gets the highest power, air/src/symbolic/builder.rs:482-511),
+//                lazily in 64 bits per coefficient; quotient = acc / Z_H(x)
+#pragma once
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "../../include/p3gpu.h"
+#include "field.cuh"
+
+namespace p3 {
+
+constexpr u32 AIR_OP_FOLD = 11;                 // instruction-only op, after the node ops P3GPU_AIR_CONST .. P3GPU_AIR_MUL
+constexpr u32 AIR_MAX_SLOTS = 384;              // 384 slots x 128 threads x 4 B = 192 KiB of shared memory per block
+constexpr u32 AIR_MAX_CONSTRAINTS = 2048;       // alpha-power table: 32 KiB of shared memory
+constexpr u32 AIR_BLOCK = 128;
+constexpr unsigned AIR_MAX_RATE_BITS = 8;       // q = log_quotient_size - log_trace_height <= 8: Z_H tables of <= 256 entries
+
+// uses_mask bits
+constexpr u32 AIR_USES_NEXT = 1, AIR_USES_SELECTORS = 2, AIR_USES_PUBLIC = 4;
+
+struct AirInsn { u32 op_dst, arg; };
+
+struct AirProgram {
+    int field = 0;
+    u32 width = 0, n_public = 0;
+    u32 n_slots = 0, n_constraints = 0, uses = 0;
+    std::vector<AirInsn> insns;
+};
+
+inline size_t air_smem_bytes(u32 n_slots, u32 n_constraints) { return (size_t)n_constraints * 16 + (size_t)n_slots * AIR_BLOCK * 4; }
+
+// Validates the node list and compiles it.  Returns P3GPU_OK, P3GPU_EINVAL (malformed nodes / constraints) or P3GPU_EUNSUPPORTED
+// (beyond the slot or constraint limit); `err` says why.
+inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints, size_t n_constraints,
+                           u32 width, u32 n_public, AirProgram &out, std::string &err) {
+    auto fail = [&](int32_t code, const std::string &m) { err = m; return code; };
+    if (field != BABY_BEAR && field != KOALA_BEAR) return fail(P3GPU_EUNSUPPORTED, "AIR program: unsupported field " + std::to_string(field));
+    const u32 P = field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
+    if (n_nodes > 0 && nodes == nullptr) return fail(P3GPU_EINVAL, "AIR program: null node list");
+    if (n_constraints > 0 && constraints == nullptr) return fail(P3GPU_EINVAL, "AIR program: null constraint list");
+    if (n_nodes >= (1ull << 31)) return fail(P3GPU_EINVAL, "AIR program: too many nodes");
+    for (size_t i = 0; i < n_nodes; i++) {
+        const p3gpu_air_node &n = nodes[i];
+        const std::string at = "AIR program: node " + std::to_string(i) + ": ";
+        switch (n.op) {
+            case P3GPU_AIR_CONST:
+                if (n.imm >= P) return fail(P3GPU_EINVAL, at + "constant is not a canonical Montgomery word");
+                break;
+            case P3GPU_AIR_MAIN_LOCAL: case P3GPU_AIR_MAIN_NEXT:
+                if (n.a >= width) return fail(P3GPU_EINVAL, at + "column " + std::to_string(n.a) + " >= width " + std::to_string(width));
+                break;
+            case P3GPU_AIR_PUBLIC:
+                if (n.a >= n_public) return fail(P3GPU_EINVAL, at + "public value " + std::to_string(n.a) + " >= " + std::to_string(n_public));
+                break;
+            case P3GPU_AIR_IS_FIRST_ROW: case P3GPU_AIR_IS_LAST_ROW: case P3GPU_AIR_IS_TRANSITION:
+                break;
+            case P3GPU_AIR_ADD: case P3GPU_AIR_SUB: case P3GPU_AIR_MUL:
+                if (n.b >= i) return fail(P3GPU_EINVAL, at + "operand b = " + std::to_string(n.b) + " is not an earlier node");
+                // fallthrough
+            case P3GPU_AIR_NEG:
+                if (n.a >= i) return fail(P3GPU_EINVAL, at + "operand a = " + std::to_string(n.a) + " is not an earlier node");
+                break;
+            default:
+                return fail(P3GPU_EINVAL, at + "unknown op " + std::to_string(n.op));
+        }
+    }
+    for (size_t k = 0; k < n_constraints; k++)
+        if (constraints[k] >= n_nodes) return fail(P3GPU_EINVAL, "AIR program: constraint " + std::to_string(k) + " names node " +
+                                                               std::to_string(constraints[k]) + " of " + std::to_string(n_nodes));
+    if (n_constraints > AIR_MAX_CONSTRAINTS)
+        return fail(P3GPU_EUNSUPPORTED, "AIR program: " + std::to_string(n_constraints) + " constraints (at most " + std::to_string(AIR_MAX_CONSTRAINTS) + ")");
+
+    auto is_binary = [](u32 op) { return op == P3GPU_AIR_ADD || op == P3GPU_AIR_SUB || op == P3GPU_AIR_MUL; };
+    // schedule: events are node indices (compute) or ~k (fold constraint k)
+    std::vector<int64_t> events;
+    std::vector<uint8_t> state(n_nodes, 0);     // 0 new, 1 on the stack, 2 emitted
+    std::vector<std::pair<u32, int>> stack;
+    for (size_t k = 0; k < n_constraints; k++) {
+        if (state[constraints[k]] != 2) {
+            stack.push_back({constraints[k], 0});
+            while (!stack.empty()) {
+                auto &top = stack.back();
+                const p3gpu_air_node &n = nodes[top.first];
+                const int n_ops = is_binary(n.op) ? 2 : n.op == P3GPU_AIR_NEG ? 1 : 0;
+                if (top.second < n_ops) {
+                    const u32 c = top.second == 0 ? n.a : n.b;
+                    top.second++;
+                    if (state[c] == 0) { state[c] = 1; stack.push_back({c, 0}); }
+                } else {
+                    state[top.first] = 2;
+                    events.push_back(top.first);
+                    stack.pop_back();
+                }
+            }
+        }
+        events.push_back(~(int64_t)k);
+    }
+    // liveness: last event that reads each node
+    std::vector<size_t> last(n_nodes, 0);
+    for (size_t p = 0; p < events.size(); p++) {
+        if (events[p] < 0) { last[constraints[~events[p]]] = p; continue; }
+        const p3gpu_air_node &n = nodes[events[p]];
+        if (is_binary(n.op) || n.op == P3GPU_AIR_NEG) last[n.a] = p;
+        if (is_binary(n.op)) last[n.b] = p;
+    }
+    std::vector<u32> slot(n_nodes, 0), free_slots;
+    AirProgram prog;
+    prog.field = field; prog.width = width; prog.n_public = n_public; prog.n_constraints = (u32)n_constraints;
+    prog.insns.reserve(events.size());
+    auto release = [&](u32 node, size_t p) { if (last[node] == p) free_slots.push_back(slot[node]); };
+    for (size_t p = 0; p < events.size(); p++) {
+        if (events[p] < 0) {
+            const u32 k = (u32)~events[p], c = constraints[k];
+            prog.insns.push_back({AIR_OP_FOLD | (k << 4), slot[c]});
+            release(c, p);
+            continue;
+        }
+        const u32 i = (u32)events[p];
+        const p3gpu_air_node &n = nodes[i];
+        u32 arg = 0;
+        switch (n.op) {
+            case P3GPU_AIR_CONST: arg = n.imm; break;
+            case P3GPU_AIR_MAIN_LOCAL: arg = n.a; break;
+            case P3GPU_AIR_MAIN_NEXT: arg = n.a; prog.uses |= AIR_USES_NEXT; break;
+            case P3GPU_AIR_PUBLIC: arg = n.a; prog.uses |= AIR_USES_PUBLIC; break;
+            case P3GPU_AIR_IS_FIRST_ROW: case P3GPU_AIR_IS_LAST_ROW: case P3GPU_AIR_IS_TRANSITION: prog.uses |= AIR_USES_SELECTORS; break;
+            case P3GPU_AIR_NEG: arg = slot[n.a]; release(n.a, p); break;
+            default:
+                arg = slot[n.a] | (slot[n.b] << 16);
+                release(n.a, p);
+                if (n.b != n.a) release(n.b, p);
+        }
+        if (free_slots.empty()) free_slots.push_back(prog.n_slots++);
+        slot[i] = free_slots.back();
+        free_slots.pop_back();
+        if (prog.n_slots > AIR_MAX_SLOTS)
+            return fail(P3GPU_EUNSUPPORTED, "AIR program: more than " + std::to_string(AIR_MAX_SLOTS) + " simultaneously live values (slots)");
+        prog.insns.push_back({n.op | (slot[i] << 4), arg});
+    }
+    out = std::move(prog);
+    return P3GPU_OK;
+}
+
+// ---- per-instruction semantics and per-row quotient, shared by the kernel and host C++ -------------------------------------
+template <int F> __host__ __device__ __forceinline__ void air_qmac(u64 (&acc)[4], u32 c, const uint4 a) {
+    // acc += c * a (base x EF4), lazily: invariant acc < p * 2^32 (open.cu lazy_mac, air.cu qmac)
+    const u32 av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int d = 0; d < 4; d++) {
+        acc[d] += (u64)c * av[d];
+        u32 hi = (u32)(acc[d] >> 32);
+        const u32 hs = hi - Fp<F>::P;
+        hi = hi < hs ? hi : hs;
+        acc[d] = ((u64)hi << 32) | (u32)acc[d];
+    }
+}
+
+__host__ __device__ __forceinline__ u32 air_bitrev(u32 i, unsigned bits) {
+    if (bits == 0) return 0;
+#ifdef __CUDA_ARCH__
+    return __brev(i) >> (32 - bits);
+#else
+    u32 r = 0;
+    for (unsigned b = 0; b < bits; b++) r |= ((i >> b) & 1u) << (bits - 1 - b);
+    return r;
+#endif
+}
+
+// Per-launch constants of the quotient evaluation over the quotient domain g * K, |K| = 2^log_q = 2^(log_n + q).
+struct AirDomain {
+    unsigned log_q, q;          // q = log_q - log_n
+    u32 shift;                  // g = GENERATOR (Montgomery)
+    u32 w_q;                    // generator of K
+    u32 w_n_inv;                // omega_N^-1
+    u32 uses;
+};
+
+// Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),
+// the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <int F, class Env> __host__ __device__ __forceinline__ uint4 air_row_quotient(Env &env, const AirDomain &d, u32 n_insns, u32 i) {
+    const u32 mask = d.log_q == 32 ? 0xffffffffu : ((1u << d.log_q) - 1u);
+    env.set_rows(air_bitrev(i, d.log_q), (d.uses & AIR_USES_NEXT) ? air_bitrev((i + (1u << d.q)) & mask, d.log_q) : 0u);
+    u32 first = 0, last = 0, trans = 0;
+    if (d.uses & AIR_USES_SELECTORS) {
+        // selectors_on_coset (commit/src/domain.rs:321-361), unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1
+        const u32 x = mont_mul<F>(d.shift, fp_pow<F>(d.w_q, i));
+        const u32 zh = env.zh(i);
+        const u32 a = fp_sub<F>(x, Fp<F>::ONE), b = fp_sub<F>(x, d.w_n_inv);
+        const u32 inv_ab = fp_inv<F>(mont_mul<F>(a, b));          // one inversion for both denominators
+        first = mont_mul<F>(zh, mont_mul<F>(b, inv_ab));
+        last = mont_mul<F>(zh, mont_mul<F>(a, inv_ab));
+        trans = b;
+    }
+    u64 acc[4] = {0, 0, 0, 0};
+    for (u32 pc = 0; pc < n_insns; pc++) {
+        const AirInsn in = env.insn(pc);
+        const u32 op = in.op_dst & 15u, dst = in.op_dst >> 4;
+        u32 v;
+        switch (op) {
+            case P3GPU_AIR_CONST: v = in.arg; break;
+            case P3GPU_AIR_MAIN_LOCAL: v = env.local(in.arg); break;
+            case P3GPU_AIR_MAIN_NEXT: v = env.next(in.arg); break;
+            case P3GPU_AIR_PUBLIC: v = env.pub(in.arg); break;
+            case P3GPU_AIR_IS_FIRST_ROW: v = first; break;
+            case P3GPU_AIR_IS_LAST_ROW: v = last; break;
+            case P3GPU_AIR_IS_TRANSITION: v = trans; break;
+            case P3GPU_AIR_ADD: v = fp_add<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+            case P3GPU_AIR_SUB: v = fp_sub<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+            case P3GPU_AIR_NEG: v = fp_neg<F>(env.slot(in.arg)); break;
+            case P3GPU_AIR_MUL: v = mont_mul<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+            default:                                                    // AIR_OP_FOLD
+                air_qmac<F>(acc, env.slot(in.arg), env.apow(dst));
+                continue;
+        }
+        env.slot(dst) = v;
+    }
+    const u32 z = env.inv_zh(i);
+    return make_uint4(mont_mul<F>(mont_redc<F>(acc[0]), z), mont_mul<F>(mont_redc<F>(acc[1]), z), mont_mul<F>(mont_redc<F>(acc[2]), z),
+                      mont_mul<F>(mont_redc<F>(acc[3]), z));
+}
+
+// Host-side launch constants + tables: Z_H(x_i) and 1/Z_H(x_i) depend on i mod 2^q only (x^N = g^N w_q^(iN), w_q^N of order 2^q).
+template <int F> inline AirDomain air_domain(unsigned log_q, unsigned log_n, u32 uses, std::vector<u32> &zh, std::vector<u32> &inv_zh) {
+    AirDomain d;
+    d.log_q = log_q; d.q = log_q - log_n; d.uses = uses;
+    d.shift = to_monty<F>(Fp<F>::GEN);
+    d.w_q = two_adic_generator<F>(log_q);
+    d.w_n_inv = fp_inv<F>(two_adic_generator<F>(log_n));
+    const size_t nz = (size_t)1 << d.q;
+    zh.resize(nz); inv_zh.resize(nz);
+    const u32 s_pow_n = fp_pow<F>(d.shift, (u64)1 << log_n), wr = two_adic_generator<F>(d.q);
+    u32 wp = Fp<F>::ONE;
+    for (size_t j = 0; j < nz; j++) {
+        zh[j] = fp_sub<F>(mont_mul<F>(s_pow_n, wp), Fp<F>::ONE);
+        inv_zh[j] = fp_inv<F>(zh[j]);
+        wp = mont_mul<F>(wp, wr);
+    }
+    return d;
+}
+
+// alpha^(K - 1 - k) for k < K, as the kernel's shared table holds it
+template <int F> inline std::vector<uint4> air_alpha_table(const u32 alpha[4], u32 K) {
+    std::vector<uint4> t(K);
+    Ef4<F> cur, al;
+    cur.c[0] = Fp<F>::ONE; cur.c[1] = cur.c[2] = cur.c[3] = 0;
+    for (int j = 0; j < 4; j++) al.c[j] = alpha[j];
+    for (u32 j = 0; j < K; j++) {
+        t[K - 1 - j] = make_uint4(cur.c[0], cur.c[1], cur.c[2], cur.c[3]);
+        cur = ef_mul<F>(cur, al);
+    }
+    return t;
+}
+
+}  // namespace p3

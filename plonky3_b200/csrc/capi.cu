@@ -497,6 +497,26 @@ int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vecto
     return air_generate_trace_cols(ctx, field, vector_len, d_inputs, n_perms, col0, col1, d_out);
 }
 
+// ---- any AIR as a constraint program (air_program.cu) -------------------------------------------------
+int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                 size_t n_constraints, uint32_t width, uint32_t n_public, p3gpu_air_program **out) {
+    P3_ENTER(ctx);
+    P3_CHECK(out, P3GPU_EINVAL, "null argument");
+    *out = nullptr;
+    return air_program_create(ctx, field, nodes, n_nodes, constraints, n_constraints, width, n_public, out);
+}
+void p3gpu_air_program_destroy(p3gpu_air_program *prog) { air_program_destroy(prog); }
+int32_t p3gpu_air_program_info(const p3gpu_air_program *prog, size_t *n_instructions, size_t *n_slots, size_t *n_constraints) {
+    return air_program_info(prog, n_instructions, n_slots, n_constraints);
+}
+int32_t p3gpu_air_quotient_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_lde, unsigned log_lde_height,
+                               unsigned log_quotient_size, unsigned log_trace_height, const uint32_t *public_values, const uint32_t alpha[4],
+                               uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(prog && d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return air_program_quotient(ctx, prog, d_lde, log_lde_height, log_quotient_size, log_trace_height, public_values, alpha, d_quotient);
+}
+
 // ---- transcript + query phase (prove driver) ---------------------------------------------------------
 int32_t p3gpu_challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out) {
     P3_ENTER(ctx);

@@ -295,6 +295,29 @@ class Gpu:
         check(self.L.p3gpu_p2air_quotient_dev(self.h, field, vector_len, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    # ------------------------------------------------------------------ any AIR as a constraint program
+    def air_program_create(self, field, nodes, constraints, width, n_public):
+        """Compile an expression DAG: nodes (n, 4) uint32 rows (op, a, b, imm), constraints: node indices in assertion order.
+        Returns an AirProgramHandle (freed with the object)."""
+        nd = np.ascontiguousarray(nodes, dtype=np.uint32).reshape(-1, 4)
+        cs = np.ascontiguousarray(constraints, dtype=np.uint32).ravel()
+        h = C.c_void_p()
+        check(self.L.p3gpu_air_program_create(self.h, field, nd.ctypes.data, nd.shape[0], cs.ctypes.data, cs.size, width, n_public, C.byref(h)))
+        return AirProgramHandle(self.L, h)
+
+    def air_quotient(self, prog, lde_dev, log_quotient_size, log_trace_height, public_values, alpha):
+        """Quotient values (2^log_quotient_size, 4) in natural order over GENERATOR * K from the first 2^log_quotient_size rows of the
+        committed bit-reversed LDE.  public_values: Montgomery words."""
+        m = self._dev(lde_dev); self._use_torch_stream()
+        H = int(m.shape[0]); log_h = H.bit_length() - 1
+        if H != 1 << log_h:
+            raise _lib.P3GpuError(f"LDE height {H} is not a power of two", _lib.EINVAL)
+        pv = np.ascontiguousarray(public_values, dtype=np.uint32).ravel()
+        q = self._empty((1 << log_quotient_size, 4))
+        check(self.L.p3gpu_air_quotient_dev(self.h, prog.h, m.data_ptr(), log_h, log_quotient_size, log_trace_height,
+                                            pv.ctypes.data if pv.size else None, self._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
+
     def pcs_commit_host(self, field, hash_kind, evals_host, log_blowup, cap_height):
         """p3gpu_pcs_commit: TwoAdicFriPcs::commit with the trace in HOST memory (numpy uint32 array or pinned CPU int32 tensor);
         the LDE and the digest layers stay on the device, only the cap returns.  Returns (cap (n, 8) array, lde, layers)."""
@@ -315,6 +338,26 @@ class Gpu:
         for k in range(nl.value):
             layers.append(out[off:off + lens[k]]); off += lens[k]
         return cap[: cap_len.value].copy(), lde, layers
+
+
+class AirProgramHandle:
+    """A compiled constraint program (p3gpu_air_program); `info()` -> (instructions, slots, constraints)."""
+
+    def __init__(self, L, h):
+        self.L, self.h = L, h
+
+    def info(self):
+        n = [C.c_size_t() for _ in range(3)]
+        check(self.L.p3gpu_air_program_info(self.h, *[C.byref(v) for v in n]))
+        return tuple(int(v.value) for v in n)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self.L.p3gpu_air_program_destroy(self.h)
+                self.h = None
+        except Exception:
+            pass
 
 
 _default = {}

@@ -1,9 +1,10 @@
-"""uni-stark `prove` for the Poseidon2 AIR with every data-parallel step on the GPU — the BASELINE config-5 benchmark
+"""uni-stark `prove` with every data-parallel step on the GPU, for the Poseidon2 AIR — the BASELINE config-5 benchmark
 (`prove_prime_field_31 --field koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel
 -m poseidon-2`).  Mirrors uni-stark/src/prover.rs:87-442 (prove_with_preprocessed) and fri/src/prover.rs:43-160 (prove_fri) with
 the reference's names; host code is only the protocol sequencing (the transcript's sponge itself runs on the device,
 challenger.py).  Non-ZK, no preprocessed columns, no public values — what the example binary proves
-(examples/src/proofs.rs:120-170).
+(examples/src/proofs.rs:120-170) — and for any AIR given as symbolic constraints (air.SymbolicAir: public values, next-row
+openings, any number of quotient chunks up to the blowup), whose quotient is p3gpu_air_quotient_dev.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
     alpha <- transcript;  quotient values on GENERATOR * K ................... p3gpu_p2air_quotient_dev
@@ -129,8 +130,9 @@ class VectorizedPoseidon2Air:
         self._upload()
         return self.gpu.p2air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1), self.vector_len)
 
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha):
+    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=()):
         """uni-stark/src/prover.rs:462-827 on the committed LDE (natural order over the quotient domain)."""
+        assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
         if self.gpu is None:
             raise _lib.P3GpuError("quotient evaluation needs a GPU context (no CPU fallback)")
         self._upload()
@@ -186,9 +188,11 @@ def verify(config: StarkConfig, air, proof, public_values=()):
     return _verify(config, air, proof, public_values)
 
 
-def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values=()) -> Proof:
-    """uni-stark/src/prover.rs:87-442.  `trace`: device (CUDA int32) matrix of height 2^n."""
+def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
+    """uni-stark/src/prover.rs:87-442.  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device (CUDA int32) matrix of
+    height 2^n.  `public_values`: canonical integers."""
     import torch
+    from . import extension as X
     pcs, f, gpu = config.pcs, config.pcs.dft.field, config.pcs.dft.gpu
     sync = torch.cuda.synchronize
     T = {}
@@ -196,12 +200,20 @@ def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values
     def span(name, t0):
         sync(); T[name] = (time.perf_counter() - t0) * 1e3
 
-    assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
+    public_values = [int(v) for v in public_values]
+    if len(public_values) != air.num_public_values():
+        raise ValueError(f"{len(public_values)} public values given, the AIR has {air.num_public_values()}")
+    if int(trace.shape[1]) != air.width():
+        raise ValueError(f"trace width {int(trace.shape[1])} differs from the AIR width {air.width()}")
     degree = int(trace.shape[0])
     log_degree = _log2_strict(degree)
     log_num_quotient_chunks = get_log_num_quotient_chunks(air)
     num_quotient_chunks = 1 << log_num_quotient_chunks
-    assert log_num_quotient_chunks == pcs.fri.log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
+    if log_num_quotient_chunks > pcs.fri.log_blowup:
+        # the quotient domain must lie inside the committed LDE (fast path of get_evaluations_on_domain); the reference asserts too
+        raise ValueError(f"constraint degree {air.max_constraint_degree()} needs {num_quotient_chunks} quotient chunks: log_blowup "
+                         f"{pcs.fri.log_blowup} < {log_num_quotient_chunks}")
+    opens_next = len(air.main_next_row_columns()) > 0
     challenger = config.initialise_challenger()
     trace_domain = pcs.natural_domain_for_degree(degree)
 
@@ -213,12 +225,14 @@ def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values
     challenger.observe_canonical(log_degree)                                             # log_degree                    :225
     challenger.observe_canonical(0)                                                      # preprocessed_width            :226
     challenger.observe_cap(trace_commit)                                                 # :230
+    for v in public_values:                                                              # :236
+        challenger.observe_canonical(v)
     alpha = challenger.sample_algebra_element()                                          # :258
 
     t0 = time.perf_counter()
     quotient_domain = (f.mul(trace_domain[0], f.generator), log_degree + log_num_quotient_chunks)      # create_disjoint_domain
     trace_on_quotient_domain = pcs.get_evaluations_on_domain(trace_data, 0, quotient_domain).bit_reverse_rows()
-    quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha)    # (2N, 4) natural order = flatten_to_base
+    quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)    # natural order = flatten_to_base
     span("compute quotient polynomial", t0)
 
     t0 = time.perf_counter()
@@ -228,7 +242,10 @@ def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values
 
     zeta = challenger.sample_algebra_element()                                           # :365
     t0 = time.perf_counter()
-    rounds = [(trace_data, [[zeta]]), (quotient_data, [[zeta]] * num_quotient_chunks)]   # main_next_row_columns() is empty: zeta only
+    trace_points = [zeta]
+    if opens_next:                                                                       # zeta * omega_N (trace_domain.next_point)
+        trace_points.append(X.ef_scale(f, np.asarray(zeta, dtype=np.uint32), f.two_adic_generator(log_degree)))
+    rounds = [(trace_data, [trace_points]), (quotient_data, [[zeta]] * num_quotient_chunks)]
     opened_values, fri_inputs = pcs.open_values_and_fri_inputs(rounds, challenger)
     span("open: evaluate + reduce", t0)
 
@@ -241,7 +258,7 @@ def prove(config: StarkConfig, air: VectorizedPoseidon2Air, trace, public_values
                  commit_pow_witnesses=fri["pow_witnesses"], final_poly=fri["final_poly"], query_pow_witness=fri["query_pow_witness"],
                  query_indices=fri["indices"], input_openings=fri["input_openings"], commit_phase_openings=fri["commit_phase_openings"],
                  degree_bits=log_degree, timings_ms=T, input_opening_indices=fri["input_opening_indices"],
-                 commit_phase_indices=fri["commit_phase_indices"])
+                 commit_phase_indices=fri["commit_phase_indices"], trace_next=opened_values[0][0][1] if opens_next else None)
 
 
 def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list,

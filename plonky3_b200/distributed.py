@@ -127,6 +127,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
+from . import extension as X
 from ._lib import check
 
 
@@ -377,23 +378,100 @@ def _bitrev(x, bits: int):
     return r
 
 
-class _ShardedTraceMmcs:
-    """The trace batch's Mmcs::open_multi_batch when its rows are spread over the ranks: every rank gathers the rows and
-    authentication paths of the queries it owns (rank idx // R, local row idx % R), the tables are all-gathered over peer
-    memory, and every rank takes each answer from its owner's slot.  The path's levels inside a sub-tree come from the owner's
-    sub-tree; the levels above it (cap_height < log2(world)) from the tree over the sub-tree roots that the commit left in the
-    control block."""
+class ShardedTrace:
+    """The trace's prover data and its opener when the trace's columns are split over the ranks of a PeerGroup: rank g holds
+    columns [col_starts[g], col_starts[g+1]), and after the sharded commit LDE rows [g R, (g+1) R), R = LDE height / world, with
+    its sub-tree.  `uni_stark.prove(config, air, block, shard=ShardedTrace(grp, col_starts))` proves the Poseidon2 AIR with it.
 
-    def __init__(self, grp: "PeerGroup", sub_layers, top_layers, log_height: int, cap_height: int):
-        self.grp, self.sub_layers, self.top_layers = grp, sub_layers, top_layers
-        self.log_height, self.height = log_height, 1 << log_height
-        self.path_len = log_height - min(cap_height, log_height)
+    It carries out the steps that read the trace's rows.  Ranks exchange data over peer memory only where a value depends on rows
+    they do not own, and after every exchange all ranks hold identical bytes, so their transcripts stay identical:
+      commit, quotient_values           prove's two branches: the sharded commit; the sharded quotient kernel on the own rows;
+      low_coset_dot, reduce_rows        the two per-matrix steps of TwoAdicFriPcs.open_values_and_fri_inputs (fri._row_steps);
+      get_max_height, open_multi_batch  the trace's query openings in prove_fri."""
+
+    def __init__(self, grp: "PeerGroup", col_starts):
+        self.grp, self.col_starts = grp, [int(x) for x in col_starts]
+        self.width = self.col_starts[-1]
+
+    def commit(self, pcs, trace_block):
+        """PeerGroup.commit of my column block.  Returns (cap, prover data = self); the cap is identical on every rank."""
+        from .dft import _log2_strict
+        grp, mmcs, gpu = self.grp, pcs.mmcs, self.grp.gpu
+        self.field, self.gpu = pcs.dft.field, gpu
+        self.log_degree = _log2_strict(int(trace_block.shape[0]))
+        self.log_height = self.log_degree + pcs.fri.log_blowup
+        H, W, world = 1 << self.log_height, self.width, grp.world
+        self.shape, self.device = (H, W), f"cuda:{gpu.device}"
+        for p in mmcs.perms:
+            p.upload(gpu)
+        grp.ensure_exchange(4 * max(H * 4, world * W * 4, world * pcs.fri.num_queries * (W + 8 * self.log_height)))
+        cap, self.sub_layers, _ = grp.commit(self.field, mmcs.hash_kind, trace_block, self.col_starts, pcs.fri.log_blowup, mmcs.cap_height)
+        flat, R = grp.rows_tensor().reshape(-1), grp.rows_per_rank
+        self.segments = [(c0, c1, flat[off:off + R * (c1 - c0)].reshape(R, c1 - c0)) for c0, c1, off in grp.column_segments()]
+        log_g = world.bit_length() - 1
+        self.top_layers = []
+        if mmcs.cap_height < log_g:                  # the tree over the sub-tree roots, as the commit left it in the control block
+            user = grp.ctrl.tensor((_lib.PEER_CTRL_BYTES // 4,))[_lib.PEER_CTRL_USER // 4:].cpu().numpy().view(np.uint32)
+            off = world * 8
+            for lvl in range(log_g):
+                n = world >> lvl
+                self.top_layers.append(user[off:off + n * 8].reshape(n, 8).copy()); off += n * 8
+        self.path_len = self.log_height - min(mmcs.cap_height, self.log_height)
+        return cap, self
+
+    def quotient_values(self, air, quotient_domain, alpha):
+        """The Poseidon2 AIR's quotient values in natural order over the quotient domain, which must be the LDE domain: the sharded
+        kernel on my rows in place, the bit-reversed slices all-gathered and put back in natural order by one gather."""
+        assert quotient_domain[1] == self.log_height, "the sharded quotient covers the LDE domain: log_num_quotient_chunks == log_blowup"
+        H = self.shape[0]
+        q_slice = self.grp.p2air_quotient(self.field, air.vector_len, self.log_height, self.log_degree, alpha)
+        q_bitrev = self.grp.exchange(q_slice).reshape(H, 4)
+        return q_bitrev[_bitrev(torch.arange(H, device=self.device, dtype=torch.int64), self.log_height)].contiguous()
+
+    def get_matrices(self, _data):
+        return [self]
+
+    def low_coset_dot(self, h, weights, scale):
+        """columnwise_dot over the first h rows: each rank's unscaled partial over the rows it owns, all-gathered, summed with
+        ef_axpy and scaled.  Field addition is exact, so the result equals the single-GPU value bit for bit."""
+        grp, gpu, f = self.grp, self.gpu, self.field
+        W, R = self.width, grp.rows_per_rank
+        row0 = grp.rank * R
+        partial = torch.zeros((W, 4), dtype=torch.int32, device=self.device)
+        used = min(R, h - row0)
+        if used > 0:
+            for c0, c1, block in self.segments:
+                partial[c0:c1] = gpu.columnwise_dot(f.id, block[:used], weights[row0:row0 + used])
+        parts = grp.exchange(partial.reshape(-1)).reshape(grp.world, W, 4)
+        acc = torch.zeros((W, 4), dtype=torch.int32, device=self.device)
+        for q in range(grp.world):
+            gpu.ef_axpy(f.id, acc, parts[q], X.ef_one(f))
+        ys = torch.zeros((W, 4), dtype=torch.int32, device=self.device)
+        gpu.ef_axpy(f.id, ys, acc, scale)
+        return ys
+
+    def reduce_rows(self, acc, alpha, terms, coeff_and_yred):
+        """The trace's reduced openings over my rows: rowwise_dot per column segment times alpha^(first column), open_reduce of
+        every term into my row slice of `acc`, then that slice all-gathered over the whole of `acc`."""
+        grp, gpu, f = self.grp, self.gpu, self.field
+        R = grp.rows_per_rank
+        mine = slice(grp.rank * R, (grp.rank + 1) * R)
+        r = torch.zeros((R, 4), dtype=torch.int32, device=self.device)
+        for c0, c1, block in self.segments:
+            gpu.ef_axpy(f.id, r, gpu.rowwise_dot(f.id, block, alpha), X.ef_pow(f, alpha, c0))
+        for inv_denoms, offset, ys in terms:
+            gpu.open_reduce(f.id, acc[mine], r, inv_denoms[mine], *coeff_and_yred(offset, ys))
+        acc.copy_(grp.exchange(acc[mine]).reshape(acc.shape))
 
     def get_max_height(self, _data):
-        return self.height
+        return self.shape[0]
 
     def open_multi_batch(self, indices, _data):
-        grp, gpu = self.grp, self.grp.gpu
+        """Mmcs::open_multi_batch: every rank gathers the rows and authentication paths of the queries it owns (rank idx // R,
+        local row idx % R), the tables are all-gathered over peer memory, and every rank takes each answer from its owner's slot.
+        The path's levels inside a sub-tree come from the owner's sub-tree; the levels above it (cap_height < log2(world)) from
+        the tree over the sub-tree roots that the commit left in the control block."""
+        grp, gpu = self.grp, self.gpu
         R, W, rank = grp.rows_per_rank, grp.w_total, grp.rank
         log_r = R.bit_length() - 1
         idx = np.asarray(indices, dtype=np.int64)
@@ -402,16 +480,15 @@ class _ShardedTraceMmcs:
         owner, local = idx // R, idx % R
         mine = np.nonzero(owner == rank)[0]
         rec = W + plen * 8
-        table = torch.zeros((n, rec), dtype=torch.int32, device=f"cuda:{gpu.device}")
+        table = torch.zeros((n, rec), dtype=torch.int32, device=self.device)
         if mine.size:
             li = np.ascontiguousarray(local[mine], dtype=np.uint32)
             mine = torch.from_numpy(mine).to(table.device)
             k = int(li.size)
-            flat = grp.rows_tensor().reshape(-1)
             gpu._use_torch_stream()
-            for c0, c1, off in grp.column_segments():
+            for c0, c1, block in self.segments:
                 piece = gpu._empty((k, c1 - c0))
-                check(gpu.L.p3gpu_gather_rows_dev(gpu.h, flat[off:].data_ptr(), R, c1 - c0, li.ctypes.data, k, 0, piece.data_ptr()))
+                check(gpu.L.p3gpu_gather_rows_dev(gpu.h, block.data_ptr(), R, c1 - c0, li.ctypes.data, k, 0, piece.data_ptr()))
                 table[mine, c0:c1] = piece
             if sub_len:
                 lay = self.sub_layers
@@ -429,141 +506,17 @@ class _ShardedTraceMmcs:
 
 def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
     """uni_stark.prove of the Poseidon2 AIR with the trace sharded by column block over the ranks of `grp` (rank g holds columns
-    [col_starts[g], col_starts[g+1]) of the 2^n-row trace).  Every rank returns the same Proof, byte for byte the one
-    `uni_stark.prove` writes for the whole trace on one GPU.
-
-    Each rank runs its own device challenger; ranks exchange data (over peer memory, no collective library) only where a
-    value depends on rows they do not own, and after every exchange all ranks hold identical bytes, so the transcripts stay
-    identical.  trace commit: PeerGroup.commit (rank g keeps LDE rows [g R, (g+1) R), R = 2N / world); quotient: evaluated
-    on the own row block in place, slices all-gathered, committed redundantly; opened values at zeta: partial column-wise dots
-    over the first coset's rows, all-gathered and summed; reduced openings of the trace: over the own rows, all-gathered;
-    FRI: redundantly on every rank; trace query openings: answered by the owner rank and all-gathered."""
-    import time
-    from . import extension as X
-    from .dft import _log2_strict
-    from .uni_stark import Proof, get_log_num_quotient_chunks, prove_fri
-    pcs, mmcs = config.pcs, config.pcs.mmcs
-    f, gpu = pcs.dft.field, grp.gpu
-    assert gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
+    [col_starts[g], col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  Every rank returns the same Proof, byte for
+    byte the one `uni_stark.prove` writes for the whole trace on one GPU; its timings_ms are each span's maximum over the ranks."""
+    from .uni_stark import VectorizedPoseidon2Air, get_log_num_quotient_chunks, prove
+    pcs = config.pcs
+    assert grp.gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
+    assert isinstance(air, VectorizedPoseidon2Air), "the sharded quotient kernel evaluates the Poseidon2 AIR only"
     assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
-    starts = [int(x) for x in col_starts]
-    world, rank, R, W = grp.world, grp.rank, grp.rows_per_rank, grp.w_total
-    assert starts[-1] == W == air.width(), "column blocks must cover the AIR's width"
-    degree = int(trace_block.shape[0])
-    log_degree = _log2_strict(degree)
-    log_blowup = pcs.fri.log_blowup
-    log_num_quotient_chunks = get_log_num_quotient_chunks(air)
-    num_quotient_chunks = 1 << log_num_quotient_chunks
-    assert log_num_quotient_chunks == log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
-    H, log_h = degree << log_blowup, log_degree + log_blowup
-    assert R * world == H
-    dev = f"cuda:{gpu.device}"
-    sync = torch.cuda.synchronize
-    T = {}
-
-    def span(name, t0):
-        sync(); T[name] = (time.perf_counter() - t0) * 1e3
-
-    for p in mmcs.perms:
-        p.upload(gpu)
-    nq = pcs.fri.num_queries
-    grp.ensure_exchange(4 * max(H * 4, world * W * 4, world * nq * (W + 8 * log_h)))
-    challenger = config.initialise_challenger()
-    trace_domain = pcs.natural_domain_for_degree(degree)
-
-    t0 = time.perf_counter()
-    trace_commit, sub_layers, _ = grp.commit(f, mmcs.hash_kind, trace_block, starts, log_blowup, mmcs.cap_height)
-    span("commit to trace data", t0)
-    log_g = world.bit_length() - 1
-    top_layers = []
-    if mmcs.cap_height < log_g:                      # the tree over the sub-tree roots, as the commit left it in the control block
-        user = grp.ctrl.tensor((_lib.PEER_CTRL_BYTES // 4,))[_lib.PEER_CTRL_USER // 4:].cpu().numpy().view(np.uint32)
-        off = world * 8
-        for lvl in range(log_g):
-            n = world >> lvl
-            top_layers.append(user[off:off + n * 8].reshape(n, 8).copy()); off += n * 8
-
-    challenger.observe_canonical(log_degree)
-    challenger.observe_canonical(log_degree)
-    challenger.observe_canonical(0)
-    challenger.observe_cap(trace_commit)
-    alpha = challenger.sample_algebra_element()
-
-    t0 = time.perf_counter()
-    quotient_domain = (f.mul(trace_domain[0], f.generator), log_h)
-    q_slice = grp.p2air_quotient(f, air.vector_len, log_h, log_degree, alpha)
-    q_bitrev = grp.exchange(q_slice).reshape(H, 4)
-    perm = _bitrev(torch.arange(H, device=dev, dtype=torch.int64), log_h)
-    quotient_flat = q_bitrev[perm].contiguous()      # natural order
-    span("compute quotient polynomial", t0)
-
-    t0 = time.perf_counter()
-    quotient_commit, quotient_data = pcs.commit_quotient(quotient_domain, quotient_flat, num_quotient_chunks)
-    span("commit to quotient poly chunks", t0)
-    challenger.observe_cap(quotient_commit)
-    zeta = challenger.sample_algebra_element()
-
-    t0 = time.perf_counter()
-    z = np.asarray([int(v) for v in zeta], dtype=np.uint32)
-    inv_denoms, adjusted = gpu.open_inv_denoms(f.id, log_h, z, X.ef_inv(f, z))
-    g_pow_n = f.pow(f.generator, degree)
-    denom_inv = f.inv(f.mul(g_pow_n, f.to_monty(degree)))
-    scal = X.ef_scale(f, X.ef_mul(f, z, X.ef_sub(f, X.ef_pow(f, z, degree), X.ef_from_base(f, g_pow_n))), denom_inv)
-    one = X.ef_one(f)
-    flat = grp.rows_tensor().reshape(-1)
-    segs = grp.column_segments()
-    chunk = lambda c0, c1, off: flat[off:off + R * (c1 - c0)].reshape(R, c1 - c0)
-    row0 = rank * R
-    # trace values at zeta: barycentric sum over the first coset's rows (memory rows [0, N)), split by owner
-    partial = torch.zeros((W, 4), dtype=torch.int32, device=dev)
-    used = min(R, degree - row0)
-    if used > 0:
-        for c0, c1, off in segs:
-            partial[c0:c1] = gpu.columnwise_dot(f.id, chunk(c0, c1, off)[:used], adjusted[row0:row0 + used])
-    parts = grp.exchange(partial.reshape(-1)).reshape(world, W, 4)
-    acc = torch.zeros((W, 4), dtype=torch.int32, device=dev)
-    for q in range(world):
-        gpu.ef_axpy(f.id, acc, parts[q], one)
-    trace_ys = torch.zeros((W, 4), dtype=torch.int32, device=dev)
-    gpu.ef_axpy(f.id, trace_ys, acc, scal)
-    challenger.observe_algebra_slice(trace_ys)
-    q_mats = mmcs.get_matrices(quotient_data)
-    q_ys = []
-    for m in q_mats:
-        ys = gpu.columnwise_dot(f.id, m[:int(m.shape[0]) >> log_blowup], adjusted, scal)
-        challenger.observe_algebra_slice(ys)
-        q_ys.append(ys)
-    alpha2 = np.asarray(challenger.sample_algebra_element(), dtype=np.uint32)
-
-    def yred_of(ys):
-        return X.ef_from_basis_rows(f, gpu.rowwise_dot(f.id, ys.t().contiguous(), alpha2).cpu().numpy().view(np.uint32))
-    # reduced openings: the trace's term over my rows (row-wise dot per column segment, shifted by alpha^(first column)) ...
-    r_local = torch.zeros((R, 4), dtype=torch.int32, device=dev)
-    for c0, c1, off in segs:
-        gpu.ef_axpy(f.id, r_local, gpu.rowwise_dot(f.id, chunk(c0, c1, off), alpha2), X.ef_pow(f, alpha2, c0))
-    red_local = torch.zeros((R, 4), dtype=torch.int32, device=dev)
-    gpu.open_reduce(f.id, red_local, r_local, inv_denoms[row0:row0 + R], X.ef_pow(f, alpha2, 0), yred_of(trace_ys))
-    reduced = grp.exchange(red_local).reshape(H, 4).clone()
-    # ... and the quotient chunks' terms, locally on the full height
-    num_reduced = W
-    for m, ys in zip(q_mats, q_ys):
-        gpu.open_reduce(f.id, reduced, gpu.rowwise_dot(f.id, m, alpha2), inv_denoms, X.ef_pow(f, alpha2, num_reduced), yred_of(ys))
-        num_reduced += int(m.shape[1])
-    span("open: evaluate + reduce", t0)
-
-    t0 = time.perf_counter()
-    trace_view = _ShardedTraceMmcs(grp, sub_layers, top_layers, log_h, mmcs.cap_height)
-    rounds = [(None, [[zeta]]), (quotient_data, [[zeta]] * num_quotient_chunks)]
-    fri = prove_fri(pcs, [reduced], challenger, rounds, input_mmcs=[trace_view, mmcs])
-    span("open: FRI", t0)
-
-    if world > 1 and dist.is_initialized():
-        every = [None] * world
-        dist.all_gather_object(every, T, group=grp.group)
-        T = {k: max(t[k] for t in every) for k in T}
-    return Proof(trace_commit=trace_commit, quotient_commit=quotient_commit, trace_local=trace_ys.cpu().numpy().view(np.uint32),
-                 quotient_chunks=[ys.cpu().numpy().view(np.uint32) for ys in q_ys], commit_phase_commits=fri["commits"],
-                 commit_pow_witnesses=fri["pow_witnesses"], final_poly=fri["final_poly"], query_pow_witness=fri["query_pow_witness"],
-                 query_indices=fri["indices"], input_openings=fri["input_openings"], commit_phase_openings=fri["commit_phase_openings"],
-                 degree_bits=log_degree, timings_ms=T, input_opening_indices=fri["input_opening_indices"],
-                 commit_phase_indices=fri["commit_phase_indices"])
+    assert get_log_num_quotient_chunks(air) == pcs.fri.log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
+    proof = prove(config, air, trace_block, shard=ShardedTrace(grp, col_starts))
+    if grp.world > 1 and dist.is_initialized():
+        every = [None] * grp.world
+        dist.all_gather_object(every, proof.timings_ms, group=grp.group)
+        proof.timings_ms = {k: max(t[k] for t in every) for k in proof.timings_ms}
+    return proof

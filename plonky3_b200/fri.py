@@ -143,6 +143,27 @@ def split_evals(num_chunks: int, evals):
     return [evals[c::num_chunks].contiguous() if _is_torch(evals) else np.ascontiguousarray(evals[c::num_chunks]) for c in range(num_chunks)]
 
 
+def _row_steps(gpu, f: Field, mmcs, m):
+    """The two steps of TwoAdicFriPcs.open_values_and_fri_inputs that read matrix `m`'s rows:
+      low_coset_dot(h, weights, scale)                the opened values at one point: the weighted sum of the first h rows, scaled;
+      reduce_rows(acc, alpha, terms, coeff_and_yred)  the reduced openings of `m` at each (1/(z - x), alpha offset, opened values)
+                                                      of `terms`, added into the height's accumulator `acc`; coeff_and_yred(offset,
+                                                      opened values) gives open_reduce's alpha^offset and Mred(z).
+    An opener whose matrix rows are spread over ranks (distributed.ShardedTrace) supplies both; any other matrix is whole on this
+    device."""
+    if hasattr(mmcs, "reduce_rows"):
+        return mmcs.low_coset_dot, mmcs.reduce_rows
+
+    def low_coset_dot(h, weights, scale):
+        return gpu.columnwise_dot(f.id, m[:h], weights, scale)
+
+    def reduce_rows(acc, alpha, terms, coeff_and_yred):
+        r = gpu.rowwise_dot(f.id, m, alpha)                                  # Mred(x) for every row
+        for inv_denoms, offset, ys in terms:
+            gpu.open_reduce(f.id, acc, r, inv_denoms, *coeff_and_yred(offset, ys))
+    return low_coset_dot, reduce_rows
+
+
 class TwoAdicFriPcs:
     """TwoAdicFriPcs<Val, Dft, InputMmcs, FriMmcs> — commit side (two_adic_pcs.rs:261-363)."""
 
@@ -186,24 +207,27 @@ class TwoAdicFriPcs:
                 raise ValueError(f"committed LDE height {lde.shape[0]} is smaller than the blowup factor {min_height}")
         return self.mmcs.commit(ldes)
 
-    def open_values_and_fri_inputs(self, data_with_points: list, challenger):
+    def open_values_and_fri_inputs(self, data_with_points: list, challenger, input_mmcs: Optional[list] = None):
         """The pre-FRI part of TwoAdicFriPcs::open (two_adic_pcs.rs:413-662) with the LDEs resident on the device.
 
         data_with_points: list of (prover_data, points_per_matrix) — prover_data a MerkleTree whose leaves are CUDA matrices
         (committed bit-reversed LDEs), points_per_matrix[i] the EF4 points (4 Montgomery words each) matrix i is opened at.
+        `input_mmcs[k]` (default self.mmcs) holds round k's matrices, as in prove_fri; see `_row_steps` for an opener whose
+        rows are spread over ranks.
         challenger protocol: observe_algebra_slice(ys), sample_algebra_element().
         Returns (all_opened_values[round][matrix][point] -> (width, 4) array, fri_inputs: list of (len, 4) CUDA vectors in
         descending length — the `fri_input` handed to prove_fri / commit_phase)."""
         from . import extension as X
         import torch
         f, gpu = self.dft.field, self.dft.gpu
-        rounds = [(self.mmcs.get_matrices(data), points) for data, points in data_with_points]
-        for mats, points in rounds:
+        openers = input_mmcs or [self.mmcs] * len(data_with_points)
+        rounds = [(mmcs.get_matrices(data), points, mmcs) for (data, points), mmcs in zip(data_with_points, openers)]
+        for mats, points, _ in rounds:
             assert len(mats) == len(points), "each matrix should have a corresponding set of evaluation points"
-        log_global_max_height = _log2_strict(max(int(m.shape[0]) for mats, _ in rounds for m in mats))
+        log_global_max_height = _log2_strict(max(int(m.shape[0]) for mats, _, _ in rounds for m in mats))
         # compute_inverse_denominators (:743-780): one vector per unique point, for the tallest matrix opened there
         max_lh = {}
-        for mats, points in rounds:
+        for mats, points, _ in rounds:
             for m, pts in zip(mats, points):
                 for z in pts:
                     k = tuple(int(v) for v in z)
@@ -213,45 +237,51 @@ class TwoAdicFriPcs:
             z = np.array(k, dtype=np.uint32)
             inv_denoms[k], adjusted[k] = gpu.open_inv_denoms(f.id, lh, z, X.ef_inv(f, z))
         # opened values by barycentric interpolation of the low coset (:496-563; interpolation.rs:161-193).  The values stay on the
-        # device for the transcript (observed there) and for Mred(z); one small copy brings them back for the proof.
-        all_opened, opened_dev = [], []
-        for mats, points in rounds:
+        # device for the transcript (observed there) and for Mred(z); one small copy brings them back for the proof.  The scale is
+        # host arithmetic on the GPU's idle path after that copy, so it is computed once per (low coset size, point).
+        all_opened, opened_dev, scales = [], [], {}
+        for mats, points, mmcs in rounds:
             per_mat, per_mat_dev = [], []
             for m, pts in zip(mats, points):
                 h = int(m.shape[0]) >> self.fri.log_blowup
                 log_h = _log2_strict(h)
+                low_coset_dot, _ = _row_steps(gpu, f, mmcs, m)
                 per_pt, per_pt_dev = [], []
                 for z in pts:
                     k = tuple(int(v) for v in z)
-                    z = np.array(k, dtype=np.uint32)
-                    g_pow_n = f.pow(f.generator, h)
-                    denom_inv = f.inv(f.mul(g_pow_n, f.to_monty(h)))
-                    scal = X.ef_scale(f, X.ef_mul(f, z, X.ef_sub(f, X.ef_pow(f, z, 1 << log_h), X.ef_from_base(f, g_pow_n))), denom_inv)
-                    ys_dev = gpu.columnwise_dot(f.id, m[:h], adjusted[k], scal)
+                    if (h, k) not in scales:
+                        z = np.array(k, dtype=np.uint32)
+                        g_pow_n = f.pow(f.generator, h)
+                        denom_inv = f.inv(f.mul(g_pow_n, f.to_monty(h)))
+                        scales[h, k] = X.ef_scale(f, X.ef_mul(f, z, X.ef_sub(f, X.ef_pow(f, z, 1 << log_h), X.ef_from_base(f, g_pow_n))), denom_inv)
+                    ys_dev = low_coset_dot(h, adjusted[k], scales[h, k])
                     challenger.observe_algebra_slice(ys_dev)
                     per_pt_dev.append(ys_dev)
                     per_pt.append(ys_dev.cpu().numpy().view(np.uint32))
                 per_mat.append(per_pt); per_mat_dev.append(per_pt_dev)
             all_opened.append(per_mat); opened_dev.append(per_mat_dev)
         alpha = np.asarray(challenger.sample_algebra_element(), dtype=np.uint32)
+
+        def coeff_and_yred(offset, ys_dev):
+            coeff = X.ef_pow(f, alpha, offset)                                   # alpha_pow_offset
+            # Mred(z) = sum_i alpha^i y_i: the same row-wise dot kernel on the 4 coefficient rows of the opened values,
+            # recombined with the basis (1, X, X^2, X^3) on the host
+            yt = ys_dev.t().contiguous()                                         # (4, width)
+            return coeff, X.ef_from_basis_rows(f, gpu.rowwise_dot(f.id, yt, alpha).cpu().numpy().view(np.uint32))
         # reduced openings per height (:598-660)
         num_reduced, reduced = {}, {}
-        for (mats, points), opened_round in zip(rounds, opened_dev):
+        for (mats, points, mmcs), opened_round in zip(rounds, opened_dev):
             for m, pts, opened_mat in zip(mats, points, opened_round):
                 H = int(m.shape[0]); lh = _log2_strict(H)
                 if lh not in reduced:
                     reduced[lh] = torch.zeros((H, 4), dtype=torch.int32, device=m.device)
                     num_reduced[lh] = 0
-                r = gpu.rowwise_dot(f.id, m, alpha)                              # Mred(x) for every row
+                terms = []                                                       # (1/(z - x), alpha offset, opened values) per point
                 for z, ys_dev in zip(pts, opened_mat):
-                    k = tuple(int(v) for v in z)
-                    coeff = X.ef_pow(f, alpha, num_reduced[lh])                  # alpha_pow_offset
-                    # Mred(z) = sum_i alpha^i y_i: the same row-wise dot kernel on the 4 coefficient rows of the opened values,
-                    # recombined with the basis (1, X, X^2, X^3) on the host
-                    yt = ys_dev.t().contiguous()                                 # (4, width)
-                    yred = X.ef_from_basis_rows(f, gpu.rowwise_dot(f.id, yt, alpha).cpu().numpy().view(np.uint32))
-                    gpu.open_reduce(f.id, reduced[lh], r, inv_denoms[k], coeff, yred)
+                    terms.append((inv_denoms[tuple(int(v) for v in z)], num_reduced[lh], ys_dev))
                     num_reduced[lh] += int(m.shape[1])
+                _, reduce_rows = _row_steps(gpu, f, mmcs, m)
+                reduce_rows(reduced[lh], alpha, terms, coeff_and_yred)
         fri_inputs = [reduced[lh] for lh in sorted(reduced, reverse=True)]
         return all_opened, fri_inputs
 

@@ -4,7 +4,9 @@
 the reference's names; host code is only the protocol sequencing (the transcript's sponge itself runs on the device,
 challenger.py).  Non-ZK, no preprocessed columns, no public values — what the example binary proves
 (examples/src/proofs.rs:120-170) — and for any AIR given as symbolic constraints (air.SymbolicAir: public values, next-row
-openings, any number of quotient chunks up to the blowup), whose quotient is p3gpu_air_quotient_dev.
+openings, any number of quotient chunks up to the blowup), whose quotient is p3gpu_air_quotient_dev.  `prove` is the one
+protocol sequence: with `shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns
+split over several GPUs, the shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
     alpha <- transcript;  quotient values on GENERATOR * K ................... p3gpu_p2air_quotient_dev
@@ -188,9 +190,12 @@ def verify(config: StarkConfig, air, proof, public_values=()):
     return _verify(config, air, proof, public_values)
 
 
-def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
+def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> Proof:
     """uni-stark/src/prover.rs:87-442.  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device (CUDA int32) matrix of
-    height 2^n.  `public_values`: canonical integers."""
+    height 2^n.  `public_values`: canonical integers.
+
+    `shard`: a distributed.ShardedTrace when the trace's columns are split over ranks; `trace` is then this rank's column block,
+    and every rank returns the proof of the whole trace."""
     import torch
     from . import extension as X
     pcs, f, gpu = config.pcs, config.pcs.dft.field, config.pcs.dft.gpu
@@ -203,8 +208,9 @@ def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
     public_values = [int(v) for v in public_values]
     if len(public_values) != air.num_public_values():
         raise ValueError(f"{len(public_values)} public values given, the AIR has {air.num_public_values()}")
-    if int(trace.shape[1]) != air.width():
-        raise ValueError(f"trace width {int(trace.shape[1])} differs from the AIR width {air.width()}")
+    width = shard.width if shard is not None else int(trace.shape[1])
+    if width != air.width():
+        raise ValueError(f"trace width {width} differs from the AIR width {air.width()}")
     degree = int(trace.shape[0])
     log_degree = _log2_strict(degree)
     log_num_quotient_chunks = get_log_num_quotient_chunks(air)
@@ -218,7 +224,10 @@ def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
     trace_domain = pcs.natural_domain_for_degree(degree)
 
     t0 = time.perf_counter()
-    trace_commit, trace_data = pcs.commit([(trace_domain, trace)])                       # prover.rs:215
+    if shard is None:
+        trace_commit, trace_data = pcs.commit([(trace_domain, trace)])                   # prover.rs:215
+    else:
+        trace_commit, trace_data = shard.commit(pcs, trace)
     span("commit to trace data", t0)
 
     challenger.observe_canonical(log_degree)                                             # log_ext_degree (non-ZK)       :224
@@ -231,8 +240,11 @@ def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
 
     t0 = time.perf_counter()
     quotient_domain = (f.mul(trace_domain[0], f.generator), log_degree + log_num_quotient_chunks)      # create_disjoint_domain
-    trace_on_quotient_domain = pcs.get_evaluations_on_domain(trace_data, 0, quotient_domain).bit_reverse_rows()
-    quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)    # natural order = flatten_to_base
+    if shard is None:
+        trace_on_quotient_domain = pcs.get_evaluations_on_domain(trace_data, 0, quotient_domain).bit_reverse_rows()
+        quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)  # natural order = flatten_to_base
+    else:
+        quotient_flat = shard.quotient_values(air, quotient_domain, alpha)
     span("compute quotient polynomial", t0)
 
     t0 = time.perf_counter()
@@ -246,11 +258,12 @@ def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
     if opens_next:                                                                       # zeta * omega_N (trace_domain.next_point)
         trace_points.append(X.ef_scale(f, np.asarray(zeta, dtype=np.uint32), f.two_adic_generator(log_degree)))
     rounds = [(trace_data, [trace_points]), (quotient_data, [[zeta]] * num_quotient_chunks)]
-    opened_values, fri_inputs = pcs.open_values_and_fri_inputs(rounds, challenger)
+    input_mmcs = [shard or pcs.mmcs, pcs.mmcs]
+    opened_values, fri_inputs = pcs.open_values_and_fri_inputs(rounds, challenger, input_mmcs)
     span("open: evaluate + reduce", t0)
 
     t0 = time.perf_counter()
-    fri = prove_fri(pcs, fri_inputs, challenger, rounds)
+    fri = prove_fri(pcs, fri_inputs, challenger, rounds, input_mmcs)
     span("open: FRI", t0)
 
     return Proof(trace_commit=trace_commit, quotient_commit=quotient_commit, trace_local=opened_values[0][0][0],
@@ -264,7 +277,7 @@ def prove(config: StarkConfig, air, trace, public_values=()) -> Proof:
 def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list,
               input_mmcs: Optional[list] = None) -> dict:
     """fri/src/prover.rs:43-160.  `input_mmcs[k]` (default pcs.mmcs) opens input batch k: anything with get_max_height(data) and
-    open_multi_batch(indices, data), such as the row-sharded trace of distributed.prove_sharded."""
+    open_multi_batch(indices, data), such as the row-sharded trace distributed.ShardedTrace."""
     import torch
     params: FriParameters = pcs.fri
     f, gpu = pcs.dft.field, pcs.dft.gpu

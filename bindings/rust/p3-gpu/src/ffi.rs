@@ -37,6 +37,19 @@ pub const P3GPU_AIR_ADD: u32 = 7;
 pub const P3GPU_AIR_SUB: u32 = 8;
 pub const P3GPU_AIR_NEG: u32 = 9;
 pub const P3GPU_AIR_MUL: u32 = 10;
+pub const P3GPU_AIR_PREPROCESSED_LOCAL: u32 = 16;
+pub const P3GPU_AIR_PREPROCESSED_NEXT: u32 = 17;
+pub const P3GPU_AIR_PERIODIC: u32 = 18;
+
+/// `p3gpu_air_layout`: what a constraint program's leaves may read.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct P3GpuAirLayout {
+    pub width: u32,
+    pub n_public: u32,
+    pub preprocessed_width: u32,
+    pub n_periodic: u32,
+}
 
 pub const P3GPU_BABY_BEAR: i32 = 0;
 pub const P3GPU_KOALA_BEAR: i32 = 1;
@@ -160,11 +173,18 @@ unsafe extern "C" {
     // any AIR as a constraint program (symbolic expression DAG -> register program -> quotient kernel)
     pub fn p3gpu_air_program_create(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize, constraints: *const u32,
                                     n_constraints: usize, width: u32, n_public: u32, out: *mut *mut P3GpuAirProgram) -> i32;
+    pub fn p3gpu_air_program_create_layout(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize,
+                                           constraints: *const u32, n_constraints: usize, layout: *const P3GpuAirLayout,
+                                           out: *mut *mut P3GpuAirProgram) -> i32;
     pub fn p3gpu_air_program_destroy(prog: *mut P3GpuAirProgram);
     pub fn p3gpu_air_program_info(prog: *const P3GpuAirProgram, n_instructions: *mut usize, n_slots: *mut usize, n_constraints: *mut usize) -> i32;
     pub fn p3gpu_air_quotient_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, d_lde: *const u32, log_lde_height: c_uint,
                                   log_quotient_size: c_uint, log_trace_height: c_uint, public_values: *const u32, alpha: *const u32,
                                   d_quotient: *mut u32) -> i32;
+    pub fn p3gpu_air_quotient_layout_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, d_lde: *const u32, log_lde_height: c_uint,
+                                         d_pre_lde: *const u32, log_pre_lde_height: c_uint, d_periodic: *const u32,
+                                         log_periodic_rows: c_uint, log_quotient_size: c_uint, log_trace_height: c_uint,
+                                         public_values: *const u32, alpha: *const u32, d_quotient: *mut u32) -> i32;
 
     // DuplexChallenger with device-resident state
     pub fn p3gpu_challenger_new(ctx: *mut P3GpuCtx, field: c_int, width: c_int, rate: c_int, out: *mut *mut P3GpuChallenger) -> i32;

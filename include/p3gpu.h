@@ -230,7 +230,9 @@ int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vecto
  * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
  * (operands refer only to earlier nodes) plus the list of constrained nodes in assertion order.  The library compiles it once
  * into a register program; p3gpu_air_quotient_dev runs that program over the quotient domain (uni-stark/src/prover.rs:462-827).
- * Not supported: periodic or preprocessed columns, extension-field constraints, ZK. */
+ * Preprocessed columns (BaseAir::preprocessed_trace) and periodic columns (BaseAir::periodic_columns) are leaves of their own; a
+ * program that declares them is created with p3gpu_air_program_create_layout and evaluated with p3gpu_air_quotient_layout_dev.
+ * Not supported: extension-field constraints, ZK. */
 enum {
     P3GPU_AIR_CONST = 0,          /* imm: the constant, Montgomery word */
     P3GPU_AIR_MAIN_LOCAL = 1,     /* a: column of the current row */
@@ -242,16 +244,27 @@ enum {
     P3GPU_AIR_ADD = 7,            /* a + b */
     P3GPU_AIR_SUB = 8,            /* a - b */
     P3GPU_AIR_NEG = 9,            /* -a */
-    P3GPU_AIR_MUL = 10            /* a * b */
+    P3GPU_AIR_MUL = 10,           /* a * b */
+    /* node values 11-15 are unused (rejected as unknown ops) */
+    P3GPU_AIR_PREPROCESSED_LOCAL = 16,  /* a: preprocessed column of the current row */
+    P3GPU_AIR_PREPROCESSED_NEXT = 17,   /* a: preprocessed column of the next row (wraps at the end of the domain) */
+    P3GPU_AIR_PERIODIC = 18             /* a: periodic column index (builder.periodic_values()[a]) */
 };
 typedef struct { uint32_t op, a, b, imm; } p3gpu_air_node;
 typedef struct p3gpu_air_program p3gpu_air_program;
+/* What a program's leaves may read: main trace width, public values, preprocessed trace width, number of periodic columns. */
+typedef struct { uint32_t width, n_public, preprocessed_width, n_periodic; } p3gpu_air_layout;
 
 /* Validates and compiles.  P3GPU_EINVAL: a column >= width, a public index >= n_public, an operand that is not an earlier node, a
  * constraint that names no node, an unknown op, a constant >= p.  P3GPU_EUNSUPPORTED: a field other than BabyBear / KoalaBear, more
  * than 2048 constraints or more than 384 simultaneously live values (the message states the limit). */
 int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
                                  size_t n_constraints, uint32_t width, uint32_t n_public, p3gpu_air_program **out);
+/* As p3gpu_air_program_create, for a program whose leaves may also read preprocessed and periodic columns: P3GPU_EINVAL as above,
+ * and for a preprocessed column >= layout->preprocessed_width or a periodic index >= layout->n_periodic.
+ * p3gpu_air_program_create(..., width, n_public, out) is this call with {width, n_public, 0, 0}. */
+int32_t p3gpu_air_program_create_layout(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                        size_t n_constraints, const p3gpu_air_layout *layout, p3gpu_air_program **out);
 void p3gpu_air_program_destroy(p3gpu_air_program *prog);
 /* instruction count (computes + folds), slot count (the most values live at once) and constraint count; NULL outputs are skipped */
 int32_t p3gpu_air_program_info(const p3gpu_air_program *prog, size_t *n_instructions, size_t *n_slots, size_t *n_constraints);
@@ -259,10 +272,23 @@ int32_t p3gpu_air_program_info(const p3gpu_air_program *prog, size_t *n_instruct
  * of the committed bit-reversed trace LDE d_lde (2^log_lde_height rows, `width` columns): the fast path of get_evaluations_on_domain
  * (two_adic_pcs.rs:376-385).  log_trace_height <= log_quotient_size <= log_lde_height, log_quotient_size - log_trace_height <= 8.
  * public_values: n_public Montgomery words (host).  d_quotient: 2^log_quotient_size EF4 values in NATURAL order (what
- * p3gpu_p2air_quotient_dev writes). */
+ * p3gpu_p2air_quotient_dev writes).  P3GPU_EINVAL for a program created with preprocessed or periodic columns in its layout: use
+ * p3gpu_air_quotient_layout_dev. */
 int32_t p3gpu_air_quotient_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_lde, unsigned log_lde_height,
                                unsigned log_quotient_size, unsigned log_trace_height, const uint32_t *public_values, const uint32_t alpha[4],
                                uint32_t *d_quotient);
+/* p3gpu_air_quotient_dev for any program, with the preprocessed and periodic inputs its layout declares:
+ *   d_pre_lde    the committed bit-reversed preprocessed LDE (2^log_pre_lde_height >= 2^log_quotient_size rows, preprocessed_width
+ *                columns), read like the trace: current row bitrev(i), next row bitrev(i + 2^q); NULL iff preprocessed_width = 0
+ *   d_periodic   the periodic table, 2^log_periodic_rows rows x n_periodic columns, row-major: every column padded to the largest
+ *                period p_max by repetition and coset-LDE'd onto p_max * 2^q rows (q = log_quotient_size - log_trace_height) over
+ *                the shift GENERATOR^(2^log_quotient_size / (p_max * 2^q)), natural order (fri/src/periodic.rs); natural index i
+ *                reads row i mod 2^log_periodic_rows.  NULL iff n_periodic = 0; log_periodic_rows <= log_quotient_size.
+ * Every check happens before anything launches. */
+int32_t p3gpu_air_quotient_layout_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_lde, unsigned log_lde_height,
+                                      const uint32_t *d_pre_lde, unsigned log_pre_lde_height, const uint32_t *d_periodic,
+                                      unsigned log_periodic_rows, unsigned log_quotient_size, unsigned log_trace_height,
+                                      const uint32_t *public_values, const uint32_t alpha[4], uint32_t *d_quotient);
 
 /* ---- transcript and query phase of the prove driver (SURVEY.md 8f rank 4 / N1) ----------------------------------------
  * DuplexChallenger<F, Poseidon2<width>, width, rate> (challenger/src/duplex_challenger.rs:60-300) with its state resident on the

@@ -31,6 +31,7 @@ EXPORTS = [
     "p3gpu_peer_allgather_dev", "p3gpu_coset_lde_batch_sharded_dev", "p3gpu_commit_sharded_dev", "p3gpu_shard_chunk_bounds",
     "p3gpu_p2air_generate_trace_cols_dev", "p3gpu_shard_col_segments", "p3gpu_peer_exchange_dev", "p3gpu_p2air_quotient_sharded_dev",
     "p3gpu_air_program_create", "p3gpu_air_program_destroy", "p3gpu_air_program_info", "p3gpu_air_quotient_dev",
+    "p3gpu_air_program_create_layout", "p3gpu_air_quotient_layout_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -127,6 +128,8 @@ def load():
         "p3gpu_air_program_destroy": (None, [vp]),
         "p3gpu_air_program_info": (i32, [vp, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]),
         "p3gpu_air_quotient_dev": (i32, [vp, vp, vp, cu, cu, cu, vp, vp, vp]),
+        "p3gpu_air_program_create_layout": (i32, [vp, ci, vp, sz, vp, sz, vp, C.POINTER(vp)]),
+        "p3gpu_air_quotient_layout_dev": (i32, [vp, vp, vp, cu, vp, cu, vp, cu, cu, cu, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

@@ -15,7 +15,12 @@ carries the reference's `degree_multiple` (expression.rs:44-48).  The prover com
 (p3gpu_air_program_create) and evaluates the quotient there (p3gpu_air_quotient_dev); there is no CPU evaluation of the quotient.
 The verifier's constraint folder evaluates the same DAG at the out-of-domain point.
 
-Not offered: periodic and preprocessed columns, extension-field constraints (assert_zero_ext), ZK.
+Preprocessed columns (`preprocessed_trace=`, read as `b.preprocessed().local[c]` / `.next[c]`) are committed once by
+`uni_stark.setup_preprocessed`; periodic columns (`periodic_columns=[[v0, .., v_{p-1}], ..]`, read as `b.periodic_values()[k]`,
+each period a power of two) are evaluated on the quotient domain from a small table the AIR builds on the device
+(`periodic_table`, fri/src/periodic.rs).
+
+Not offered: extension-field constraints (assert_zero_ext), ZK.
 """
 from __future__ import annotations
 
@@ -28,6 +33,7 @@ from .field import Field
 
 # node ops (include/p3gpu.h P3GPU_AIR_*)
 CONST, MAIN_LOCAL, MAIN_NEXT, PUBLIC, IS_FIRST_ROW, IS_LAST_ROW, IS_TRANSITION, ADD, SUB, NEG, MUL = range(11)
+PREPROCESSED_LOCAL, PREPROCESSED_NEXT, PERIODIC = 16, 17, 18
 BINARY = (ADD, SUB, MUL)
 
 
@@ -67,8 +73,8 @@ class Expr:
 
 
 class _Row:
-    def __init__(self, g, op, width):
-        self.g, self.op, self.width = g, op, width
+    def __init__(self, g, op, width, what="the trace width"):
+        self.g, self.op, self.width, self.what = g, op, width, what
 
     def __len__(self): return self.width
 
@@ -76,7 +82,7 @@ class _Row:
         if isinstance(c, slice):
             return [self[k] for k in range(*c.indices(self.width))]
         if not 0 <= c < self.width:
-            raise IndexError(f"column {c} outside the trace width {self.width}")
+            raise IndexError(f"column {c} outside {self.what} {self.width}")
         return self.g._node(self.op, c)
 
 
@@ -85,6 +91,14 @@ class _Main:
 
     def __init__(self, g, width):
         self.local, self.next = _Row(g, MAIN_LOCAL, width), _Row(g, MAIN_NEXT, width)
+
+
+class _Preprocessed:
+    """builder.preprocessed(): `local[c]` (current row) and `next[c]` (next row) of the preprocessed trace."""
+
+    def __init__(self, g, width):
+        self.local = _Row(g, PREPROCESSED_LOCAL, width, "the preprocessed width")
+        self.next = _Row(g, PREPROCESSED_NEXT, width, "the preprocessed width")
 
 
 class _Ops:
@@ -106,6 +120,8 @@ class _Ops:
     def when_transition(self): return self.when(self._root.is_transition())
 
     def main(self): return self._root.main()
+    def preprocessed(self): return self._root.preprocessed()
+    def periodic_values(self): return self._root.periodic_values()
     def public_values(self): return self._root.public_values()
     def is_first_row(self): return self._root.is_first_row()
     def is_last_row(self): return self._root.is_last_row()
@@ -124,8 +140,9 @@ class _Filtered(_Ops):
 class SymbolicAirBuilder(_Ops):
     """Records an AIR's constraints as a hash-consed expression DAG (nodes in topological order)."""
 
-    def __init__(self, field: Field, width: int, num_public_values: int = 0):
+    def __init__(self, field: Field, width: int, num_public_values: int = 0, preprocessed_width: int = 0, num_periodic: int = 0):
         self.field, self.width, self.num_public = field, int(width), int(num_public_values)
+        self.preprocessed_width, self.num_periodic = int(preprocessed_width), int(num_periodic)
         self._root = self
         self.nodes: list = []          # (op, a, b, imm)
         self.degrees: list = []
@@ -140,7 +157,8 @@ class SymbolicAirBuilder(_Ops):
         i = self._memo.get(key)
         if i is None:
             d = self.degrees
-            deg = {MAIN_LOCAL: 1, MAIN_NEXT: 1, IS_FIRST_ROW: 1, IS_LAST_ROW: 1}.get(op, 0)      # degree_multiple
+            deg = {MAIN_LOCAL: 1, MAIN_NEXT: 1, IS_FIRST_ROW: 1, IS_LAST_ROW: 1, PREPROCESSED_LOCAL: 1, PREPROCESSED_NEXT: 1,
+                   PERIODIC: 1}.get(op, 0)                                                          # degree_multiple
             if op in (ADD, SUB):
                 deg = max(d[a], d[b])
             elif op == NEG:
@@ -159,6 +177,10 @@ class SymbolicAirBuilder(_Ops):
         return self._node(CONST, imm=self.field.to_monty(int(v) % self.field.P))
 
     def main(self): return _Main(self, self.width)
+    def preprocessed(self): return _Preprocessed(self, self.preprocessed_width)
+
+    def periodic_values(self):
+        return [self._node(PERIODIC, k) for k in range(self.num_periodic)]
 
     def public_values(self):
         return [self._node(PUBLIC, k) for k in range(self.num_public)]
@@ -177,13 +199,42 @@ class SymbolicAirBuilder(_Ops):
         return np.array(self.nodes, dtype=np.uint32).reshape(-1, 4)
 
 
+def _is_pow2(n: int) -> bool:
+    return n > 0 and n & (n - 1) == 0
+
+
+def periodic_column_error(periodic_columns, trace_length: int):
+    """check_periodic_column_lengths (uni-stark/src/verifier.rs:25-50): None, or why a column cannot be evaluated over a trace
+    of `trace_length` rows (a period that is not a power of two, or one longer than the trace)."""
+    for k, col in enumerate(periodic_columns):
+        p = len(col)
+        if not _is_pow2(p):
+            return f"periodic column {k}: period {p} is not a power of two"
+        if p > trace_length:
+            return f"periodic column {k}: period {p} exceeds the trace length {trace_length}"
+    return None
+
+
 class SymbolicAir:
-    """An AIR given by `eval_fn(builder)`, in the surface uni_stark.prove and verifier.verify read."""
+    """An AIR given by `eval_fn(builder)`, in the surface uni_stark.prove and verifier.verify read.
+
+    preprocessed_trace              (height, width) host (numpy uint32) or device matrix of Montgomery words: BaseAir::preprocessed_trace
+    preprocessed_next_row_columns   the preprocessed columns read on the next row (default: all, air/src/air.rs:138-140); empty means
+                                    the proof opens the preprocessed trace at zeta only
+    periodic_columns                list of columns of canonical values, each of a power-of-two length (its period)"""
 
     def __init__(self, field: Field, width: int, eval_fn: Callable, num_public_values: int = 0,
-                 main_next_row_columns: Optional[Sequence[int]] = None, max_constraint_degree: Optional[int] = None, gpu=None):
+                 main_next_row_columns: Optional[Sequence[int]] = None, max_constraint_degree: Optional[int] = None, gpu=None,
+                 preprocessed_trace=None, preprocessed_next_row_columns: Optional[Sequence[int]] = None,
+                 periodic_columns: Optional[Sequence[Sequence[int]]] = None):
         self.field, self.gpu = field, gpu
-        b = SymbolicAirBuilder(field, width, num_public_values)
+        self._pre_trace = preprocessed_trace
+        pre_width = int(preprocessed_trace.shape[1]) if preprocessed_trace is not None else 0
+        self._periodic = [[int(v) % field.P for v in col] for col in (periodic_columns or [])]
+        for k, col in enumerate(self._periodic):
+            if not _is_pow2(len(col)):
+                raise ValueError(f"periodic column {k}: period {len(col)} is not a power of two")
+        b = SymbolicAirBuilder(field, width, num_public_values, pre_width, len(self._periodic))
         eval_fn(b)
         self.builder = b
         self.nodes = b.node_array()
@@ -192,13 +243,26 @@ class SymbolicAir:
         self._next_cols = list(range(b.width)) if main_next_row_columns is None else [int(c) for c in main_next_row_columns]
         if not self._next_cols and any(n[0] == MAIN_NEXT for n in b.nodes):
             raise ValueError("the constraints read the next row but main_next_row_columns() is empty")
+        self._pre_next_cols = (list(range(pre_width)) if preprocessed_next_row_columns is None
+                               else [int(c) for c in preprocessed_next_row_columns])
+        if not self._pre_next_cols and any(n[0] == PREPROCESSED_NEXT for n in b.nodes):
+            raise ValueError("the constraints read the preprocessed next row but preprocessed_next_row_columns() is empty")
         self._degree_hint = max_constraint_degree
         self._program = None
+        self._periodic_tables = {}
 
     # ---- BaseAir / the degree the quotient is split by
     def width(self) -> int: return self.builder.width
     def num_public_values(self) -> int: return self.builder.num_public
     def main_next_row_columns(self): return list(self._next_cols)
+    def preprocessed_width(self) -> int: return self.builder.preprocessed_width
+    def preprocessed_trace(self): return self._pre_trace
+    def preprocessed_next_row_columns(self): return list(self._pre_next_cols)
+    def num_periodic_columns(self) -> int: return len(self._periodic)
+    def periodic_columns(self): return [list(c) for c in self._periodic]
+
+    def _has_layout(self) -> bool:
+        return self.preprocessed_width() > 0 or self.num_periodic_columns() > 0
 
     def constraint_degrees(self):
         return [self.builder.degrees[c] for c in self.builder.constraints]
@@ -214,23 +278,61 @@ class SymbolicAir:
         if self.gpu is None:
             raise _lib.P3GpuError("quotient evaluation needs a GPU context (no CPU fallback)")
         if self._program is None:
-            self._program = self.gpu.air_program_create(self.field.id, self.nodes, self.constraints, self.width(), self.num_public_values())
+            if self._has_layout():
+                layout = (self.width(), self.num_public_values(), self.preprocessed_width(), self.num_periodic_columns())
+                self._program = self.gpu.air_program_create_layout(self.field.id, self.nodes, self.constraints, layout)
+            else:
+                self._program = self.gpu.air_program_create(self.field.id, self.nodes, self.constraints, self.width(), self.num_public_values())
         return self._program
 
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=()):
+    def periodic_table(self, log_degree: int, log_quotient_size: int):
+        """build_periodic_lde_table_two_adic (fri/src/periodic.rs:43-160) on the device: every column padded to the largest period
+        p_max by repetition, coset-LDE'd onto p_max * 2^q rows (q = log_quotient_size - log_degree, the quotient domain's blowup) over
+        the shift GENERATOR^(|K| / (p_max 2^q)), natural order: natural index i of the quotient domain reads row i mod (p_max 2^q).
+        (p_max * 2^q, n_periodic) device matrix, built once per (trace height, quotient size); None without periodic columns."""
+        if not self._periodic:
+            return None
+        key = (int(log_degree), int(log_quotient_size))
+        if key not in self._periodic_tables:
+            import torch
+            f, n = self.field, 1 << log_degree
+            err = periodic_column_error(self._periodic, n)
+            if err:
+                raise ValueError(err)
+            p_max = max(len(c) for c in self._periodic)
+            q = log_quotient_size - log_degree
+            padded = np.array([[c[i % len(c)] for c in self._periodic] for i in range(p_max)], dtype=np.uint64)
+            m = torch.from_numpy(f.to_monty_array(padded).astype(np.uint32).view(np.int32))
+            if isinstance(getattr(self.gpu, "device", None), int):
+                m = m.to(f"cuda:{self.gpu.device}")
+            shift = f.pow(f.generator, n // p_max)                     # GENERATOR^(|K| / (p_max 2^q)), |K| = n 2^q
+            self._periodic_tables[key] = self.gpu.coset_lde_batch(f.id, m, q, shift, bitrev_rows=False)
+        return self._periodic_tables[key]
+
+    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
         """uni-stark/src/prover.rs:462-827: `trace_lde_dev` holds the trace on the quotient domain GENERATOR * K, |K| = its height, in
-        bit-reversed row order (the committed LDE or its prefix).  Returns (|K|, 4) in natural order.  `public_values`: canonical."""
+        bit-reversed row order (the committed LDE or its prefix).  Returns (|K|, 4) in natural order.  `public_values`: canonical.
+        `preprocessed_on_quotient_domain`: the preprocessed trace the same way (required iff the AIR has preprocessed columns)."""
         if len(public_values) != self.num_public_values():
             raise ValueError(f"{len(public_values)} public values given, the AIR has {self.num_public_values()}")
-        prog = self.program()
+        if (preprocessed_on_quotient_domain is not None) != (self.preprocessed_width() > 0):
+            raise ValueError(f"the AIR has {self.preprocessed_width()} preprocessed columns: the preprocessed trace on the quotient domain "
+                             f"is {'given' if preprocessed_on_quotient_domain is not None else 'missing'}")
         H = int(trace_lde_dev.shape[0])
+        log_q = H.bit_length() - 1
         pv = [self.field.to_monty(int(v) % self.field.P) for v in public_values]
-        return self.gpu.air_quotient(prog, trace_lde_dev, H.bit_length() - 1, log_degree, pv, alpha)
+        if not self._has_layout():
+            return self.gpu.air_quotient(self.program(), trace_lde_dev, log_q, log_degree, pv, alpha)
+        table = self.periodic_table(log_degree, log_q)
+        prog = self.program()
+        return self.gpu.air_quotient_layout(prog, trace_lde_dev, preprocessed_on_quotient_domain, table, log_q, log_degree, pv, alpha)
 
     # ---- verifier: the constraint folder on the same DAG
-    def eval_folded_constraints(self, e, local, nxt, public_values, is_first_row, is_last_row, is_transition, alpha):
+    def eval_folded_constraints(self, e, local, nxt, public_values, is_first_row, is_last_row, is_transition, alpha, *,
+                                preprocessed_local=None, preprocessed_next=None, periodic_values=None):
         """VerifierConstraintFolder (uni-stark/src/folder.rs): acc = acc * alpha + c per constraint, on canonical EF4 values (`e`:
-        verifier.Ext), every node evaluated once."""
+        verifier.Ext), every node evaluated once.  The preprocessed rows and periodic values at zeta are given when the AIR has
+        them."""
         f = self.field
         vals = []
         for op, a, b, imm in self.builder.nodes:
@@ -248,6 +350,12 @@ class SymbolicAir:
                 v = is_last_row
             elif op == IS_TRANSITION:
                 v = is_transition
+            elif op == PREPROCESSED_LOCAL:
+                v = preprocessed_local[a]
+            elif op == PREPROCESSED_NEXT:
+                v = preprocessed_next[a]
+            elif op == PERIODIC:
+                v = periodic_values[a]
             elif op == ADD:
                 v = e.add(vals[a], vals[b])
             elif op == SUB:

@@ -5,7 +5,10 @@
 // read with uniform loads (one L1 transaction per warp and instruction), so opcodes never diverge.  Slots live in shared memory laid
 // out [slot][thread] (128 threads per block): conflict-free, and the footprint — slots x 512 B + constraints x 16 B for the
 // alpha-power table — is known at compile time of the program, so `create` can refuse a program that does not fit before anything
-// launches.  Trace values are read straight from the committed bit-reversed LDE (memory row bitrev(i), next row bitrev(i + 2^q)).
+// launches.  Trace values are read straight from the committed bit-reversed LDE (memory row bitrev(i), next row bitrev(i + 2^q)),
+// preprocessed values the same way from the committed preprocessed LDE, periodic values from row i mod (p_max * 2^q) of the small
+// periodic table (read-only path; at most p_max * 2^q x n_periodic words, cache-resident).  A program that reads neither runs the
+// instance without them (EXT = false): the same code as before they existed.
 #include "common.h"
 #include "air_program.cuh"
 
@@ -26,6 +29,10 @@ struct AirQArgs {
     const u32 *zh, *izh;        // Z_H and 1 / Z_H by i mod 2^q
     const u32 *pubs;
     u32 *q;
+    const u32 *pre;             // preprocessed LDE (EXT instances only)
+    size_t pre_width;
+    const u32 *periodic;        // periodic table, row-major (EXT instances only)
+    u32 n_periodic;
     AirDomain d;
 };
 
@@ -33,14 +40,20 @@ template <int F> struct AirDevEnv {
     const AirQArgs *a;
     const uint4 *ap;
     u32 *sl;                    // this thread's slot 0; slot s at sl[s * AIR_BLOCK]
-    const u32 *row, *nrow;
+    const u32 *row, *nrow, *prow, *pnrow, *per;
     __device__ __forceinline__ AirInsn insn(u32 pc) const {
         const uint2 v = __ldg(reinterpret_cast<const uint2 *>(a->prog) + pc);
         return AirInsn{v.x, v.y};
     }
     __device__ __forceinline__ u32 &slot(u32 s) { return sl[s * AIR_BLOCK]; }
     __device__ __forceinline__ void set_rows(u32 m, u32 mn) { row = a->lde + (size_t)m * a->width; nrow = a->lde + (size_t)mn * a->width; }
+    __device__ __forceinline__ void set_ext_rows(u32 m, u32 mn, u32 pr) {
+        prow = a->pre + (size_t)m * a->pre_width; pnrow = a->pre + (size_t)mn * a->pre_width; per = a->periodic + (size_t)pr * a->n_periodic;
+    }
     __device__ __forceinline__ u32 local(u32 c) const { return __ldg(row + c); }
+    __device__ __forceinline__ u32 pre_local(u32 c) const { return __ldg(prow + c); }
+    __device__ __forceinline__ u32 pre_next(u32 c) const { return __ldg(pnrow + c); }
+    __device__ __forceinline__ u32 periodic(u32 k) const { return __ldg(per + k); }
     __device__ __forceinline__ u32 next(u32 c) const { return __ldg(nrow + c); }
     __device__ __forceinline__ u32 pub(u32 k) const { return __ldg(a->pubs + k); }
     __device__ __forceinline__ uint4 apow(u32 k) const { return ap[k]; }
@@ -48,7 +61,7 @@ template <int F> struct AirDevEnv {
     __device__ __forceinline__ u32 inv_zh(u32 i) const { return __ldg(a->izh + (i & ((1u << a->d.q) - 1u))); }
 };
 
-template <int F> __global__ void __launch_bounds__(AIR_BLOCK) air_program_quotient_kernel(const AirQArgs a) {
+template <int F, bool EXT> __global__ void __launch_bounds__(AIR_BLOCK) air_program_quotient_kernel(const AirQArgs a) {
     extern __shared__ uint4 air_sm[];
     for (u32 t = threadIdx.x; t < a.n_cons; t += AIR_BLOCK) air_sm[t] = __ldg(a.apow + t);
     __syncthreads();
@@ -58,14 +71,15 @@ template <int F> __global__ void __launch_bounds__(AIR_BLOCK) air_program_quotie
     env.a = &a;
     env.ap = air_sm;
     env.sl = reinterpret_cast<u32 *>(air_sm + a.n_cons) + threadIdx.x;
-    reinterpret_cast<uint4 *>(a.q)[i] = air_row_quotient<F>(env, a.d, a.n_insns, i);
+    reinterpret_cast<uint4 *>(a.q)[i] = air_row_quotient<F, EXT>(env, a.d, a.n_insns, i);
 }
 
 int32_t air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const u32 *constraints, size_t n_constraints,
-                           u32 width, u32 n_public, p3gpu_air_program **out) {
+                           const p3gpu_air_layout &layout, p3gpu_air_program **out) {
     std::string err;
     AirProgram prog;
-    const int32_t rc = air_compile(field, nodes, n_nodes, constraints, n_constraints, width, n_public, prog, err);
+    const int32_t rc = air_compile(field, nodes, n_nodes, constraints, n_constraints, layout.width, layout.n_public, layout.preprocessed_width,
+                                   layout.n_periodic, prog, err);
     P3_CHECK(rc == P3GPU_OK, rc, "%s", err.c_str());
     std::unique_ptr<p3gpu_air_program> p(new p3gpu_air_program);
     p->device = ctx->device;
@@ -96,14 +110,15 @@ int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t 
 }
 
 template <int F>
-static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, unsigned log_q, unsigned log_n,
-                                   const u32 *pubs, const u32 *alpha, u32 *d_q) {
+static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, const u32 *d_pre, const u32 *d_periodic,
+                                   unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs, const u32 *alpha, u32 *d_q) {
     const AirProgram &p = pg->prog;
     for (u32 k = 0; k < p.n_public; k++) P3_CHECK(pubs[k] < Fp<F>::P, P3GPU_EINVAL, "public value %u is not a canonical Montgomery word", k);
     for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
     std::vector<u32> zh, izh;
     AirQArgs qa;
     qa.d = air_domain<F>(log_q, log_n, p.uses, zh, izh);
+    qa.d.periodic_mask = (1u << log_periodic_rows) - 1u;
     const std::vector<uint4> ap = air_alpha_table<F>(alpha, p.n_constraints);
     // one staging copy: alpha table | Z_H | 1/Z_H | public values
     const size_t nz = zh.size(), words = (size_t)p.n_constraints * 4 + 2 * nz + p.n_public;
@@ -122,8 +137,10 @@ static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, 
     qa.apow = reinterpret_cast<const uint4 *>(dt);
     qa.zh = dt + (size_t)p.n_constraints * 4; qa.izh = qa.zh + nz; qa.pubs = qa.izh + nz;
     qa.q = d_q;
+    qa.pre = d_pre; qa.pre_width = p.pre_width;
+    qa.periodic = d_periodic; qa.n_periodic = p.n_periodic;
     const size_t smem = air_smem_bytes(p.n_slots, p.n_constraints);
-    auto kern = air_program_quotient_kernel<F>;
+    auto kern = (p.uses & AIR_USES_EXT) ? air_program_quotient_kernel<F, true> : air_program_quotient_kernel<F, false>;
     if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const size_t n = (size_t)1 << log_q;
     kern<<<(unsigned)((n + AIR_BLOCK - 1) / AIR_BLOCK), AIR_BLOCK, smem, ctx->stream>>>(qa);
@@ -132,10 +149,14 @@ static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, 
     return P3GPU_OK;
 }
 
-int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, unsigned log_lde, unsigned log_q, unsigned log_n,
-                             const u32 *pubs, const u32 *alpha, u32 *d_q) {
+int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, unsigned log_lde, const u32 *d_pre, unsigned log_pre,
+                             const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs,
+                             const u32 *alpha, u32 *d_q, bool layout_entry) {
     P3_CHECK(pg->device == ctx->device, P3GPU_EINVAL, "AIR program was created on device %d, the context is on device %d", pg->device, ctx->device);
-    const int field = pg->prog.field;
+    const AirProgram &p = pg->prog;
+    const int field = p.field;
+    P3_CHECK(layout_entry || (p.pre_width == 0 && p.n_periodic == 0), P3GPU_EINVAL,
+             "the AIR program has preprocessed or periodic columns: evaluate it with p3gpu_air_quotient_layout_dev");
     const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
     P3_CHECK(log_n <= log_q && log_q <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL,
              "need log_trace_height %u <= log_quotient_size %u <= log_lde_height %u <= %u", log_n, log_q, log_lde, two_adicity);
@@ -144,8 +165,26 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const 
     P3_CHECK(pg->prog.n_public == 0 || pubs != nullptr, P3GPU_EINVAL, "the program reads %u public values, none given", pg->prog.n_public);
     P3_CHECK(reinterpret_cast<uintptr_t>(d_q) % 16 == 0 && reinterpret_cast<uintptr_t>(d_lde) % 4 == 0, P3GPU_EINVAL, "quotient: misaligned buffer");
     P3_CHECK(air_smem_bytes(pg->prog.n_slots, pg->prog.n_constraints) <= 227 * 1024, P3GPU_EUNSUPPORTED, "AIR program needs more shared memory than a block has");
-    if (field == BABY_BEAR) return air_quotient_launch<BABY_BEAR>(ctx, pg, d_lde, log_q, log_n, pubs, alpha, d_q);
-    return air_quotient_launch<KOALA_BEAR>(ctx, pg, d_lde, log_q, log_n, pubs, alpha, d_q);
+    // preprocessed LDE: given iff the layout has preprocessed columns, read like the trace LDE's quotient-domain prefix
+    P3_CHECK((p.pre_width > 0) == (d_pre != nullptr), P3GPU_EINVAL, "preprocessed LDE %s, the program's preprocessed width is %u",
+             d_pre ? "given" : "missing", p.pre_width);
+    if (d_pre) {
+        P3_CHECK(log_q <= log_pre && log_pre <= two_adicity, P3GPU_EINVAL, "preprocessed LDE of 2^%u rows: need 2^%u <= height <= 2^%u", log_pre,
+                 log_q, two_adicity);
+        P3_CHECK(reinterpret_cast<uintptr_t>(d_pre) % 4 == 0, P3GPU_EINVAL, "quotient: misaligned preprocessed LDE");
+    }
+    // periodic table: given iff the layout has periodic columns, at most one row per quotient point
+    P3_CHECK((p.n_periodic > 0) == (d_periodic != nullptr), P3GPU_EINVAL, "periodic table %s, the program has %u periodic columns",
+             d_periodic ? "given" : "missing", p.n_periodic);
+    if (d_periodic) {
+        P3_CHECK(log_periodic_rows <= log_q, P3GPU_EINVAL, "periodic table of 2^%u rows over a quotient domain of 2^%u", log_periodic_rows, log_q);
+        P3_CHECK(reinterpret_cast<uintptr_t>(d_periodic) % 4 == 0, P3GPU_EINVAL, "quotient: misaligned periodic table");
+    } else {
+        log_periodic_rows = 0;
+    }
+    if (field == BABY_BEAR)
+        return air_quotient_launch<BABY_BEAR>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q);
+    return air_quotient_launch<KOALA_BEAR>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q);
 }
 
 }  // namespace p3

@@ -2,15 +2,16 @@
 // compiled once into a register program that air_program.cu's quotient kernel interprets over the quotient domain.
 //
 // This header holds everything that is not a CUDA launch — the node validation, the compiler, the per-instruction semantics and
-// the per-row quotient evaluation — so host C++ can include it (tests/cpp/air_program_check.cpp runs it against the oracle on the
-// CPU) exactly as the kernel does.
+// the per-row quotient evaluation — so host C++ can include it (tests/cpp/air_program_check.cpp and, for the EXT instance,
+// tests/cpp/air_layout_check.cpp run it against the oracle on the CPU) exactly as the kernel does.
 //
 //   nodes        p3gpu_air_node {op, a, b, imm} in topological order (operands refer only to earlier nodes)
 //   compile      drop dead nodes; per constraint in assertion order emit its not yet emitted cone (post-order), then FOLD it;
 //                slots by liveness (an operand's slot is released at its last use, before the result is allocated), so the slot
 //                count is the maximum number of simultaneously live values
 //   instruction  2 words: op_dst = op | dst << 4, arg = operand (binary: a | b << 16; leaf: column / public index / Montgomery
-//                constant; FOLD: dst is the constraint index, arg the slot)
+//                constant; FOLD: dst is the constraint index, arg the slot).  Node ops 0-10 are their own opcodes; the preprocessed
+//                and periodic leaves (node ops 16-18) become opcodes 12-14, so every opcode fits the 4-bit field
 //   fold         acc += c_k * alpha^(K - 1 - k) (the first constraint gets the highest power, air/src/symbolic/builder.rs:482-511),
 //                lazily in 64 bits per coefficient; quotient = acc / Z_H(x)
 #pragma once
@@ -24,6 +25,7 @@
 namespace p3 {
 
 constexpr u32 AIR_OP_FOLD = 11;                 // instruction-only op, after the node ops P3GPU_AIR_CONST .. P3GPU_AIR_MUL
+constexpr u32 AIR_OP_PRE_LOCAL = 12, AIR_OP_PRE_NEXT = 13, AIR_OP_PERIODIC = 14;     // P3GPU_AIR_PREPROCESSED_LOCAL / _NEXT, PERIODIC
 constexpr u32 AIR_MAX_SLOTS = 384;              // 384 slots x 128 threads x 4 B = 192 KiB of shared memory per block
 constexpr u32 AIR_MAX_CONSTRAINTS = 2048;       // alpha-power table: 32 KiB of shared memory
 constexpr u32 AIR_BLOCK = 128;
@@ -31,12 +33,14 @@ constexpr unsigned AIR_MAX_RATE_BITS = 8;       // q = log_quotient_size - log_t
 
 // uses_mask bits
 constexpr u32 AIR_USES_NEXT = 1, AIR_USES_SELECTORS = 2, AIR_USES_PUBLIC = 4;
+constexpr u32 AIR_USES_PRE_LOCAL = 8, AIR_USES_PRE_NEXT = 16, AIR_USES_PERIODIC = 32;
+constexpr u32 AIR_USES_EXT = AIR_USES_PRE_LOCAL | AIR_USES_PRE_NEXT | AIR_USES_PERIODIC;
 
 struct AirInsn { u32 op_dst, arg; };
 
 struct AirProgram {
     int field = 0;
-    u32 width = 0, n_public = 0;
+    u32 width = 0, n_public = 0, pre_width = 0, n_periodic = 0;
     u32 n_slots = 0, n_constraints = 0, uses = 0;
     std::vector<AirInsn> insns;
 };
@@ -45,8 +49,9 @@ inline size_t air_smem_bytes(u32 n_slots, u32 n_constraints) { return (size_t)n_
 
 // Validates the node list and compiles it.  Returns P3GPU_OK, P3GPU_EINVAL (malformed nodes / constraints) or P3GPU_EUNSUPPORTED
 // (beyond the slot or constraint limit); `err` says why.
+// pre_width / n_periodic: the preprocessed columns and periodic columns the leaves may read (0: none).
 inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints, size_t n_constraints,
-                           u32 width, u32 n_public, AirProgram &out, std::string &err) {
+                           u32 width, u32 n_public, u32 pre_width, u32 n_periodic, AirProgram &out, std::string &err) {
     auto fail = [&](int32_t code, const std::string &m) { err = m; return code; };
     if (field != BABY_BEAR && field != KOALA_BEAR) return fail(P3GPU_EUNSUPPORTED, "AIR program: unsupported field " + std::to_string(field));
     const u32 P = field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
@@ -67,6 +72,14 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
                 if (n.a >= n_public) return fail(P3GPU_EINVAL, at + "public value " + std::to_string(n.a) + " >= " + std::to_string(n_public));
                 break;
             case P3GPU_AIR_IS_FIRST_ROW: case P3GPU_AIR_IS_LAST_ROW: case P3GPU_AIR_IS_TRANSITION:
+                break;
+            case P3GPU_AIR_PREPROCESSED_LOCAL: case P3GPU_AIR_PREPROCESSED_NEXT:
+                if (n.a >= pre_width)
+                    return fail(P3GPU_EINVAL, at + "preprocessed column " + std::to_string(n.a) + " >= preprocessed width " + std::to_string(pre_width));
+                break;
+            case P3GPU_AIR_PERIODIC:
+                if (n.a >= n_periodic)
+                    return fail(P3GPU_EINVAL, at + "periodic column " + std::to_string(n.a) + " >= " + std::to_string(n_periodic));
                 break;
             case P3GPU_AIR_ADD: case P3GPU_AIR_SUB: case P3GPU_AIR_MUL:
                 if (n.b >= i) return fail(P3GPU_EINVAL, at + "operand b = " + std::to_string(n.b) + " is not an earlier node");
@@ -120,6 +133,7 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
     std::vector<u32> slot(n_nodes, 0), free_slots;
     AirProgram prog;
     prog.field = field; prog.width = width; prog.n_public = n_public; prog.n_constraints = (u32)n_constraints;
+    prog.pre_width = pre_width; prog.n_periodic = n_periodic;
     prog.insns.reserve(events.size());
     auto release = [&](u32 node, size_t p) { if (last[node] == p) free_slots.push_back(slot[node]); };
     for (size_t p = 0; p < events.size(); p++) {
@@ -131,13 +145,16 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
         }
         const u32 i = (u32)events[p];
         const p3gpu_air_node &n = nodes[i];
-        u32 arg = 0;
+        u32 arg = 0, op = n.op;
         switch (n.op) {
             case P3GPU_AIR_CONST: arg = n.imm; break;
             case P3GPU_AIR_MAIN_LOCAL: arg = n.a; break;
             case P3GPU_AIR_MAIN_NEXT: arg = n.a; prog.uses |= AIR_USES_NEXT; break;
             case P3GPU_AIR_PUBLIC: arg = n.a; prog.uses |= AIR_USES_PUBLIC; break;
             case P3GPU_AIR_IS_FIRST_ROW: case P3GPU_AIR_IS_LAST_ROW: case P3GPU_AIR_IS_TRANSITION: prog.uses |= AIR_USES_SELECTORS; break;
+            case P3GPU_AIR_PREPROCESSED_LOCAL: arg = n.a; op = AIR_OP_PRE_LOCAL; prog.uses |= AIR_USES_PRE_LOCAL; break;
+            case P3GPU_AIR_PREPROCESSED_NEXT: arg = n.a; op = AIR_OP_PRE_NEXT; prog.uses |= AIR_USES_PRE_NEXT; break;
+            case P3GPU_AIR_PERIODIC: arg = n.a; op = AIR_OP_PERIODIC; prog.uses |= AIR_USES_PERIODIC; break;
             case P3GPU_AIR_NEG: arg = slot[n.a]; release(n.a, p); break;
             default:
                 arg = slot[n.a] | (slot[n.b] << 16);
@@ -149,10 +166,15 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
         free_slots.pop_back();
         if (prog.n_slots > AIR_MAX_SLOTS)
             return fail(P3GPU_EUNSUPPORTED, "AIR program: more than " + std::to_string(AIR_MAX_SLOTS) + " simultaneously live values (slots)");
-        prog.insns.push_back({n.op | (slot[i] << 4), arg});
+        prog.insns.push_back({op | (slot[i] << 4), arg});
     }
     out = std::move(prog);
     return P3GPU_OK;
+}
+
+inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints, size_t n_constraints,
+                           u32 width, u32 n_public, AirProgram &out, std::string &err) {
+    return air_compile(field, nodes, n_nodes, constraints, n_constraints, width, n_public, 0, 0, out, err);
 }
 
 // ---- per-instruction semantics and per-row quotient, shared by the kernel and host C++ -------------------------------------
@@ -187,16 +209,23 @@ struct AirDomain {
     u32 w_q;                    // generator of K
     u32 w_n_inv;                // omega_N^-1
     u32 uses;
+    u32 periodic_mask;          // rows of the periodic table - 1 (natural index i reads row i & periodic_mask)
 };
 
 // Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),
-// the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).
+// the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).  EXT (a program that reads
+// preprocessed or periodic columns) compiles in opcodes 12-14: Env then also supplies set_ext_rows(m, m_next, periodic_row),
+// pre_local(c), pre_next(c) and periodic(k).  Without EXT those opcodes and row pointers do not exist in the instance.
 #ifdef __CUDACC__
 #pragma nv_exec_check_disable
 #endif
-template <int F, class Env> __host__ __device__ __forceinline__ uint4 air_row_quotient(Env &env, const AirDomain &d, u32 n_insns, u32 i) {
+template <int F, bool EXT = false, class Env>
+__host__ __device__ __forceinline__ uint4 air_row_quotient(Env &env, const AirDomain &d, u32 n_insns, u32 i) {
     const u32 mask = d.log_q == 32 ? 0xffffffffu : ((1u << d.log_q) - 1u);
-    env.set_rows(air_bitrev(i, d.log_q), (d.uses & AIR_USES_NEXT) ? air_bitrev((i + (1u << d.q)) & mask, d.log_q) : 0u);
+    const u32 next_uses = EXT ? (AIR_USES_NEXT | AIR_USES_PRE_NEXT) : AIR_USES_NEXT;
+    const u32 m = air_bitrev(i, d.log_q), mn = (d.uses & next_uses) ? air_bitrev((i + (1u << d.q)) & mask, d.log_q) : 0u;
+    env.set_rows(m, mn);
+    if constexpr (EXT) env.set_ext_rows(m, mn, i & d.periodic_mask);
     u32 first = 0, last = 0, trans = 0;
     if (d.uses & AIR_USES_SELECTORS) {
         // selectors_on_coset (commit/src/domain.rs:321-361), unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1
@@ -225,7 +254,13 @@ template <int F, class Env> __host__ __device__ __forceinline__ uint4 air_row_qu
             case P3GPU_AIR_SUB: v = fp_sub<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
             case P3GPU_AIR_NEG: v = fp_neg<F>(env.slot(in.arg)); break;
             case P3GPU_AIR_MUL: v = mont_mul<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
-            default:                                                    // AIR_OP_FOLD
+            default:                                                    // AIR_OP_FOLD (and, with EXT, opcodes 12-14)
+                if constexpr (EXT) {
+                    if (op != AIR_OP_FOLD) {
+                        v = op == AIR_OP_PRE_LOCAL ? env.pre_local(in.arg) : op == AIR_OP_PRE_NEXT ? env.pre_next(in.arg) : env.periodic(in.arg);
+                        break;
+                    }
+                }
                 air_qmac<F>(acc, env.slot(in.arg), env.apow(dst));
                 continue;
         }
@@ -239,7 +274,7 @@ template <int F, class Env> __host__ __device__ __forceinline__ uint4 air_row_qu
 // Host-side launch constants + tables: Z_H(x_i) and 1/Z_H(x_i) depend on i mod 2^q only (x^N = g^N w_q^(iN), w_q^N of order 2^q).
 template <int F> inline AirDomain air_domain(unsigned log_q, unsigned log_n, u32 uses, std::vector<u32> &zh, std::vector<u32> &inv_zh) {
     AirDomain d;
-    d.log_q = log_q; d.q = log_q - log_n; d.uses = uses;
+    d.log_q = log_q; d.q = log_q - log_n; d.uses = uses; d.periodic_mask = 0;
     d.shift = to_monty<F>(Fp<F>::GEN);
     d.w_q = two_adic_generator<F>(log_q);
     d.w_n_inv = fp_inv<F>(two_adic_generator<F>(log_n));

@@ -503,7 +503,15 @@ int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node
     P3_ENTER(ctx);
     P3_CHECK(out, P3GPU_EINVAL, "null argument");
     *out = nullptr;
-    return air_program_create(ctx, field, nodes, n_nodes, constraints, n_constraints, width, n_public, out);
+    const p3gpu_air_layout layout = {width, n_public, 0, 0};
+    return air_program_create(ctx, field, nodes, n_nodes, constraints, n_constraints, layout, out);
+}
+int32_t p3gpu_air_program_create_layout(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                        size_t n_constraints, const p3gpu_air_layout *layout, p3gpu_air_program **out) {
+    P3_ENTER(ctx);
+    P3_CHECK(out && layout, P3GPU_EINVAL, "null argument");
+    *out = nullptr;
+    return air_program_create(ctx, field, nodes, n_nodes, constraints, n_constraints, *layout, out);
 }
 void p3gpu_air_program_destroy(p3gpu_air_program *prog) { air_program_destroy(prog); }
 int32_t p3gpu_air_program_info(const p3gpu_air_program *prog, size_t *n_instructions, size_t *n_slots, size_t *n_constraints) {
@@ -514,7 +522,17 @@ int32_t p3gpu_air_quotient_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, co
                                uint32_t *d_quotient) {
     P3_ENTER(ctx);
     P3_CHECK(prog && d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
-    return air_program_quotient(ctx, prog, d_lde, log_lde_height, log_quotient_size, log_trace_height, public_values, alpha, d_quotient);
+    return air_program_quotient(ctx, prog, d_lde, log_lde_height, nullptr, 0, nullptr, 0, log_quotient_size, log_trace_height, public_values,
+                                alpha, d_quotient, false);
+}
+int32_t p3gpu_air_quotient_layout_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_lde, unsigned log_lde_height,
+                                      const uint32_t *d_pre_lde, unsigned log_pre_lde_height, const uint32_t *d_periodic,
+                                      unsigned log_periodic_rows, unsigned log_quotient_size, unsigned log_trace_height,
+                                      const uint32_t *public_values, const uint32_t alpha[4], uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(prog && d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return air_program_quotient(ctx, prog, d_lde, log_lde_height, d_pre_lde, log_pre_lde_height, d_periodic, log_periodic_rows,
+                                log_quotient_size, log_trace_height, public_values, alpha, d_quotient, true);
 }
 
 // ---- transcript + query phase (prove driver) ---------------------------------------------------------

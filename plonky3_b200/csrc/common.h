@@ -155,11 +155,14 @@ int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned wo
 
 // air_program.cu: any AIR as a constraint program (air_program.cuh)
 int32_t air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const u32 *constraints, size_t n_constraints,
-                           u32 width, u32 n_public, p3gpu_air_program **out);
+                           const p3gpu_air_layout &layout, p3gpu_air_program **out);
 void air_program_destroy(p3gpu_air_program *prog);
 int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t *n_slots, size_t *n_cons);
-int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const u32 *d_lde, unsigned log_lde, unsigned log_q, unsigned log_n,
-                             const u32 *pubs, const u32 *alpha, u32 *d_q);
+// layout_entry: called through p3gpu_air_quotient_layout_dev (d_pre / d_periodic as the program's layout declares them); otherwise
+// through p3gpu_air_quotient_dev, which refuses a program with preprocessed or periodic columns
+int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const u32 *d_lde, unsigned log_lde, const u32 *d_pre,
+                             unsigned log_pre, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n,
+                             const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
 
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);

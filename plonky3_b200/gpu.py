@@ -318,6 +318,39 @@ class Gpu:
                                             pv.ctypes.data if pv.size else None, self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    def air_program_create_layout(self, field, nodes, constraints, layout):
+        """air_program_create for a program that may read preprocessed and periodic columns: layout = (width, n_public,
+        preprocessed_width, n_periodic)."""
+        nd = np.ascontiguousarray(nodes, dtype=np.uint32).reshape(-1, 4)
+        cs = np.ascontiguousarray(constraints, dtype=np.uint32).ravel()
+        lay = np.ascontiguousarray(layout, dtype=np.uint32)
+        assert lay.size == 4
+        h = C.c_void_p()
+        check(self.L.p3gpu_air_program_create_layout(self.h, field, nd.ctypes.data, nd.shape[0], cs.ctypes.data, cs.size, lay.ctypes.data,
+                                                     C.byref(h)))
+        return AirProgramHandle(self.L, h)
+
+    def air_quotient_layout(self, prog, lde_dev, pre_lde_dev, periodic_dev, log_quotient_size, log_trace_height, public_values, alpha):
+        """air_quotient with the preprocessed LDE (committed, bit-reversed; None without preprocessed columns) and the periodic table
+        ((p_max * 2^q, n_periodic), natural order; None without periodic columns)."""
+        m = self._dev(lde_dev); self._use_torch_stream()
+        H = int(m.shape[0]); log_h = H.bit_length() - 1
+        pre = self._dev(pre_lde_dev) if pre_lde_dev is not None else None
+        per = self._dev(periodic_dev) if periodic_dev is not None else None
+        for name, t in (("LDE", m), ("preprocessed LDE", pre), ("periodic table", per)):
+            if t is not None and int(t.shape[0]) & (int(t.shape[0]) - 1):
+                raise _lib.P3GpuError(f"{name} height {int(t.shape[0])} is not a power of two", _lib.EINVAL)
+        pv = np.ascontiguousarray(public_values, dtype=np.uint32).ravel()
+        q = self._empty((1 << log_quotient_size, 4))
+        check(self.L.p3gpu_air_quotient_layout_dev(self.h, prog.h, m.data_ptr(), log_h,
+                                                   pre.data_ptr() if pre is not None else None,
+                                                   int(pre.shape[0]).bit_length() - 1 if pre is not None else 0,
+                                                   per.data_ptr() if per is not None else None,
+                                                   int(per.shape[0]).bit_length() - 1 if per is not None else 0,
+                                                   log_quotient_size, log_trace_height, pv.ctypes.data if pv.size else None,
+                                                   self._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
+
     def pcs_commit_host(self, field, hash_kind, evals_host, log_blowup, cap_height):
         """p3gpu_pcs_commit: TwoAdicFriPcs::commit with the trace in HOST memory (numpy uint32 array or pinned CPU int32 tensor);
         the LDE and the digest layers stay on the device, only the cap returns.  Returns (cap (n, 8) array, lde, layers)."""

@@ -52,10 +52,11 @@ def _option_vec_ef(a) -> bytes:
 
 
 def proof_to_postcard(proof) -> bytes:
-    """`proof`: plonky3_b200.uni_stark.Proof (non-ZK, no preprocessed trace)."""
+    """`proof`: plonky3_b200.uni_stark.Proof (non-ZK)."""
     out = bytearray()
     out += _vec_of(proof.trace_commit, 8) + _vec_of(proof.quotient_commit, 8) + b"\x00"
-    out += _vec_of(proof.trace_local, 4) + _option_vec_ef(proof.trace_next) + b"\x00\x00"
+    out += _vec_of(proof.trace_local, 4) + _option_vec_ef(proof.trace_next)
+    out += _option_vec_ef(getattr(proof, "preprocessed_local", None)) + _option_vec_ef(getattr(proof, "preprocessed_next", None))
     out += _varint(len(proof.quotient_chunks)) + b"".join(_vec_of(c, 4) for c in proof.quotient_chunks) + b"\x00"
     out += _varint(len(proof.commit_phase_commits)) + b"".join(_vec_of(c, 8) for c in proof.commit_phase_commits)
     out += _varint(len(proof.commit_pow_witnesses)) + _words(np.array(proof.commit_pow_witnesses, dtype=np.uint32))
@@ -134,8 +135,8 @@ def proof_from_postcard(data: bytes, prime=None) -> dict:
         raise ValueError("ZK (random) commitments are not supported")
     p["trace_local"] = r.vec_of(4)
     p["trace_next"] = r.option_vec_ef()
-    if r.byte() != 0 or r.byte() != 0:
-        raise ValueError("preprocessed openings are not supported")
+    p["preprocessed_local"] = r.option_vec_ef()
+    p["preprocessed_next"] = r.option_vec_ef()
     p["quotient_chunks"] = [r.vec_of(4) for _ in range(r.varint())]
     if r.byte() != 0:
         raise ValueError("ZK (random) openings are not supported")

@@ -4,7 +4,8 @@
 the reference's names; host code is only the protocol sequencing (the transcript's sponge itself runs on the device,
 challenger.py).  Non-ZK, no preprocessed columns, no public values — what the example binary proves
 (examples/src/proofs.rs:120-170) — and for any AIR given as symbolic constraints (air.SymbolicAir: public values, next-row
-openings, any number of quotient chunks up to the blowup), whose quotient is p3gpu_air_quotient_dev.  `prove` is the one
+openings, any number of quotient chunks up to the blowup, preprocessed columns committed once by `setup_preprocessed`, periodic
+columns), whose quotient is p3gpu_air_quotient_dev / p3gpu_air_quotient_layout_dev.  `prove` is the one
 protocol sequence: with `shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns
 split over several GPUs, the shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
 
@@ -169,6 +170,8 @@ class Proof:
     degree_bits: int
     timings_ms: dict = dc_field(default_factory=dict)
     trace_next: Optional[np.ndarray] = None       # (width, 4) when the AIR reads the next row (uni-stark/src/proof.rs:52-56)
+    preprocessed_local: Optional[np.ndarray] = None   # (preprocessed width, 4) when the AIR has preprocessed columns
+    preprocessed_next: Optional[np.ndarray] = None    # ... and its preprocessed_next_row_columns() is not empty
     input_opening_indices: list = dc_field(default_factory=list)     # per input batch: the height-reduced query indices
     commit_phase_indices: list = dc_field(default_factory=list)      # per FRI round: the opened group index of every query
 
@@ -178,21 +181,77 @@ class Proof:
         return proof_to_postcard(self)
 
 
+@dataclass
+class PreprocessedVerifierKey:
+    """uni-stark/src/preprocessed.rs PreprocessedVerifierKey: what the verifier needs of the committed preprocessed trace."""
+    width: int
+    degree_bits: int
+    commitment: np.ndarray
+
+
+@dataclass
+class PreprocessedProverData:
+    """uni-stark/src/preprocessed.rs PreprocessedProverData: the preprocessed trace committed once (LDE and tree resident), reusable
+    by every proof of the same AIR and height."""
+    width: int
+    degree_bits: int
+    commitment: np.ndarray
+    prover_data: object
+
+
+def _air_preprocessed_width(air) -> int:
+    return int(getattr(air, "preprocessed_width", lambda: 0)())
+
+
+def _air_pre_next(air) -> bool:
+    return len(getattr(air, "preprocessed_next_row_columns", lambda: [])()) > 0
+
+
+def _air_periodic(air) -> list:
+    return list(getattr(air, "periodic_columns", lambda: [])())
+
+
+def setup_preprocessed(config: StarkConfig, air, degree_bits: int):
+    """uni-stark/src/preprocessed.rs:46-91: commit the AIR's preprocessed trace on the trace domain of 2^degree_bits rows (same blowup
+    as the trace).  Returns (PreprocessedProverData, PreprocessedVerifierKey), or None when the AIR has no preprocessed columns."""
+    import torch
+    width = _air_preprocessed_width(air)
+    if width == 0:
+        return None
+    trace = air.preprocessed_trace()
+    if int(trace.shape[0]) != 1 << degree_bits:
+        raise ValueError(f"preprocessed trace height {int(trace.shape[0])} must equal the trace degree 2^{degree_bits}")
+    pcs = config.pcs
+    gpu = pcs.dft.gpu
+    if not isinstance(trace, torch.Tensor):
+        trace = torch.from_numpy(np.ascontiguousarray(trace, dtype=np.uint32).view(np.int32))
+        if isinstance(getattr(gpu, "device", None), int):
+            trace = trace.to(f"cuda:{gpu.device}")
+    commitment, data = pcs.commit([(pcs.natural_domain_for_degree(1 << degree_bits), trace)])
+    return (PreprocessedProverData(width, degree_bits, commitment, data), PreprocessedVerifierKey(width, degree_bits, commitment))
+
+
 def get_log_num_quotient_chunks(air) -> int:
     """uni-stark/src/symbolic.rs get_log_num_quotient_chunks: log2_ceil(max(constraint_degree, 2) - 1) (non-ZK)."""
     d = max(air.max_constraint_degree(), 2)
     return max(d - 2, 0).bit_length()
 
 
-def verify(config: StarkConfig, air, proof, public_values=()):
-    """uni-stark/src/verifier.rs:282-295.  Raises verifier.VerificationError."""
+def verify(config: StarkConfig, air, proof, public_values=(), *, preprocessed_vk: Optional[PreprocessedVerifierKey] = None):
+    """uni-stark/src/verifier.rs:282-295 (verify_with_preprocessed).  Raises verifier.VerificationError."""
     from .verifier import verify as _verify
-    return _verify(config, air, proof, public_values)
+    if preprocessed_vk is None:
+        return _verify(config, air, proof, public_values)
+    return _verify(config, air, proof, public_values, preprocessed_vk=preprocessed_vk)
 
 
-def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> Proof:
-    """uni-stark/src/prover.rs:87-442.  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device (CUDA int32) matrix of
-    height 2^n.  `public_values`: canonical integers.
+def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
+    """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device
+    (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
+
+    `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
+    after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is
+    empty).  Periodic columns need nothing here: the AIR evaluates them on the quotient domain.
 
     `shard`: a distributed.ShardedTrace when the trace's columns are split over ranks; `trace` is then this rank's column block,
     and every rank returns the proof of the whole trace."""
@@ -215,11 +274,28 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> P
     log_degree = _log2_strict(degree)
     log_num_quotient_chunks = get_log_num_quotient_chunks(air)
     num_quotient_chunks = 1 << log_num_quotient_chunks
+    pre_width = _air_preprocessed_width(air)
+    periodic = _air_periodic(air)
+    if pre_width > 0 and preprocessed is None:
+        raise ValueError(f"the AIR has {pre_width} preprocessed columns: call setup_preprocessed and pass its prover data")
+    if preprocessed is not None:
+        if preprocessed.width != pre_width:
+            raise ValueError(f"preprocessed prover data of width {preprocessed.width}, the AIR has {pre_width} preprocessed columns")
+        if preprocessed.degree_bits != log_degree:
+            raise ValueError(f"preprocessed trace height 2^{preprocessed.degree_bits} differs from the trace height 2^{log_degree}")
+    if periodic:
+        from .air import periodic_column_error
+        err = periodic_column_error(periodic, degree)
+        if err:
+            raise ValueError(err)
+    if shard is not None and (pre_width or periodic):
+        raise ValueError("the row-sharded prove does not take preprocessed or periodic columns")
     if log_num_quotient_chunks > pcs.fri.log_blowup:
         # the quotient domain must lie inside the committed LDE (fast path of get_evaluations_on_domain); the reference asserts too
         raise ValueError(f"constraint degree {air.max_constraint_degree()} needs {num_quotient_chunks} quotient chunks: log_blowup "
                          f"{pcs.fri.log_blowup} < {log_num_quotient_chunks}")
     opens_next = len(air.main_next_row_columns()) > 0
+    pre_next = pre_width > 0 and _air_pre_next(air)
     challenger = config.initialise_challenger()
     trace_domain = pcs.natural_domain_for_degree(degree)
 
@@ -232,8 +308,10 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> P
 
     challenger.observe_canonical(log_degree)                                             # log_ext_degree (non-ZK)       :224
     challenger.observe_canonical(log_degree)                                             # log_degree                    :225
-    challenger.observe_canonical(0)                                                      # preprocessed_width            :226
+    challenger.observe_canonical(pre_width)                                              # preprocessed_width            :226
     challenger.observe_cap(trace_commit)                                                 # :230
+    if pre_width > 0:
+        challenger.observe_cap(preprocessed.commitment)                                  # :231-232
     for v in public_values:                                                              # :236
         challenger.observe_canonical(v)
     alpha = challenger.sample_algebra_element()                                          # :258
@@ -242,7 +320,13 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> P
     quotient_domain = (f.mul(trace_domain[0], f.generator), log_degree + log_num_quotient_chunks)      # create_disjoint_domain
     if shard is None:
         trace_on_quotient_domain = pcs.get_evaluations_on_domain(trace_data, 0, quotient_domain).bit_reverse_rows()
-        quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)  # natural order = flatten_to_base
+        if pre_width > 0 or periodic:
+            pre_q = (pcs.get_evaluations_on_domain(preprocessed.prover_data, 0, quotient_domain).bit_reverse_rows()
+                     if pre_width > 0 else None)                                           # :272
+            quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values,
+                                                preprocessed_on_quotient_domain=pre_q)
+        else:
+            quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)  # natural order = flatten_to_base
     else:
         quotient_flat = shard.quotient_values(air, quotient_domain, alpha)
     span("compute quotient polynomial", t0)
@@ -255,10 +339,16 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> P
     zeta = challenger.sample_algebra_element()                                           # :365
     t0 = time.perf_counter()
     trace_points = [zeta]
-    if opens_next:                                                                       # zeta * omega_N (trace_domain.next_point)
-        trace_points.append(X.ef_scale(f, np.asarray(zeta, dtype=np.uint32), f.two_adic_generator(log_degree)))
+    zeta_next = None
+    if opens_next or pre_next:                                                           # zeta * omega_N (trace_domain.next_point)
+        zeta_next = X.ef_scale(f, np.asarray(zeta, dtype=np.uint32), f.two_adic_generator(log_degree))
+    if opens_next:
+        trace_points.append(zeta_next)
     rounds = [(trace_data, [trace_points]), (quotient_data, [[zeta]] * num_quotient_chunks)]
     input_mmcs = [shard or pcs.mmcs, pcs.mmcs]
+    if pre_width > 0:                                                                    # the preprocessed round last (:379-391)
+        rounds.append((preprocessed.prover_data, [[zeta, zeta_next] if pre_next else [zeta]]))
+        input_mmcs.append(pcs.mmcs)
     opened_values, fri_inputs = pcs.open_values_and_fri_inputs(rounds, challenger, input_mmcs)
     span("open: evaluate + reduce", t0)
 
@@ -271,7 +361,9 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None) -> P
                  commit_pow_witnesses=fri["pow_witnesses"], final_poly=fri["final_poly"], query_pow_witness=fri["query_pow_witness"],
                  query_indices=fri["indices"], input_openings=fri["input_openings"], commit_phase_openings=fri["commit_phase_openings"],
                  degree_bits=log_degree, timings_ms=T, input_opening_indices=fri["input_opening_indices"],
-                 commit_phase_indices=fri["commit_phase_indices"], trace_next=opened_values[0][0][1] if opens_next else None)
+                 commit_phase_indices=fri["commit_phase_indices"], trace_next=opened_values[0][0][1] if opens_next else None,
+                 preprocessed_local=opened_values[2][0][0] if pre_width > 0 else None,
+                 preprocessed_next=opened_values[2][0][1] if pre_next else None)
 
 
 def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list,

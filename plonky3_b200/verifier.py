@@ -1,6 +1,6 @@
 """uni-stark `verify` for proofs in the reference's wire form (proof_io.py), mirroring
 
-    uni-stark/src/verifier.rs:282-561   verify_with_preprocessed (non-ZK, no preprocessed trace)
+    uni-stark/src/verifier.rs:282-561   verify_with_preprocessed (non-ZK; preprocessed and periodic columns)
     fri/src/two_adic_pcs.rs:684-715     TwoAdicFriPcs::verify
     fri/src/verifier.rs:158-436         verify_fri;  :471-606 fold_query;  :617-833 open_inputs
     fri/src/two_adic_pcs.rs:108-131     TwoAdicFriFolding::fold_row
@@ -216,11 +216,36 @@ def verify_fri(e: Ext, params, input_mmcs, proof: dict, challenger, rounds):
             raise VerificationError(f"commit phase MMCS error: {ex}") from None
 
 
-def verify(config, air, proof, public_values=()):
+def eval_periodic_poly(e: Ext, values, point):
+    """fri/src/periodic.rs:209-259: the degree < p interpolant of `values` (canonical) over the subgroup of size p = len(values),
+    at the EF point, by the barycentric form (x^p - 1) / p * sum_i v_i w^i / (x - w^i)."""
+    p = len(values)
+    if p == 1:
+        return e.base(values[0])
+    w = e.root(p.bit_length() - 1)
+    xp1 = e.sub(e.pow(point, p), e.ONE)
+    if not any(xp1):                                               # the point lies on the subgroup
+        wi = 1
+        for v in values:
+            if point == e.base(wi):
+                return e.base(v)
+            wi = wi * w % e.P
+        return e.ZERO
+    acc, wi = e.ZERO, 1
+    for v in values:
+        acc = e.add(acc, e.scale(e.inverse(e.sub(point, e.base(wi))), v * wi % e.P))
+        wi = wi * w % e.P
+    return e.scale(e.mul(xp1, acc), e.inv(p))
+
+
+def verify(config, air, proof, public_values=(), *, preprocessed_vk=None):
     """uni-stark verify.  `proof`: wire bytes, a uni_stark.Proof, or the dict proof_from_postcard returns.  `public_values`: canonical
     integers.  `air` supplies width(), num_public_values(), main_next_row_columns(), max_constraint_degree() and
     eval_folded_constraints(ext, local, next, public_values, is_first_row, is_last_row, is_transition, alpha) (the
-    VerifierConstraintFolder, uni-stark/src/folder.rs).  Returns None; raises VerificationError."""
+    VerifierConstraintFolder, uni-stark/src/folder.rs); an AIR with preprocessed or periodic columns also supplies
+    preprocessed_width(), preprocessed_next_row_columns(), periodic_columns() and takes the keywords preprocessed_local,
+    preprocessed_next and periodic_values in its folder.  `preprocessed_vk`: uni_stark.PreprocessedVerifierKey, required iff the AIR
+    has preprocessed columns.  Returns None; raises VerificationError."""
     from .uni_stark import get_log_num_quotient_chunks
     if hasattr(proof, "to_postcard"):
         proof = proof.to_postcard()
@@ -246,10 +271,25 @@ def verify(config, air, proof, public_values=()):
     else:
         _need(proof["trace_next"] is None, "opened values dimension mismatch")
     _need(len(proof["quotient_chunks"]) == nchunks and all(len(c) == 4 for c in proof["quotient_chunks"]), "opened values dimension mismatch")
+    # process_preprocessed_trace (verifier.rs:203-277): the width is the key's, else the AIR's; the opened rows must match it
+    pre_width = preprocessed_vk.width if preprocessed_vk is not None else int(getattr(air, "preprocessed_width", lambda: 0)())
+    pre_next = len(getattr(air, "preprocessed_next_row_columns", lambda: [])()) > 0
+    pre_local_v, pre_next_v = proof.get("preprocessed_local"), proof.get("preprocessed_next")
+    _need((0 if pre_local_v is None else len(pre_local_v)) == pre_width
+          and (0 if pre_next_v is None else len(pre_next_v)) == (pre_width if pre_next else 0), "preprocessed trace width mismatch")
+    _need((pre_width == 0) == (preprocessed_vk is None), "preprocessed verifier key inconsistent with the AIR")
+    if preprocessed_vk is not None:
+        _need(preprocessed_vk.degree_bits == db, "preprocessed degree mismatch")
+    periodic = [list(c) for c in getattr(air, "periodic_columns", lambda: [])()]
+    from .air import periodic_column_error
+    err = periodic_column_error(periodic, n)                       # check_periodic_column_lengths (verifier.rs:25-50)
+    _need(err is None, f"invalid periodic column: {err}")
 
     ch = config.initialise_challenger()
-    ch.observe_canonical(db); ch.observe_canonical(db); ch.observe_canonical(0)       # degree_bits, base_degree_bits, preprocessed width
+    ch.observe_canonical(db); ch.observe_canonical(db); ch.observe_canonical(pre_width)     # degree_bits, base_degree_bits, preprocessed width
     ch.observe_slice(np.asarray(proof["trace_commit"], dtype=np.uint32))
+    if pre_width > 0:
+        ch.observe_slice(np.asarray(preprocessed_vk.commitment, dtype=np.uint32))
     for v in public_values:
         ch.observe_canonical(v)
     alpha = e.ec(ch.sample_algebra_element())
@@ -265,6 +305,12 @@ def verify(config, air, proof, public_values=()):
     trace_pts = [(zeta, local)] + ([(zeta_next, nxt)] if main_next else [])
     rounds = [(proof["trace_commit"], [(db, trace_pts)]), (proof["quotient_commit"], [(db, [(zeta, c)]) for c in chunks])]
     opened = [proof["trace_local"]] + ([proof["trace_next"]] if main_next else []) + list(proof["quotient_chunks"])
+    pre_local, pre_nxt = None, None
+    if pre_width > 0:                                              # the preprocessed round last
+        pre_local = [e.ec(v) for v in pre_local_v]
+        pre_nxt = [e.ec(v) for v in pre_next_v] if pre_next else [e.ZERO] * pre_width
+        rounds.append((preprocessed_vk.commitment, [(db, [(zeta, pre_local)] + ([(zeta_next, pre_nxt)] if pre_next else []))]))
+        opened += [pre_local_v] + ([pre_next_v] if pre_next else [])
     for ys in opened:                                              # TwoAdicFriPcs::verify: every opened value, in commitment order
         ch.observe_slice(np.asarray(ys, dtype=np.uint32))
     verify_fri(e, params, pcs.mmcs, proof, ch, rounds)
@@ -284,5 +330,10 @@ def verify(config, air, proof, public_values=()):
     is_first = e.mul(z_h, e.inverse(e.sub(zeta, e.ONE)))                       # selectors_at_point, field/src/coset.rs
     is_last = e.mul(z_h, e.inverse(e.sub(zeta, e.base(ginv))))
     is_trans = e.sub(zeta, e.base(ginv))
-    folded = air.eval_folded_constraints(e, local, nxt, list(public_values), is_first, is_last, is_trans, alpha)
+    if pre_width > 0 or periodic:
+        periodic_values = [eval_periodic_poly(e, col, e.pow(zeta, n // len(col))) for col in periodic]
+        folded = air.eval_folded_constraints(e, local, nxt, list(public_values), is_first, is_last, is_trans, alpha,
+                                             preprocessed_local=pre_local, preprocessed_next=pre_nxt, periodic_values=periodic_values)
+    else:
+        folded = air.eval_folded_constraints(e, local, nxt, list(public_values), is_first, is_last, is_trans, alpha)
     _need(e.mul(folded, e.inverse(z_h)) == quotient, "out-of-domain evaluation mismatch")

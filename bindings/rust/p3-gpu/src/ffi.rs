@@ -194,6 +194,9 @@ unsafe extern "C" {
     pub fn p3gpu_challenger_observe(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, h_values: *const u32, n: usize) -> i32;
     pub fn p3gpu_challenger_sample(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, h_out: *mut u32, n: usize) -> i32;
     pub fn p3gpu_challenger_grind(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, bits: c_uint, witness: *mut u32) -> i32;
+    pub fn p3gpu_challenger_new_keccak256(ctx: *mut P3GpuCtx, field: c_int, out: *mut *mut P3GpuChallenger) -> i32;
+    pub fn p3gpu_challenger_observe_digest(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, h_words: *const u32, n: usize) -> i32;
+    pub fn p3gpu_challenger_sample_bits(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, bits: c_uint, n: usize, h_out: *mut u32) -> i32;
 }
 
 /// The reference's prover-side trait methods have no `Result`: shape violations panic (`log2_strict_usize`,

@@ -304,6 +304,20 @@ int32_t p3gpu_challenger_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, uint32_t *
 /* GrindingChallenger::grind (grinding_challenger.rs:100-232): parallel search on the device, returns the SMALLEST witness (what a
  * serial reference build returns), observes it and consumes the checked sample. */
 int32_t p3gpu_challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, uint32_t *witness);
+/* SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>> (challenger/src/serializing_challenger.rs, hash_challenger.rs;
+ * the transcript of the Keccak configuration, examples/src/types.rs:19-35), created empty as by from_hasher(vec![], Keccak256Hash).
+ * Every p3gpu_challenger_* entry point takes either kind of handle.  On this kind `observe` / `observe_dev` take Montgomery words
+ * and absorb the 4 little-endian bytes of each canonical value; `sample` rejection-samples field elements from 4 bytes popped off
+ * the END of the 32-byte digest (masked to 31 bits, resampled while >= p) and returns Montgomery words; `grind` returns the smallest
+ * witness (Montgomery word), observes it and consumes the checked sample. */
+int32_t p3gpu_challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out);
+/* Observe n digest words as the MMCS commits them (a cap, or any digest): on the duplex handle they are field elements (Montgomery
+ * words, as p3gpu_challenger_observe); on the Keccak-256 handle a [u64; 4] digest held as 8 words is observed as its 32
+ * little-endian bytes, i.e. the words' own bytes in order. */
+int32_t p3gpu_challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const uint32_t *h_words, size_t n);
+/* CanSampleBits, n times (synchronous): the duplex handle masks the canonical value of a sampled element; the Keccak-256 handle masks
+ * the raw u32 of 4 popped bytes.  P3GPU_EINVAL unless 2^bits < p, before anything launches. */
+int32_t p3gpu_challenger_sample_bits(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, size_t n, uint32_t *h_out);
 /* Mmcs::open_batch for n indices at once (merkle-tree/src/mmcs/batch.rs:75-121): d_out[q] = row (h_indices[q] >> index_shift) of a
  * device matrix; and the authentication paths: d_out[q][l] = sibling digest at layer l, l < path_len = layers - 1 - cap_height. */
 int32_t p3gpu_gather_rows_dev(p3gpu_ctx *ctx, const uint32_t *d_mat, size_t h, size_t w, const uint32_t *h_indices, size_t n, unsigned index_shift,

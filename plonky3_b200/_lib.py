@@ -32,6 +32,7 @@ EXPORTS = [
     "p3gpu_p2air_generate_trace_cols_dev", "p3gpu_shard_col_segments", "p3gpu_peer_exchange_dev", "p3gpu_p2air_quotient_sharded_dev",
     "p3gpu_air_program_create", "p3gpu_air_program_destroy", "p3gpu_air_program_info", "p3gpu_air_quotient_dev",
     "p3gpu_air_program_create_layout", "p3gpu_air_quotient_layout_dev",
+    "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -130,6 +131,9 @@ def load():
         "p3gpu_air_quotient_dev": (i32, [vp, vp, vp, cu, cu, cu, vp, vp, vp]),
         "p3gpu_air_program_create_layout": (i32, [vp, ci, vp, sz, vp, sz, vp, C.POINTER(vp)]),
         "p3gpu_air_quotient_layout_dev": (i32, [vp, vp, vp, cu, vp, cu, vp, cu, cu, cu, vp, vp, vp]),
+        "p3gpu_challenger_new_keccak256": (i32, [vp, ci, C.POINTER(vp)]),
+        "p3gpu_challenger_observe_digest": (i32, [vp, vp, vp, sz]),
+        "p3gpu_challenger_sample_bits": (i32, [vp, vp, cu, sz, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

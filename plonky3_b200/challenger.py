@@ -1,6 +1,7 @@
 """DuplexChallenger (challenger/src/duplex_challenger.rs:60-300) + GrindingChallenger::grind (grinding_challenger.rs:100-232) with the
 sponge resident on the GPU (csrc/challenger.cu): caps and opened values produced on the device are absorbed there; only sampled
-challenges come back.  Protocol plumbing of the prove driver (uni_stark.py), mirroring the reference's method names."""
+challenges come back.  SerializingChallenger32 over a Keccak-256 HashChallenger is the same on the device for the Keccak
+configuration.  Protocol plumbing of the prove driver (uni_stark.py), mirroring the reference's method names."""
 from __future__ import annotations
 
 import ctypes as C
@@ -73,6 +74,97 @@ class DuplexChallenger:
         """CanSampleBits (duplex_challenger.rs:270-283): canonical value of one sample, masked."""
         assert (1 << bits) < self.field.P
         return self.field.from_monty(self.sample()) & ((1 << bits) - 1)
+
+    # ---- GrindingChallenger
+    def grind(self, bits: int) -> int:
+        w = C.c_uint32()
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_challenger_grind(self.gpu.h, self.h, bits, C.byref(w)))
+        return int(w.value)
+
+
+class SerializingChallenger32:
+    """SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>> (challenger/src/serializing_challenger.rs,
+    hash_challenger.rs): the transcript of the Keccak configuration (examples/src/types.rs:19-35), resident on the GPU like
+    DuplexChallenger and with the same method surface.  Field elements are observed as the 4 little-endian bytes of their canonical
+    values; a [u64; 4] digest (8 words) as its 32 bytes; samples are rejection-sampled from 4 bytes popped off the end of the
+    Keccak-256 digest; `sample_bits` masks the raw u32; `grind` returns the smallest witness.  Values in and out are Montgomery
+    words, as everywhere else in the prover."""
+
+    def __init__(self, field: Field, gpu):
+        self.field, self.gpu = field, gpu
+        h = C.c_void_p()
+        gpu._use_torch_stream()
+        check(gpu.L.p3gpu_challenger_new_keccak256(gpu.h, field.id, C.byref(h)))
+        self.h = h
+
+    @classmethod
+    def from_hasher(cls, initial_state, field: Field, gpu):
+        """from_hasher(initial_state, Keccak256Hash): `initial_state` bytes become the start of the input buffer.  The transcript
+        takes whole 32-bit words, so their number must be a multiple of 4."""
+        init = bytes(initial_state)
+        if len(init) % 4:
+            raise ValueError("the initial state must be a whole number of 32-bit words")
+        c = cls(field, gpu)
+        if init:
+            c._observe_digest(np.frombuffer(init, dtype="<u4").astype(np.uint32))
+        return c
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None) and self.gpu.h:
+                self.gpu.L.p3gpu_challenger_free(self.gpu.h, self.h)
+                self.h = None
+        except Exception:
+            pass
+
+    def clone(self):
+        c = object.__new__(SerializingChallenger32)
+        c.field, c.gpu = self.field, self.gpu
+        h = C.c_void_p()
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_challenger_clone(self.gpu.h, self.h, C.byref(h)))
+        c.h = h
+        return c
+
+    # ---- CanObserve
+    def observe_slice(self, values):
+        """Montgomery words (field elements); a CUDA int32 tensor is absorbed on the device without a copy."""
+        self.gpu._use_torch_stream()
+        if _is_torch(values) and values.is_cuda:
+            v = values.contiguous()
+            check(self.gpu.L.p3gpu_challenger_observe_dev(self.gpu.h, self.h, v.data_ptr(), v.numel()))
+            self._keep = v
+            return
+        v = np.ascontiguousarray(values.cpu().numpy().view(np.uint32) if _is_torch(values) else values, dtype=np.uint32).ravel()
+        check(self.gpu.L.p3gpu_challenger_observe(self.gpu.h, self.h, v.ctypes.data, v.size))
+
+    def _observe_digest(self, words):
+        v = np.ascontiguousarray(words.cpu().numpy().view(np.uint32) if _is_torch(words) else words, dtype=np.uint32).ravel()
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_challenger_observe_digest(self.gpu.h, self.h, v.ctypes.data, v.size))
+
+    def observe(self, value: int): self.observe_slice(np.array([value], dtype=np.uint32))
+    def observe_canonical(self, x: int): self.observe(self.field.to_monty(x))
+    def observe_cap(self, cap): self._observe_digest(cap)                             # CanObserve<MerkleCap<F, [u64; 4]>>: the bytes
+    def observe_algebra_slice(self, ys): self.observe_slice(ys)
+
+    # ---- CanSample
+    def sample_many(self, n: int) -> np.ndarray:
+        out = np.empty(n, dtype=np.uint32)
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_challenger_sample(self.gpu.h, self.h, out.ctypes.data, n))
+        return out
+
+    def sample(self) -> int: return int(self.sample_many(1)[0])
+    def sample_algebra_element(self) -> np.ndarray: return self.sample_many(4)
+
+    def sample_bits(self, bits: int) -> int:
+        """CanSampleBits: the raw u32 of 4 popped bytes, masked (not a reduced field element)."""
+        out = np.empty(1, dtype=np.uint32)
+        self.gpu._use_torch_stream()
+        check(self.gpu.L.p3gpu_challenger_sample_bits(self.gpu.h, self.h, bits, 1, out.ctypes.data))
+        return int(out[0])
 
     # ---- GrindingChallenger
     def grind(self, bits: int) -> int:

@@ -572,6 +572,21 @@ int32_t p3gpu_challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bi
     P3_CHECK(ch && witness, P3GPU_EINVAL, "null argument");
     return challenger_grind(ctx, ch, bits, witness);
 }
+int32_t p3gpu_challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out) {
+    P3_ENTER(ctx);
+    P3_CHECK(out, P3GPU_EINVAL, "null argument");
+    return challenger_new_keccak256(ctx, field, out);
+}
+int32_t p3gpu_challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const uint32_t *h_words, size_t n) {
+    P3_ENTER(ctx);
+    P3_CHECK(ch && (h_words || n == 0), P3GPU_EINVAL, "null argument");
+    return challenger_observe_digest(ctx, ch, h_words, n);
+}
+int32_t p3gpu_challenger_sample_bits(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, size_t n, uint32_t *h_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(ch && (h_out || n == 0), P3GPU_EINVAL, "null argument");
+    return challenger_sample_bits(ctx, ch, bits, n, h_out);
+}
 int32_t p3gpu_gather_rows_dev(p3gpu_ctx *ctx, const uint32_t *d_mat, size_t h, size_t w, const uint32_t *h_indices, size_t n, unsigned index_shift,
                               uint32_t *d_out) {
     P3_ENTER(ctx);

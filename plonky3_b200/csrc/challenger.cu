@@ -11,15 +11,26 @@
 #include "common.h"
 #include "hash_core.cuh"
 
+//
+// The second kind of handle is SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>> (challenger/src/
+// serializing_challenger.rs, hash_challenger.rs), the transcript of the Keccak configuration (examples/src/types.rs:19-35).  The
+// reference keeps every observed byte in an input buffer and hashes all of it when a sample finds the output buffer empty; the
+// digest then becomes both the new input buffer and the output buffer, whose bytes are popped from the end.  Absorbing the input
+// block by block as it fills gives the same digest, so the device keeps a running Keccak state plus the pending partial block (at
+// most 33 words: every input is a whole number of 32-bit words) instead of a buffer that grows with the opened values.
 struct p3gpu_challenger {
+    int kind;           // CH_DUPLEX or CH_KECCAK256
     int field, width, rate;
-    p3::u32 *state;     // device: [0, width) sponge state | [32, 32+rate) input buffer | [64, 64+rate) output buffer | [96] n_in | [97] n_out
+    p3::u32 *state;     // device, duplex: [0, width) sponge state | [32, 32+rate) input buffer | [64, 64+rate) output buffer | [96] n_in | [97] n_out
+                        //         keccak: [0, 50) Keccak state (lo[25], hi[25]) | [64, 98) pending words | [98] n_pending | [100, 108) output words | [108] n_out words
     p3::u32 *stage;     // device staging for host observes / samples (4096 words)
 };
 
 namespace p3 {
 
+constexpr int CH_DUPLEX = 0, CH_KECCAK256 = 1;
 constexpr int CH_IN = 32, CH_OUT = 64, CH_NIN = 96, CH_NOUT = 97, CH_WORDS = 128, CH_STAGE = 4096;
+constexpr int KCH_PEND = 64, KCH_NPEND = 98, KCH_OUT = 100, KCH_NOUT = 108;
 
 template <int F, int W>
 __device__ void ch_duplexing(u32 *st, int rate, const Poseidon2Consts &k) {
@@ -87,6 +98,108 @@ __global__ void __launch_bounds__(128) ch_grind_kernel(const u32 *st, int rate, 
     if ((from_monty<F>(last) & mask) == 0) atomicMin(best, cand);
 }
 
+// ---- SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>> ------------------------------------------------------
+__device__ __forceinline__ void kch_load(const u32 *st, KState &s) {
+#pragma unroll
+    for (int i = 0; i < 25; i++) { s.lo[i] = st[i]; s.hi[i] = st[25 + i]; }
+}
+__device__ __forceinline__ void kch_store(u32 *st, const KState &s) {
+#pragma unroll
+    for (int i = 0; i < 25; i++) { st[i] = s.lo[i]; st[25 + i] = s.hi[i]; }
+}
+__device__ __forceinline__ void kch_full_block(u32 *st, KState &s) {
+    u32 w[KECCAK256_RATE_WORDS];
+#pragma unroll
+    for (int i = 0; i < KECCAK256_RATE_WORDS; i++) w[i] = st[KCH_PEND + i];
+    keccak256_absorb_block(s, w);
+    st[KCH_NPEND] = 0;
+}
+
+// HashChallenger::flush: digest of everything observed; the digest is the new input buffer and the output buffer
+__device__ void kch_flush(u32 *st) {
+    KState s;
+    kch_load(st, s);
+    u32 w[KECCAK256_RATE_WORDS];
+#pragma unroll
+    for (int i = 0; i < KECCAK256_RATE_WORDS; i++) w[i] = st[KCH_PEND + i];
+    keccak256_final_block(s, w, st[KCH_NPEND]);
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const u32 d = keccak256_digest_word(s, k);
+        st[KCH_PEND + k] = d;
+        st[KCH_OUT + k] = d;
+    }
+    for (int i = 0; i < 50; i++) st[i] = 0;
+    st[KCH_NPEND] = 8;
+    st[KCH_NOUT] = 8;
+}
+
+// four bytes popped from the END of the output buffer, as u32::from_le_bytes of the popped order (bytes 31, 30, 29, 28 first)
+__device__ __forceinline__ u32 kch_pop_u32(u32 *st) {
+    if (st[KCH_NOUT] == 0) kch_flush(st);
+    const u32 m = st[KCH_NOUT] - 1;
+    st[KCH_NOUT] = m;
+    return __byte_perm(st[KCH_OUT + m], 0, 0x0123);
+}
+
+// MONTY: observe Montgomery words as the 4 little-endian bytes of their canonical values (CanObserve<F>); otherwise the words'
+// own bytes (a [u64; 4] digest held as 8 words)
+template <int F, bool MONTY>
+__global__ void kch_observe_kernel(u32 *st, const u32 *vals, size_t n) {
+    if (threadIdx.x | blockIdx.x) return;
+    if (n == 0) return;
+    KState s;
+    kch_load(st, s);
+    st[KCH_NOUT] = 0;                                                          // any buffered output is now invalid
+    u32 m = st[KCH_NPEND];
+    for (size_t j = 0; j < n; j++) {
+        st[KCH_PEND + m] = MONTY ? from_monty<F>(vals[j]) : vals[j];
+        if (++m == (u32)KECCAK256_RATE_WORDS) { kch_full_block(st, s); m = 0; }
+    }
+    st[KCH_NPEND] = m;
+    kch_store(st, s);
+}
+
+// raw = false: field elements by rejection sampling of 31-bit values (CanSample<F>), returned as Montgomery words; raw = true: the
+// u32 of 4 popped bytes AND `mask` (CanSampleBits)
+template <int F>
+__global__ void kch_sample_kernel(u32 *st, u32 *out, size_t n, bool raw, u32 mask) {
+    if (threadIdx.x | blockIdx.x) return;
+    for (size_t j = 0; j < n; j++) {
+        if (raw) { out[j] = kch_pop_u32(st) & mask; continue; }
+        u32 v;
+        do { v = kch_pop_u32(st) & 0x7fffffffu; } while (v >= Fp<F>::P);
+        out[j] = to_monty<F>(v);
+    }
+}
+
+// Candidate c is valid iff observe(c); sample_bits(bits) == 0.  The full blocks of the transcript are already absorbed (the
+// midstate); every thread absorbs the pending words, its candidate and the padding — one or two Keccak-f — and takes the first
+// sampled u32, which is the byte-reversed last digest word.  best = smallest valid c.
+template <int F>
+__global__ void __launch_bounds__(128) kch_grind_kernel(const u32 *st, u32 base, u32 count, u32 mask, u32 *best) {
+    const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= count) return;
+    const u32 cand = base + t;
+    if (cand >= Fp<F>::P) return;
+    const u32 n = st[KCH_NPEND];
+    KState s;
+    kch_load(st, s);
+    u32 w[KECCAK256_RATE_WORDS];
+#pragma unroll
+    for (int i = 0; i < KECCAK256_RATE_WORDS; i++) w[i] = (u32)i < n ? st[KCH_PEND + i] : ((u32)i == n ? cand : 0u);
+    u32 tail = n + 1;
+    if (tail == (u32)KECCAK256_RATE_WORDS) { keccak256_absorb_block(s, w); tail = 0; }
+    keccak256_final_block(s, w, tail);
+    const u32 sample = __byte_perm(keccak256_digest_word(s, 7), 0, 0x0123);
+    if ((sample & mask) == 0) atomicMin(best, cand);
+}
+
+template <typename Fn> static int32_t field_dispatch(int field, Fn &&fn) {
+    if (field == BABY_BEAR) return fn(std::integral_constant<int, BABY_BEAR>());
+    return fn(std::integral_constant<int, KOALA_BEAR>());
+}
+
 template <typename Fn> static int32_t ch_dispatch(int field, int width, Fn &&fn) {
     if (field == BABY_BEAR && width == 16) return fn(std::integral_constant<int, BABY_BEAR>(), std::integral_constant<int, 16>());
     if (field == BABY_BEAR && width == 24) return fn(std::integral_constant<int, BABY_BEAR>(), std::integral_constant<int, 24>());
@@ -100,17 +213,25 @@ static int32_t ch_consts(p3gpu_ctx *ctx, const p3gpu_challenger *ch, const Posei
     return P3GPU_OK;
 }
 
-int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out) {
-    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "unknown field %d", field);
-    P3_CHECK(width == 16 || width == 24, P3GPU_EUNSUPPORTED, "challenger permutation width %d unsupported (16 or 24)", width);
-    P3_CHECK(rate > 0 && rate < width && rate <= 24, P3GPU_EINVAL, "challenger rate %d out of range", rate);
+static int32_t challenger_alloc(p3gpu_ctx *ctx, int kind, int field, int width, int rate, p3gpu_challenger **out) {
     p3gpu_challenger *ch = new p3gpu_challenger();
-    ch->field = field; ch->width = width; ch->rate = rate;
+    ch->kind = kind; ch->field = field; ch->width = width; ch->rate = rate;
     if (cudaMalloc(&ch->state, (CH_WORDS + CH_STAGE) * 4) != cudaSuccess) { delete ch; cudaGetLastError(); set_error("cudaMalloc failed"); return P3GPU_ENOMEM; }
     ch->stage = ch->state + CH_WORDS;
     P3_CUDA(cudaMemsetAsync(ch->state, 0, CH_WORDS * 4, ctx->stream));
     *out = ch;
     return P3GPU_OK;
+}
+int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out) {
+    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "unknown field %d", field);
+    P3_CHECK(width == 16 || width == 24, P3GPU_EUNSUPPORTED, "challenger permutation width %d unsupported (16 or 24)", width);
+    P3_CHECK(rate > 0 && rate < width && rate <= 24, P3GPU_EINVAL, "challenger rate %d out of range", rate);
+    return challenger_alloc(ctx, CH_DUPLEX, field, width, rate, out);
+}
+// SerializingChallenger32::from_hasher(vec![], Keccak256Hash): an empty input buffer and an empty output buffer (all-zero state)
+int32_t challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out) {
+    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "unknown field %d", field);
+    return challenger_alloc(ctx, CH_KECCAK256, field, 0, 0, out);
 }
 void challenger_free(p3gpu_ctx *ctx, p3gpu_challenger *ch) {
     if (!ch) return;
@@ -119,12 +240,24 @@ void challenger_free(p3gpu_ctx *ctx, p3gpu_challenger *ch) {
     delete ch;
 }
 int32_t challenger_clone(p3gpu_ctx *ctx, const p3gpu_challenger *src, p3gpu_challenger **out) {
-    P3_TRY(challenger_new(ctx, src->field, src->width, src->rate, out));
+    P3_TRY(challenger_alloc(ctx, src->kind, src->field, src->width, src->rate, out));
     P3_CUDA(cudaMemcpyAsync((*out)->state, src->state, CH_WORDS * 4, cudaMemcpyDeviceToDevice, ctx->stream));
     return P3GPU_OK;
 }
 
+static int32_t kch_observe_dev(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *d_vals, size_t n, bool monty) {
+    if (n == 0) return P3GPU_OK;
+    P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
+        if (monty) kch_observe_kernel<decltype(f)::value, true><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        else kch_observe_kernel<decltype(f)::value, false><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        return P3GPU_OK;
+    }));
+    ctx->launches++;
+    P3_CUDA(cudaGetLastError());
+    return P3GPU_OK;
+}
 int32_t challenger_observe_dev(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *d_vals, size_t n) {
+    if (ch->kind == CH_KECCAK256) return kch_observe_dev(ctx, ch, d_vals, n, true);
     if (n == 0) return P3GPU_OK;
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
@@ -146,9 +279,32 @@ int32_t challenger_observe_host(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 
     }
     return P3GPU_OK;
 }
+// Digests as the MMCS commits them: [F; 8] digests are field elements (the duplex handle observes them like any value); a Keccak
+// MMCS's [u64; 4] digests are observed as their 32 little-endian bytes (CanObserve<MerkleCap<F, [u64; N]>>), the words' own bytes.
+int32_t challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *h_words, size_t n) {
+    if (ch->kind == CH_DUPLEX) return challenger_observe_host(ctx, ch, h_words, n);
+    for (size_t off = 0; off < n; off += CH_STAGE) {
+        const size_t m = std::min<size_t>(CH_STAGE, n - off);
+        P3_CUDA(cudaMemcpyAsync(ch->stage, h_words + off, m * 4, cudaMemcpyHostToDevice, ctx->stream));
+        P3_TRY(kch_observe_dev(ctx, ch, ch->stage, m, false));
+    }
+    return P3GPU_OK;
+}
+static int32_t kch_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size_t n, bool raw, u32 mask) {
+    P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
+        kch_sample_kernel<decltype(f)::value><<<1, 1, 0, ctx->stream>>>(ch->state, ch->stage, n, raw, mask);
+        return P3GPU_OK;
+    }));
+    ctx->launches++;
+    P3_CUDA(cudaGetLastError());
+    P3_CUDA(cudaMemcpyAsync(h_out, ch->stage, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    P3_CUDA(cudaStreamSynchronize(ctx->stream));
+    return P3GPU_OK;
+}
 int32_t challenger_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size_t n) {
     P3_CHECK(n <= (size_t)CH_STAGE, P3GPU_EINVAL, "too many samples in one call");
     if (n == 0) return P3GPU_OK;
+    if (ch->kind == CH_KECCAK256) return kch_sample(ctx, ch, h_out, n, false, 0);
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
     P3_TRY(ch_dispatch(ch->field, ch->width, [&](auto f, auto w) -> int32_t {
@@ -161,12 +317,51 @@ int32_t challenger_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size
     P3_CUDA(cudaStreamSynchronize(ctx->stream));
     return P3GPU_OK;
 }
+// CanSampleBits: the duplex challenger masks the canonical value of a sampled field element (duplex_challenger.rs:270-283); the
+// serializing challenger masks the raw u32 of 4 popped bytes (serializing_challenger.rs sample_bits).  Both need 2^bits < p.
+int32_t challenger_sample_bits(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, size_t n, u32 *h_out) {
+    const u32 p = ch->field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
+    P3_CHECK(bits < 32 && (1ull << bits) < p, P3GPU_EINVAL, "sample_bits(%u): 2^bits must be below the field order", bits);
+    P3_CHECK(n <= (size_t)CH_STAGE, P3GPU_EINVAL, "too many samples in one call");
+    if (n == 0) return P3GPU_OK;
+    if (ch->kind == CH_KECCAK256) return kch_sample(ctx, ch, h_out, n, true, (1u << bits) - 1u);
+    P3_TRY(challenger_sample(ctx, ch, h_out, n));
+    for (size_t i = 0; i < n; i++)
+        h_out[i] = (ch->field == BABY_BEAR ? from_monty<BABY_BEAR>(h_out[i]) : from_monty<KOALA_BEAR>(h_out[i])) & (u32)((1ull << bits) - 1);
+    return P3GPU_OK;
+}
+static int32_t kch_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, u32 *witness_monty) {
+    const u32 p = ch->field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
+    u32 *best = ch->stage + CH_STAGE - 1;
+    const u32 mask = (1u << bits) - 1u, batch = 1u << std::min(22u, bits + 3);
+    u32 found = 0xffffffffu;
+    for (u64 base = 0; base < p && found == 0xffffffffu; base += batch) {
+        P3_CUDA(cudaMemsetAsync(best, 0xff, 4, ctx->stream));
+        P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
+            kch_grind_kernel<decltype(f)::value><<<(batch + 127) / 128, 128, 0, ctx->stream>>>(ch->state, (u32)base, batch, mask, best);
+            return P3GPU_OK;
+        }));
+        ctx->launches++;
+        P3_CUDA(cudaGetLastError());
+        P3_CUDA(cudaMemcpyAsync(&found, best, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        P3_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    P3_CHECK(found != 0xffffffffu, P3GPU_EINVAL, "failed to find proof-of-work witness");
+    const u32 wm = ch->field == BABY_BEAR ? to_monty<BABY_BEAR>(found) : to_monty<KOALA_BEAR>(found);
+    P3_TRY(challenger_observe_host(ctx, ch, &wm, 1));
+    u32 s = 1;
+    P3_TRY(kch_sample(ctx, ch, &s, 1, true, mask));
+    P3_CHECK(s == 0, P3GPU_ECUDA, "proof-of-work witness failed the check");
+    *witness_monty = wm;
+    return P3GPU_OK;
+}
 // grind(bits): smallest witness w (canonical integer; returned in Montgomery form) such that observe(w); sample_bits(bits) == 0.
 // The witness is observed and the sample consumed, exactly like check_witness (grinding_challenger.rs:226-229).
 int32_t challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, u32 *witness_monty) {
     P3_CHECK(bits < 31, P3GPU_EINVAL, "proof-of-work bits %u too large", bits);
     const u32 p = ch->field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
     if (bits == 0) { *witness_monty = 0; return P3GPU_OK; }
+    if (ch->kind == CH_KECCAK256) return kch_grind(ctx, ch, bits, witness_monty);
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
     u32 *best = ch->stage + CH_STAGE - 1;

@@ -193,4 +193,55 @@ __device__ __forceinline__ void keccak_f(KState &s) {
     }
 }
 
+// =================================================================================================
+// Keccak-256 (keccak/src/lib.rs Keccak256Hash = tiny-keccak Keccak::v256)
+// =================================================================================================
+// Rate 136 bytes, Keccak's original padding: 0x01 after the message and 0x80 OR'd into the last byte of the block (not SHA3's
+// 0x06).  Blocks are handled as 34 little-endian 32-bit words, word 2i / 2i + 1 being lane i's lo / hi half.  Every transcript
+// input is a whole number of words (4-byte field elements, 32-byte digests), so the transcript (challenger.cu) uses the word
+// functions; `keccak256` hashes any byte string and is the host tests' entry point.
+constexpr int KECCAK256_RATE_WORDS = 34;
+
+__device__ __forceinline__ void keccak256_absorb_block(KState &s, const u32 (&w)[KECCAK256_RATE_WORDS]) {
+#pragma unroll
+    for (int i = 0; i < KECCAK256_RATE_WORDS / 2; i++) { s.lo[i] ^= w[2 * i]; s.hi[i] ^= w[2 * i + 1]; }
+    keccak_f(s);
+}
+
+// The last block: the first n < 34 words of `w` hold the message tail (the rest is ignored); padding is added and the block
+// absorbed.  The digest is then words 0..7 = lo[0], hi[0], ..., lo[3], hi[3].  Static indices only, so the block stays in
+// registers.
+__device__ __forceinline__ void keccak256_final_block(KState &s, const u32 (&w)[KECCAK256_RATE_WORDS], u32 n) {
+    u32 b[KECCAK256_RATE_WORDS];
+#pragma unroll
+    for (int i = 0; i < KECCAK256_RATE_WORDS; i++) b[i] = ((u32)i < n ? w[i] : 0u) ^ ((u32)i == n ? 0x01u : 0u);
+    b[KECCAK256_RATE_WORDS - 1] ^= 0x80000000u;
+    keccak256_absorb_block(s, b);
+}
+
+__device__ __forceinline__ u32 keccak256_digest_word(const KState &s, int k) { return (k & 1) ? s.hi[k >> 1] : s.lo[k >> 1]; }
+
+__device__ inline void keccak256(const unsigned char *msg, size_t len, unsigned char out[32]) {
+    KState s;
+#pragma unroll
+    for (int i = 0; i < 25; i++) { s.lo[i] = 0; s.hi[i] = 0; }
+    u32 w[KECCAK256_RATE_WORDS];
+    size_t off = 0;
+    for (;;) {
+        const size_t n = len - off < 136 ? len - off : 136;
+        for (int i = 0; i < KECCAK256_RATE_WORDS; i++) w[i] = 0;
+        for (size_t j = 0; j < n; j++) w[j >> 2] |= (u32)msg[off + j] << (8 * (j & 3));
+        off += n;
+        if (n == 136) { keccak256_absorb_block(s, w); continue; }
+        w[n >> 2] ^= 0x01u << (8 * (n & 3));                  // padding inside a partly filled word
+        w[KECCAK256_RATE_WORDS - 1] ^= 0x80000000u;
+        keccak256_absorb_block(s, w);
+        break;
+    }
+    for (int k = 0; k < 8; k++) {
+        const u32 v = keccak256_digest_word(s, k);
+        for (int j = 0; j < 4; j++) out[4 * k + j] = (unsigned char)(v >> (8 * j));
+    }
+}
+
 }  // namespace p3

@@ -25,7 +25,7 @@ from typing import List, Optional
 import numpy as np
 
 from . import _lib
-from .challenger import DuplexChallenger
+from .challenger import DuplexChallenger, SerializingChallenger32
 from .dft import Radix2DitParallel, _log2_strict
 from .field import Field
 from .fri import FriParameters, TwoAdicFriFolding, TwoAdicFriPcs, commit_phase
@@ -154,6 +154,18 @@ class StarkConfig:
 
 
 @dataclass
+class KeccakStarkConfig:
+    """The Keccak configuration (examples/src/proofs.rs:82-124, types.rs:19-35): a Keccak MMCS (MerkleTreeMmcs.keccak) and the
+    transcript SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>>.  Its digests are [u64; 4], which the wire form
+    writes as varints (proof_io.DIGEST_U64X4)."""
+    pcs: TwoAdicFriPcs
+    digest_codec: str = "u64x4"
+
+    def initialise_challenger(self) -> SerializingChallenger32:
+        return SerializingChallenger32.from_hasher([], self.pcs.dft.field, self.pcs.dft.gpu)
+
+
+@dataclass
 class Proof:
     """uni-stark/src/proof.rs:19-62 + fri/src/proof.rs:12-24 as plain arrays (Montgomery words)."""
     trace_commit: np.ndarray
@@ -174,11 +186,12 @@ class Proof:
     preprocessed_next: Optional[np.ndarray] = None    # ... and its preprocessed_next_row_columns() is not empty
     input_opening_indices: list = dc_field(default_factory=list)     # per input batch: the height-reduced query indices
     commit_phase_indices: list = dc_field(default_factory=list)      # per FRI round: the opened group index of every query
+    digest_codec: str = "f8"                      # how the configuration's digests serialise (proof_io: "f8" [F; 8], "u64x4" [u64; 4])
 
     def to_postcard(self) -> bytes:
         """The reference's wire form (`postcard::to_allocvec(&proof)`, uni-stark/tests/fib_air.rs:401-412)."""
         from .proof_io import proof_to_postcard
-        return proof_to_postcard(self)
+        return proof_to_postcard(self, digest=self.digest_codec)
 
 
 @dataclass
@@ -211,7 +224,7 @@ def _air_periodic(air) -> list:
     return list(getattr(air, "periodic_columns", lambda: [])())
 
 
-def setup_preprocessed(config: StarkConfig, air, degree_bits: int):
+def setup_preprocessed(config, air, degree_bits: int):
     """uni-stark/src/preprocessed.rs:46-91: commit the AIR's preprocessed trace on the trace domain of 2^degree_bits rows (same blowup
     as the trace).  Returns (PreprocessedProverData, PreprocessedVerifierKey), or None when the AIR has no preprocessed columns."""
     import torch
@@ -237,7 +250,7 @@ def get_log_num_quotient_chunks(air) -> int:
     return max(d - 2, 0).bit_length()
 
 
-def verify(config: StarkConfig, air, proof, public_values=(), *, preprocessed_vk: Optional[PreprocessedVerifierKey] = None):
+def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[PreprocessedVerifierKey] = None):
     """uni-stark/src/verifier.rs:282-295 (verify_with_preprocessed).  Raises verifier.VerificationError."""
     from .verifier import verify as _verify
     if preprocessed_vk is None:
@@ -245,9 +258,10 @@ def verify(config: StarkConfig, air, proof, public_values=(), *, preprocessed_vk
     return _verify(config, air, proof, public_values, preprocessed_vk=preprocessed_vk)
 
 
-def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
-    """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device
-    (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
+def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
+    """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
+    call goes through the challenger it initialises.  `air`: VectorizedPoseidon2Air or air.SymbolicAir.  `trace`: device (CUDA int32)
+    matrix of height 2^n.  `public_values`: canonical integers.
 
     `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
     after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is
@@ -363,7 +377,8 @@ def prove(config: StarkConfig, air, trace, public_values=(), *, shard=None, prep
                  degree_bits=log_degree, timings_ms=T, input_opening_indices=fri["input_opening_indices"],
                  commit_phase_indices=fri["commit_phase_indices"], trace_next=opened_values[0][0][1] if opens_next else None,
                  preprocessed_local=opened_values[2][0][0] if pre_width > 0 else None,
-                 preprocessed_next=opened_values[2][0][1] if pre_next else None)
+                 preprocessed_next=opened_values[2][0][1] if pre_next else None,
+                 digest_codec=getattr(config, "digest_codec", "f8"))
 
 
 def prove_fri(pcs: TwoAdicFriPcs, inputs: list, challenger: DuplexChallenger, prover_data_with_opening_points: list,

@@ -107,6 +107,13 @@ def fold_row(e: Ext, index: int, log_height: int, log_arity: int, beta, evals):
     return acc
 
 
+def _observe_cap(challenger, cap):
+    """Observe a commitment as digests, not as field elements: a byte transcript (SerializingChallenger32 over a Keccak MMCS) absorbs a
+    [u64; 4] digest as its 32 bytes, which the words' canonical values are not.  A transcript without observe_cap only ever sees
+    [F; 8] digests, which are field elements."""
+    getattr(challenger, "observe_cap", challenger.observe_slice)(np.asarray(cap, dtype=np.uint32))
+
+
 def _check_witness(challenger, e: Ext, bits: int, witness_word: int) -> bool:
     """GrindingChallenger::check_witness (grinding_challenger.rs:60-70)."""
     if bits == 0:
@@ -134,7 +141,7 @@ def verify_fri(e: Ext, params, input_mmcs, proof: dict, challenger, rounds):
     _need(len(proof["commit_pow_witnesses"]) == len(proof["commit_phase_commits"]), "commit PoW witness count mismatch")
     betas = []
     for cap, wit in zip(proof["commit_phase_commits"], proof["commit_pow_witnesses"]):
-        challenger.observe_slice(np.asarray(cap, dtype=np.uint32))
+        _observe_cap(challenger, cap)
         _need(_check_witness(challenger, e, params.commit_proof_of_work_bits, wit), "invalid proof-of-work witness")
         betas.append(e.ec(challenger.sample_algebra_element()))
     final_poly = [e.ec(co) for co in proof["final_poly"]]
@@ -245,13 +252,15 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk=None):
     VerifierConstraintFolder, uni-stark/src/folder.rs); an AIR with preprocessed or periodic columns also supplies
     preprocessed_width(), preprocessed_next_row_columns(), periodic_columns() and takes the keywords preprocessed_local,
     preprocessed_next and periodic_values in its folder.  `preprocessed_vk`: uni_stark.PreprocessedVerifierKey, required iff the AIR
-    has preprocessed columns.  Returns None; raises VerificationError."""
+    has preprocessed columns.  `config.digest_codec` (default "f8") selects the wire form of digests: "u64x4" for the Keccak
+    configuration (uni_stark.KeccakStarkConfig).  Returns None; raises VerificationError."""
     from .uni_stark import get_log_num_quotient_chunks
+    digest = getattr(config, "digest_codec", "f8")                # [F; 8] digests unless the configuration says otherwise
     if hasattr(proof, "to_postcard"):
         proof = proof.to_postcard()
     if isinstance(proof, (bytes, bytearray)):
         try:
-            proof = proof_from_postcard(bytes(proof), config.pcs.dft.field.P)
+            proof = proof_from_postcard(bytes(proof), config.pcs.dft.field.P, digest=digest)
         except ValueError as ex:
             raise VerificationError(f"malformed proof: {ex}") from None
     pcs = config.pcs
@@ -287,13 +296,13 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk=None):
 
     ch = config.initialise_challenger()
     ch.observe_canonical(db); ch.observe_canonical(db); ch.observe_canonical(pre_width)     # degree_bits, base_degree_bits, preprocessed width
-    ch.observe_slice(np.asarray(proof["trace_commit"], dtype=np.uint32))
+    _observe_cap(ch, proof["trace_commit"])
     if pre_width > 0:
-        ch.observe_slice(np.asarray(preprocessed_vk.commitment, dtype=np.uint32))
+        _observe_cap(ch, preprocessed_vk.commitment)
     for v in public_values:
         ch.observe_canonical(v)
     alpha = e.ec(ch.sample_algebra_element())
-    ch.observe_slice(np.asarray(proof["quotient_commit"], dtype=np.uint32))
+    _observe_cap(ch, proof["quotient_commit"])
     zeta = e.ec(ch.sample_algebra_element())
     z_h = e.sub(e.pow(zeta, n), e.ONE)
     _need(any(z_h), "out-of-domain point lies in the trace domain")

@@ -226,6 +226,23 @@ int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, cons
 int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms,
                                             size_t col0, size_t col1, uint32_t *d_out);
 
+/* ---- Keccak-f AIR: the AIR of prove_prime_field_31 -o keccak-f-permutations (keccak-air/src), BabyBear and KoalaBear -------
+ * One Keccak-f round per row, 24 rows per permutation, P3GPU_KECCAK_AIR_COLS columns (columns.rs KeccakCols); 3182 constraints of
+ * degree 3, so two quotient chunks (log_blowup >= 1). */
+#define P3GPU_KECCAK_AIR_COLS 2633
+/* generate_trace_rows (keccak-air/src/generation.rs:16-64): d_inputs n_hashes x 25 u64 (input[x + 5 y] = state[x][y]) -> d_trace,
+ * H x P3GPU_KECCAK_AIR_COLS Montgomery words with H = (24 n_hashes).next_power_of_two() (1 for n_hashes = 0), padding included
+ * (the zero-input permutation's rows, repeated, the last copy cut).  d_inputs 8-byte aligned (may be NULL iff n_hashes = 0),
+ * d_trace 4-byte aligned. */
+int32_t p3gpu_keccak_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint64_t *d_inputs, size_t n_hashes, uint32_t *d_trace);
+/* quotient_values (uni-stark/src/prover.rs:462-827) of the Keccak AIR over GENERATOR * K, |K| = 2^(log_trace_height + 1), from the
+ * first 2^(log_trace_height + 1) rows of the committed bit-reversed trace LDE d_lde (2^log_lde_height rows x P3GPU_KECCAK_AIR_COLS).
+ * d_quotient: 2^(log_trace_height + 1) EF4 values in NATURAL order.  P3GPU_EINVAL before any launch: a NULL or non-4-byte-aligned
+ * pointer, log_trace_height + 1 > log_lde_height, log_lde_height above the field's two-adicity, alpha not canonical;
+ * P3GPU_EUNSUPPORTED: a field other than BabyBear / KoalaBear. */
+int32_t p3gpu_keccak_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient);
+
 /* ---- any AIR as a constraint program (DESIGN.md section 4.7) ----------------------------------------------------------------
  * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
  * (operands refer only to earlier nodes) plus the list of constrained nodes in assertion order.  The library compiles it once

@@ -212,6 +212,17 @@ struct AirDomain {
     u32 periodic_mask;          // rows of the periodic table - 1 (natural index i reads row i & periodic_mask)
 };
 
+// selectors_on_coset (commit/src/domain.rs:321-361) at x_i = g * w_q^i, unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1.
+// zh = Z_H(x_i).  Shared by the constraint-program kernel and the hand-written Keccak AIR kernel (keccak_air.cu).
+template <int F> __host__ __device__ __forceinline__ void air_selectors(const AirDomain &d, u32 i, u32 zh, u32 &first, u32 &last, u32 &trans) {
+    const u32 x = mont_mul<F>(d.shift, fp_pow<F>(d.w_q, i));
+    const u32 a = fp_sub<F>(x, Fp<F>::ONE), b = fp_sub<F>(x, d.w_n_inv);
+    const u32 inv_ab = fp_inv<F>(mont_mul<F>(a, b));          // one inversion for both denominators
+    first = mont_mul<F>(zh, mont_mul<F>(b, inv_ab));
+    last = mont_mul<F>(zh, mont_mul<F>(a, inv_ab));
+    trans = b;
+}
+
 // Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),
 // the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).  EXT (a program that reads
 // preprocessed or periodic columns) compiles in opcodes 12-14: Env then also supplies set_ext_rows(m, m_next, periodic_row),
@@ -227,16 +238,7 @@ __host__ __device__ __forceinline__ uint4 air_row_quotient(Env &env, const AirDo
     env.set_rows(m, mn);
     if constexpr (EXT) env.set_ext_rows(m, mn, i & d.periodic_mask);
     u32 first = 0, last = 0, trans = 0;
-    if (d.uses & AIR_USES_SELECTORS) {
-        // selectors_on_coset (commit/src/domain.rs:321-361), unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1
-        const u32 x = mont_mul<F>(d.shift, fp_pow<F>(d.w_q, i));
-        const u32 zh = env.zh(i);
-        const u32 a = fp_sub<F>(x, Fp<F>::ONE), b = fp_sub<F>(x, d.w_n_inv);
-        const u32 inv_ab = fp_inv<F>(mont_mul<F>(a, b));          // one inversion for both denominators
-        first = mont_mul<F>(zh, mont_mul<F>(b, inv_ab));
-        last = mont_mul<F>(zh, mont_mul<F>(a, inv_ab));
-        trans = b;
-    }
+    if (d.uses & AIR_USES_SELECTORS) air_selectors<F>(d, i, env.zh(i), first, last, trans);
     u64 acc[4] = {0, 0, 0, 0};
     for (u32 pc = 0; pc < n_insns; pc++) {
         const AirInsn in = env.insn(pc);

@@ -497,6 +497,21 @@ int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vecto
     return air_generate_trace_cols(ctx, field, vector_len, d_inputs, n_perms, col0, col1, d_out);
 }
 
+// ---- Keccak-f AIR: trace generation + quotient (keccak_air.cu) ----------------------------------------
+int32_t p3gpu_keccak_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint64_t *d_inputs, size_t n_hashes, uint32_t *d_trace) {
+    P3_ENTER(ctx);
+    P3_CHECK((d_inputs || n_hashes == 0) && d_trace, P3GPU_EINVAL, "null argument");
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 8 == 0 && reinterpret_cast<uintptr_t>(d_trace) % 4 == 0, P3GPU_EINVAL,
+             "Keccak AIR trace: misaligned buffer");
+    return keccak_air_generate(ctx, field, d_inputs, n_hashes, d_trace);
+}
+int32_t p3gpu_keccak_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return keccak_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+
 // ---- any AIR as a constraint program (air_program.cu) -------------------------------------------------
 int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
                                  size_t n_constraints, uint32_t width, uint32_t n_public, p3gpu_air_program **out) {

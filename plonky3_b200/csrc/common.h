@@ -164,6 +164,11 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, cons
                              unsigned log_pre, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n,
                              const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
 
+// keccak_air.cu: Keccak-f AIR trace generation / quotient
+size_t keccak_air_height(size_t n_hashes);
+int32_t keccak_air_generate(p3gpu_ctx *ctx, int field, const u64 *d_inputs, size_t n_hashes, u32 *d_trace);
+int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);
 void challenger_free(p3gpu_ctx *ctx, p3gpu_challenger *ch);

@@ -295,6 +295,34 @@ class Gpu:
         check(self.L.p3gpu_p2air_quotient_dev(self.h, field, vector_len, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    # ------------------------------------------------------------------ Keccak-f AIR
+    @staticmethod
+    def keccak_air_height(n_hashes: int) -> int:
+        """(24 n).next_power_of_two(): the trace height of n permutations (1 for n = 0)."""
+        return 1 << max(24 * int(n_hashes) - 1, 0).bit_length()
+
+    def keccak_air_generate_trace(self, field, inputs_dev):
+        """(n, 25) contiguous CUDA int64 tensor of u64 lanes (input[x + 5 y] = state[x][y]) -> the (H, 2633) trace, padding included."""
+        import torch
+        assert inputs_dev.is_cuda and inputs_dev.dtype == torch.int64 and inputs_dev.is_contiguous(), "inputs: contiguous CUDA int64 (n, 25)"
+        assert inputs_dev.dim() == 2 and int(inputs_dev.shape[1]) == 25
+        self._use_torch_stream()
+        n = int(inputs_dev.shape[0])
+        out = self._empty((self.keccak_air_height(n), _lib.KECCAK_AIR_COLS))
+        check(self.L.p3gpu_keccak_air_generate_trace_dev(self.h, field, inputs_dev.data_ptr() if n else None, n, out.data_ptr()))
+        return out
+
+    def keccak_air_quotient(self, field, lde_dev, log_trace_height, alpha):
+        """Quotient values (2^(log_trace_height + 1), 4) in natural order over GENERATOR * K from the first 2^(log_trace_height + 1)
+        rows of the committed bit-reversed LDE."""
+        m = self._dev(lde_dev); self._use_torch_stream()
+        H = int(m.shape[0]); log_h = H.bit_length() - 1
+        if H != 1 << log_h or int(m.shape[1]) != _lib.KECCAK_AIR_COLS:
+            raise _lib.P3GpuError(f"LDE of shape {tuple(m.shape)}: need 2^k rows x {_lib.KECCAK_AIR_COLS}", _lib.EINVAL)
+        q = self._empty((2 << log_trace_height, 4))
+        check(self.L.p3gpu_keccak_air_quotient_dev(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
+
     # ------------------------------------------------------------------ any AIR as a constraint program
     def air_program_create(self, field, nodes, constraints, width, n_public):
         """Compile an expression DAG: nodes (n, 4) uint32 rows (op, a, b, imm), constraints: node indices in assertion order.

@@ -274,9 +274,12 @@ class SymbolicAir:
         return max(self.constraint_degrees(), default=0)
 
     # ---- prover: the quotient on the device
-    def program(self):
+    def _need_gpu(self, what):
         if self.gpu is None:
-            raise _lib.P3GpuError("quotient evaluation needs a GPU context (no CPU fallback)")
+            raise _lib.P3GpuError(f"{what} needs a GPU context (no CPU fallback)")
+
+    def program(self):
+        self._need_gpu("quotient evaluation")
         if self._program is None:
             if self._has_layout():
                 layout = (self.width(), self.num_public_values(), self.preprocessed_width(), self.num_periodic_columns())

@@ -19,7 +19,6 @@ from __future__ import annotations
 
 import numpy as np
 
-from . import _lib
 from .air import SymbolicAir
 from .field import Field
 
@@ -196,10 +195,6 @@ class KeccakAir(SymbolicAir):
     def __init__(self, field: Field, gpu=None):
         super().__init__(field, WIDTH, eval_keccak, gpu=gpu)
 
-    def _need_gpu(self, what):
-        if self.gpu is None:
-            raise _lib.P3GpuError(f"{what} needs a GPU context (no CPU fallback)")
-
     def generate_trace_rows(self, inputs_dev):
         """generate_trace_rows (keccak-air/src/generation.rs:16-64): (n, 25) device int64 tensor of u64 lanes, input[x + 5 y] =
         state[x][y] -> the ((24 n).next_power_of_two(), 2633) device trace, padding included."""
@@ -215,10 +210,12 @@ class KeccakAir(SymbolicAir):
             x = x.to(f"cuda:{self.gpu.device}")
         return self.generate_trace_rows(x)
 
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=()):
+    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
         """uni-stark/src/prover.rs:462-827 on the hand-written kernel: `trace_lde_dev` holds the trace on GENERATOR * K, |K| = 2N, in
         bit-reversed row order (the committed LDE's prefix).  Returns (2N, 4) in natural order."""
         if len(public_values) != 0:
             raise ValueError(f"{len(public_values)} public values given, the Keccak AIR has none")
+        if preprocessed_on_quotient_domain is not None:
+            raise ValueError("the Keccak AIR has no preprocessed columns")
         self._need_gpu("quotient evaluation")
         return self.gpu.keccak_air_quotient(self.field.id, trace_lde_dev, int(log_degree), alpha)

@@ -1,20 +1,24 @@
-"""uni-stark `prove` with every data-parallel step on the GPU, for the Poseidon2 AIR — the BASELINE config-5 benchmark
-(`prove_prime_field_31 --field koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel
--m poseidon-2`).  Mirrors uni-stark/src/prover.rs:87-442 (prove_with_preprocessed) and fri/src/prover.rs:43-160 (prove_fri) with
-the reference's names; host code is only the protocol sequencing (the transcript's sponge itself runs on the device,
-challenger.py).  Non-ZK, no preprocessed columns, no public values — what the example binary proves
-(examples/src/proofs.rs:120-170) — and for any AIR given as symbolic constraints (air.SymbolicAir: public values, next-row
-openings, any number of quotient chunks up to the blowup, preprocessed columns committed once by `setup_preprocessed`, periodic
-columns), whose quotient is p3gpu_air_quotient_dev / p3gpu_air_quotient_layout_dev.  `prove` is the one
-protocol sequence: with `shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns
-split over several GPUs, the shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
+"""uni-stark `prove` and `verify` with every data-parallel step on the GPU.  Mirrors uni-stark/src/prover.rs:87-442
+(prove_with_preprocessed) and fri/src/prover.rs:43-160 (prove_fri) with the reference's names; host code is only the protocol
+sequencing (the transcript's sponge itself runs on the device, challenger.py).  Non-ZK.
+
+`prove` is the one protocol sequence, for any AIR in air.SymbolicAir's surface: public values, next-row openings, any number of
+quotient chunks up to the blowup, preprocessed columns committed once by `setup_preprocessed`, periodic columns.  The AIR evaluates
+its own quotient on the device: a plain SymbolicAir through the constraint-program kernel (p3gpu_air_quotient_dev /
+p3gpu_air_quotient_layout_dev); poseidon2_air.VectorizedPoseidon2Air, the config-5 benchmark's AIR (`prove_prime_field_31 --field
+koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`), and
+keccak_air.KeccakAir through their hand-written kernels.  With `shard=distributed.ShardedTrace(...)` the same lines prove the
+Poseidon2 AIR with the trace's columns split over several GPUs, the shard standing in for the trace commit, the quotient values and
+the trace's row reads of the opening.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
-    alpha <- transcript;  quotient values on GENERATOR * K ................... p3gpu_p2air_quotient_dev
-    commit_quotient (2 chunks) ................................................ LDE + Merkle as above
+    alpha <- transcript;  quotient values on GENERATOR * K ................... air.quotient_values (p3gpu_p2air_quotient_dev, ...)
+    commit_quotient (2 chunks for degree 3) ................................... LDE + Merkle as above
     zeta <- transcript;  pcs.open: opened values + reduced openings .......... p3gpu_open_* / columnwise / rowwise dot kernels
     prove_fri: commit phase (fold + commit per round), grind, query openings . p3gpu_fri_fold_dev, p3gpu_challenger_grind,
                                                                                p3gpu_gather_rows_dev / p3gpu_merkle_paths_dev
+
+RoundConstants, VectorizedPoseidon2Air and VECTOR_LEN live in poseidon2_air and are re-exported here.
 """
 from __future__ import annotations
 
@@ -24,122 +28,12 @@ from typing import List, Optional
 
 import numpy as np
 
-from . import _lib
 from .challenger import DuplexChallenger, SerializingChallenger32
 from .dft import Radix2DitParallel, _log2_strict
-from .field import Field
 from .fri import FriParameters, TwoAdicFriFolding, TwoAdicFriPcs, commit_phase
 from .merkle_tree import MerkleTreeMmcs
 from .poseidon2 import Poseidon2
-
-VECTOR_LEN = 8           # examples/src/airs.rs: P2_VECTOR_LEN = 1 << 3
-
-
-@dataclass
-class RoundConstants:
-    """poseidon2-air/src/constants.rs:28-57 (Montgomery form)."""
-    beginning_full_round_constants: np.ndarray    # (4, 16)
-    partial_round_constants: np.ndarray           # (rounds_p,)
-    ending_full_round_constants: np.ndarray       # (4, 16)
-
-
-class VectorizedPoseidon2Air:
-    """VectorizedPoseidon2Air<KoalaBear, ..., WIDTH 16, SBOX_DEGREE 3, SBOX_REGISTERS 0, 4, 20, VECTOR_LEN 8> on the GPU."""
-
-    def __init__(self, field: Field, constants: RoundConstants, gpu, vector_len: int = VECTOR_LEN):
-        self.field, self.constants, self.gpu, self.vector_len = field, constants, gpu, vector_len
-        self.rounds_p = int(np.asarray(constants.partial_round_constants).size)
-        self._upload()
-
-    def _upload(self):
-        c = self.constants
-        if self.gpu is None:                     # verifier-only use: the constraint folder below is host code
-            return
-        self.gpu.p2air_set_constants(self.field.id, c.beginning_full_round_constants, c.partial_round_constants, c.ending_full_round_constants)
-
-    def width(self) -> int:                      # BaseAir::width (vectorized.rs)
-        return self.vector_len * (144 + self.rounds_p)
-
-    def max_constraint_degree(self) -> int:      # air.rs:151-160 for (3, 0)
-        return 3
-
-    def num_public_values(self) -> int: return 0
-    def main_next_row_columns(self): return []   # no transition constraints: the next row is never opened (verifier.rs:431-440)
-
-    def eval_folded_constraints(self, e, local, nxt, public_values, is_first_row, is_last_row, is_transition, alpha):
-        """The verifier's constraint folder (uni-stark/src/folder.rs VerifierConstraintFolder: acc = acc * alpha + c per
-        assert_zero) over the opened row at zeta, scalar host code on canonical EF4 values (`e`: verifier.Ext).  Constraint order =
-        poseidon2-air/src/air.rs eval: per permutation the committed post-state of every full round (16 each) and the S-box output
-        of every partial round; degree-3 S-box without registers."""
-        f, P = self.field, self.field.P
-        c = self.constants
-        beg = [[f.from_monty(int(v)) for v in r] for r in np.asarray(c.beginning_full_round_constants).reshape(4, 16)]
-        end = [[f.from_monty(int(v)) for v in r] for r in np.asarray(c.ending_full_round_constants).reshape(4, 16)]
-        part = [f.from_monty(int(v)) for v in np.asarray(c.partial_round_constants).ravel()]
-        ip = lambda k: pow(pow(2, k, P), P - 2, P)
-        # internal diagonal of Poseidon2KoalaBear<16> (koala-bear/src/poseidon2.rs:410-428)
-        v16 = [P - 2, 1, 2, ip(1), 3, 4, P - ip(1), P - 3, P - 4, ip(8), ip(3), ip(24), P - ip(8), P - ip(3), P - ip(4), P - ip(24)]
-        add, sc, mul = e.add, e.scale, e.mul
-
-        def mat4(x):
-            a, b, cc, d = x
-            return [add(add(sc(a, 2), sc(b, 3)), add(cc, d)), add(add(a, sc(b, 2)), add(sc(cc, 3), d)),
-                    add(add(a, b), add(sc(cc, 2), sc(d, 3))), add(add(sc(a, 3), b), add(cc, sc(d, 2)))]
-
-        def mds(s):
-            s = sum((mat4(s[i:i + 4]) for i in range(0, 16, 4)), [])
-            t = [[0, 0, 0, 0] for _ in range(4)]
-            for i in range(16):
-                t[i % 4] = add(t[i % 4], s[i])
-            return [add(s[i], t[i % 4]) for i in range(16)]
-
-        cube = lambda x: mul(mul(x, x), x)
-        cols = 144 + self.rounds_p
-        acc = [0, 0, 0, 0]
-        for v in range(self.vector_len):
-            col = local[v * cols:(v + 1) * cols]
-            s = mds(col[:16]); k = 16
-            for rc in beg:
-                s = mds([cube(add(s[i], e.base(rc[i]))) for i in range(16)])
-                for i in range(16):
-                    acc = add(mul(acc, alpha), e.sub(s[i], col[k + i])); s[i] = col[k + i]
-                k += 16
-            for r in range(self.rounds_p):
-                x = cube(add(s[0], e.base(part[r])))
-                acc = add(mul(acc, alpha), e.sub(x, col[k])); s[0] = col[k]; k += 1
-                t = [0, 0, 0, 0]
-                for i in range(16):
-                    t = add(t, s[i])
-                s = [add(sc(s[i], v16[i]), t) for i in range(16)]
-            for rc in end:
-                s = mds([cube(add(s[i], e.base(rc[i]))) for i in range(16)])
-                for i in range(16):
-                    acc = add(mul(acc, alpha), e.sub(s[i], col[k + i])); s[i] = col[k + i]
-                k += 16
-        return acc
-
-    def generate_trace_rows(self, inputs_dev):
-        """generate_vectorized_trace_rows (generation.rs:14-70): (n_perms, 16) device inputs -> (n_perms / 8, 1312) device trace."""
-        if self.gpu is None:
-            raise _lib.P3GpuError("trace generation needs a GPU context (no CPU fallback)")
-        self._upload()
-        return self.gpu.p2air_generate_trace(self.field.id, inputs_dev, self.vector_len)
-
-    def generate_trace_cols(self, inputs_dev, col0: int, col1: int):
-        """Columns [col0, col1) of `generate_trace_rows(inputs_dev)` without building the full trace: one rank's column block
-        for `distributed.prove_sharded`."""
-        if self.gpu is None:
-            raise _lib.P3GpuError("trace generation needs a GPU context (no CPU fallback)")
-        self._upload()
-        return self.gpu.p2air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1), self.vector_len)
-
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=()):
-        """uni-stark/src/prover.rs:462-827 on the committed LDE (natural order over the quotient domain)."""
-        assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
-        if self.gpu is None:
-            raise _lib.P3GpuError("quotient evaluation needs a GPU context (no CPU fallback)")
-        self._upload()
-        return self.gpu.p2air_quotient(self.field.id, trace_lde_dev, log_degree, alpha, self.vector_len)
+from .poseidon2_air import VECTOR_LEN, RoundConstants, VectorizedPoseidon2Air  # noqa: F401  (re-exported)
 
 
 @dataclass
@@ -212,23 +106,11 @@ class PreprocessedProverData:
     prover_data: object
 
 
-def _air_preprocessed_width(air) -> int:
-    return int(getattr(air, "preprocessed_width", lambda: 0)())
-
-
-def _air_pre_next(air) -> bool:
-    return len(getattr(air, "preprocessed_next_row_columns", lambda: [])()) > 0
-
-
-def _air_periodic(air) -> list:
-    return list(getattr(air, "periodic_columns", lambda: [])())
-
-
 def setup_preprocessed(config, air, degree_bits: int):
     """uni-stark/src/preprocessed.rs:46-91: commit the AIR's preprocessed trace on the trace domain of 2^degree_bits rows (same blowup
     as the trace).  Returns (PreprocessedProverData, PreprocessedVerifierKey), or None when the AIR has no preprocessed columns."""
     import torch
-    width = _air_preprocessed_width(air)
+    width = air.preprocessed_width()
     if width == 0:
         return None
     trace = air.preprocessed_trace()
@@ -260,8 +142,8 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
 
 def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
     """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
-    call goes through the challenger it initialises.  `air`: VectorizedPoseidon2Air, keccak_air.KeccakAir or air.SymbolicAir.  `trace`: device (CUDA int32)
-    matrix of height 2^n.  `public_values`: canonical integers.
+    call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air or
+    keccak_air.KeccakAir.  `trace`: device (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
 
     `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
     after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is
@@ -288,8 +170,8 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
     log_degree = _log2_strict(degree)
     log_num_quotient_chunks = get_log_num_quotient_chunks(air)
     num_quotient_chunks = 1 << log_num_quotient_chunks
-    pre_width = _air_preprocessed_width(air)
-    periodic = _air_periodic(air)
+    pre_width = air.preprocessed_width()
+    periodic = air.periodic_columns()
     if pre_width > 0 and preprocessed is None:
         raise ValueError(f"the AIR has {pre_width} preprocessed columns: call setup_preprocessed and pass its prover data")
     if preprocessed is not None:
@@ -309,7 +191,7 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
         raise ValueError(f"constraint degree {air.max_constraint_degree()} needs {num_quotient_chunks} quotient chunks: log_blowup "
                          f"{pcs.fri.log_blowup} < {log_num_quotient_chunks}")
     opens_next = len(air.main_next_row_columns()) > 0
-    pre_next = pre_width > 0 and _air_pre_next(air)
+    pre_next = pre_width > 0 and len(air.preprocessed_next_row_columns()) > 0
     challenger = config.initialise_challenger()
     trace_domain = pcs.natural_domain_for_degree(degree)
 
@@ -334,13 +216,10 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
     quotient_domain = (f.mul(trace_domain[0], f.generator), log_degree + log_num_quotient_chunks)      # create_disjoint_domain
     if shard is None:
         trace_on_quotient_domain = pcs.get_evaluations_on_domain(trace_data, 0, quotient_domain).bit_reverse_rows()
-        if pre_width > 0 or periodic:
-            pre_q = (pcs.get_evaluations_on_domain(preprocessed.prover_data, 0, quotient_domain).bit_reverse_rows()
-                     if pre_width > 0 else None)                                           # :272
-            quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values,
-                                                preprocessed_on_quotient_domain=pre_q)
-        else:
-            quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values)  # natural order = flatten_to_base
+        pre_q = (pcs.get_evaluations_on_domain(preprocessed.prover_data, 0, quotient_domain).bit_reverse_rows()
+                 if pre_width > 0 else None)                                               # :272
+        quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values,   # natural order = flatten_to_base
+                                            preprocessed_on_quotient_domain=pre_q)
     else:
         quotient_flat = shard.quotient_values(air, quotient_domain, alpha)
     span("compute quotient polynomial", t0)

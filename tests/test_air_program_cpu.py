@@ -18,7 +18,8 @@ from plonky3_b200 import _lib
 from plonky3_b200.air import (ADD, CONST, IS_FIRST_ROW, IS_LAST_ROW, IS_TRANSITION, MAIN_LOCAL, MAIN_NEXT, MUL, NEG, PUBLIC, SUB,
                               SymbolicAir)
 from plonky3_b200.field import BabyBear, KoalaBear
-from plonky3_b200.uni_stark import RoundConstants, get_log_num_quotient_chunks
+from plonky3_b200.poseidon2_air import RoundConstants, VectorizedPoseidon2Air, poseidon2_eval
+from plonky3_b200.uni_stark import get_log_num_quotient_chunks
 
 ROOT = pathlib.Path(__file__).resolve().parent.parent
 GOLD = ROOT / "tests" / "golden"
@@ -111,7 +112,7 @@ def test_degree_inference_matches_the_reference():
                 assert air.max_constraint_degree() == deg
                 assert get_log_num_quotient_chunks(air) == (deg - 1 - 1).bit_length()     # log2_ceil(deg - 1)
                 assert len(air.constraints) == 20 * (1 + boundary + transition)
-    ev, width = E.poseidon2_eval(KoalaBear, _p2_constants())
+    ev, width = poseidon2_eval(KoalaBear, _p2_constants())
     p2 = SymbolicAir(KoalaBear, width, ev, main_next_row_columns=[])
     assert (width, p2.max_constraint_degree(), len(p2.constraints), get_log_num_quotient_chunks(p2)) == (1312, 3, 8 * 148, 1)
     # a hint overrides the inferred degree (uni-stark/src/symbolic.rs)
@@ -168,7 +169,7 @@ def test_deep_chains_reuse_slots(checker, f):
 
 
 def _example_airs():
-    p2_ev, p2_w = E.poseidon2_eval(KoalaBear, _p2_constants(), vector_len=1)
+    p2_ev, p2_w = poseidon2_eval(KoalaBear, _p2_constants(), vector_len=1)
     return {
         "fibonacci": (BabyBear, SymbolicAir(BabyBear, 2, E.fib_eval, 3), 3, 0),
         "mul_air_3": (BabyBear, SymbolicAir(BabyBear, 60, E.mul_air_eval(3, True, True)), 4, 1),
@@ -257,6 +258,16 @@ def test_folder_matches_hand_written_fibonacci():
     for _ in range(20):
         args = ([ef(), ef()], [ef(), ef()], [int(v) for v in rng.integers(0, BabyBear.P, 3)], ef(), ef(), ef(), ef())
         assert air.eval_folded_constraints(e, *args) == V.FibonacciAir().eval_folded_constraints(e, *args)
+    # the Poseidon2 AIR's folder (its builder eval through SymbolicAir) against the restated verifier's, on random opened rows
+    from oracle import p3_oracle as O
+    oair = O.air_from_rng(KoalaBear.id, O.SmallRng(1))
+    p2 = VectorizedPoseidon2Air(KoalaBear, RoundConstants(np.array(oair.beg).reshape(4, 16), np.array(oair.part)[: oair.rounds_p],
+                                                          np.array(oair.end).reshape(4, 16)), None)
+    fold, fld = V.poseidon2_air(oair)["constraints"], V.Fld(KoalaBear.id)
+    ef = lambda: [int(v) for v in rng.integers(0, KoalaBear.P, 4)]
+    for _ in range(3):
+        args = ([ef() for _ in range(p2.width())], [], [], ef(), ef(), ef(), ef())
+        assert p2.eval_folded_constraints(Ext(KoalaBear), *args) == fold(fld, *args)
 
 
 def test_next_row_needs_next_columns():

@@ -21,7 +21,8 @@ from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
 from plonky3_b200.gpu import default_gpu
 from plonky3_b200.merkle_tree import MerkleTreeMmcs
 from plonky3_b200.poseidon2 import Poseidon2, default_poseidon2
-from plonky3_b200.uni_stark import RoundConstants, StarkConfig, VectorizedPoseidon2Air, prove, verify
+from plonky3_b200.poseidon2_air import RoundConstants, VectorizedPoseidon2Air, poseidon2_eval
+from plonky3_b200.uni_stark import StarkConfig, prove, verify
 from plonky3_b200.verifier import VerificationError
 from test_air_program_cpu import random_dag
 
@@ -158,7 +159,7 @@ def test_poseidon2_program_equals_hand_written_kernel(gpu, log_n):
     oair, rc = _p2_constants()
     f = KoalaBear
     hand = VectorizedPoseidon2Air(f, rc, gpu)
-    ev, width = E.poseidon2_eval(f, rc)
+    ev, width = poseidon2_eval(f, rc)
     dsl = SymbolicAir(f, width, ev, main_next_row_columns=[], gpu=gpu)
     inputs = O.random_matrix(f.id, 8 << log_n, 16, seed=log_n)
     trace = hand.generate_trace_rows(dev(inputs))
@@ -183,7 +184,7 @@ def test_poseidon2_program_proves_the_same_bytes(gpu):
     mmcs = MerkleTreeMmcs.poseidon2(p16, p24, cap_height=3, gpu=gpu)
     config = StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), mmcs, FriParameters(1, 0, 3, 30, 0, 8, mmcs)), p24, 16)
     hand = VectorizedPoseidon2Air(f, rc, gpu)
-    ev, width = E.poseidon2_eval(f, rc)
+    ev, width = poseidon2_eval(f, rc)
     dsl = SymbolicAir(f, width, ev, main_next_row_columns=[], gpu=gpu)
     trace = hand.generate_trace_rows(dev(O.random_matrix(f.id, 8 << log_n, 16, seed=3)))
     raw = prove(config, hand, trace).to_postcard()

@@ -27,7 +27,7 @@ import air_examples as E                                     # noqa: E402
 from plonky3_b200.air import SymbolicAir                     # noqa: E402
 from plonky3_b200.field import KoalaBear                     # noqa: E402
 from plonky3_b200.gpu import default_gpu                     # noqa: E402
-from plonky3_b200.uni_stark import RoundConstants, VectorizedPoseidon2Air      # noqa: E402
+from plonky3_b200.poseidon2_air import RoundConstants, VectorizedPoseidon2Air, poseidon2_eval      # noqa: E402
 
 
 def timed(fn, reps, warmup):
@@ -67,7 +67,7 @@ def poseidon2(args, f, gpu, name, rng, alpha):
     rcs = RoundConstants(f.to_monty_array(rng.integers(0, f.P, (4, 16)).astype(np.uint64)),
                          f.to_monty_array(rng.integers(0, f.P, 20).astype(np.uint64)), f.to_monty_array(rng.integers(0, f.P, (4, 16)).astype(np.uint64)))
     hand = VectorizedPoseidon2Air(f, rcs, gpu)
-    ev, width = E.poseidon2_eval(f, rcs)
+    ev, width = poseidon2_eval(f, rcs)
     dsl = SymbolicAir(f, width, ev, main_next_row_columns=[], gpu=gpu)
     inputs = torch.from_numpy(rng.integers(0, f.P, (8 << args.log_n, 16), dtype=np.uint32).view(np.int32)).cuda()
     trace = hand.generate_trace_rows(inputs)

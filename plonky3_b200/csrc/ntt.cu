@@ -29,7 +29,9 @@
 // (radix_2_dit_parallel.rs:245, fri/src/two_adic_pcs.rs:313-318).  No standalone bit-reversal or scaling pass exists.
 // With two equal passes on the cp.async kernel (2^20 rows by default) the LDE is three launches: inverse pass 1, ONE fused
 // pass (ntt_lde_mid_kernel: inverse pass 2 and every coset's forward pass 1, tile by tile through shared memory and registers)
-// and forward pass 2, so the coefficients are written and read once.  Every other LDE runs the four passes as separate launches.
+// and forward pass 2, so the coefficients are written and read once.  Forward pass 2 runs on whole-row bands in 4-CTA clusters
+// (ntt_band_pass_kernel: one bulk copy per quarter band in and out, the two cross-quarter layers over distributed shared memory)
+// where a quarter band fits its ring slot.  Every other LDE runs the four passes as separate launches.
 // The fused pass runs warp-specialised where its registers allow (all instances but the runtime-width one at r = 10): a producer
 // lane loads each tile with one tensor copy and owns the tile stores and their read-out waits (DESIGN 4.1).
 #include <algorithm>
@@ -531,6 +533,156 @@ ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
         P3_STAMP(5);
     }
     if (tma_store && threadIdx.x == 0) bulk_wait_all();
+}
+
+// ---- last pass of the two-pass coset LDE on whole-row bands, in clusters of CL CTAs ------------------------------------
+// The forward networks' second pass (layers [n - R, n)) of coset block `coset` works on bands of 2^R CONTIGUOUS rows: band T is
+// rows T*2^R .. (T+1)*2^R - 1, one contiguous run of 2^R * w words in memory.  A cluster of CL CTAs takes a band, CTA q its rows
+// [q*RQ, (q+1)*RQ), RQ = 2^R / CL (its "quarter" at CL = 4): the quarter comes in as ONE 1-D bulk copy and leaves as ONE, with no
+// row segments, partial sectors or per-thread addresses.
+//   * step X: the band's first log2(CL) layers pair rows 2^R/2 .. RQ apart, i.e. row j of every quarter: one radix-CL step over
+//     distributed shared memory, CTA q taking rows j in [q*RQ/CL, (q+1)*RQ/CL) of the CL quarters (ld/st.shared::cluster), between
+//     two cluster barriers (every peer has its quarter; every peer has its results);
+//   * steps A and B: the remaining layers pair rows inside a quarter: two register steps on the quarter in place (as steps 1 and
+//     2 of ntt_pass_fast_kernel), then the final reduction, and one thread stores the quarter;
+//   * a 2-deep ring: thread 0 loads band k+1 into the other buffer (with its 2^R - 1 twiddles) once band k's exchange is over and
+//     the store of band k-1 has read that buffer out, so the load streams in during steps A and B and the store during the next
+//     band's exchange.
+// Threads are laid along columns (item = row * w + column): every warp access to shared memory is a run of consecutive words.
+constexpr int BAND_THREADS = 512;
+constexpr size_t BAND_SLOT_BYTES = 100 * 1024;   // the largest quarter a ring slot takes (2^R/CL rows x w x 4 bytes)
+
+__device__ __forceinline__ u32 cluster_rank() { u32 r; asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned; barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ u32 cluster_map(u32 smem_addr, u32 rank) {
+    u32 r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ uint4 ld_cluster_v4(u32 addr) {
+    uint4 v;
+    asm volatile("ld.shared::cluster.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_cluster_v4(u32 addr, uint4 v) {
+    asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void bulk_store(void *gmem, const void *smem, u32 bytes) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem), "r"((u32)__cvta_generic_to_shared(smem)), "r"(bytes) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
+
+// a: l0 = log_n - R_LOG, l1 = log_n (rows of a band contiguous), dense in / out blocks of a.n_cosets cosets, w % 4 == 0, 16-byte aligned.
+template <int F, int R_LOG, int CL>
+__global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __grid_constant__ PassArgs a) {
+    constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
+    constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
+    constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
+    static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const u32 w = a.w;
+    const u32 qwords = RQ * w;                                     // one quarter
+    u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
+    uint2 *tws0 = reinterpret_cast<uint2 *>(data0 + 2 * qwords);
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(tws0 + 2 * R);
+    const u32 full_a = (u32)__cvta_generic_to_shared(full);
+    const u32 q = cluster_rank();
+    const u32 n_clusters = gridDim.x / CL;
+    const int band_log = a.log_n - R_LOG;
+    const u32 total = a.n_cosets << band_log;
+
+    auto issue = [&](u32 t, u32 buf) {   // thread 0: band t's quarter and twiddles into ring slot buf
+        const u32 coset = t >> band_log, T = t & ((1u << band_log) - 1u);
+        const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
+        uint2 *tws = tws0 + buf * R;
+        tws[1] = tw[((size_t)1 << a.l0) + T];
+        const u32 bar = full_a + 8 * buf;
+        const bool load = !P3_SKIP(a.skip_load);
+        mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
+        if (load) bulk_load(data0 + buf * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
+        load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+    };
+
+    u32 t = blockIdx.x / CL;
+    if (threadIdx.x == 0) {
+        mbar_init(full_a, 1); mbar_init(full_a + 8, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        if (t < total) issue(t, 0);
+    }
+    __syncthreads();
+    for (u32 k = 0; t < total; t += n_clusters, k++) {
+        const u32 buf = k & 1u;
+        u32 *data = data0 + buf * qwords;
+        const uint2 *tws = tws0 + buf * R;
+        mbar_wait(full_a + 8 * buf, (k >> 1) & 1u);
+        cluster_sync_all();   // every CTA of the cluster holds its quarter of band t
+        // ---- step X: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p
+        {
+            u32 peer[CL];
+#pragma unroll
+            for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(data), (u32)p);
+            // an item is 4 adjacent columns: one 16-byte access per peer keeps 4x the bytes in flight of word accesses (the exchange
+            // is bound by the latency of remote shared memory, not by its bandwidth)
+            const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (RQ / CL) * (w / 4), base = 16 * q * items;
+            for (u32 it = threadIdx.x; it < items; it += BAND_THREADS) {
+                const u32 off = base + 16 * it;
+                uint4 v[CL];
+#pragma unroll
+                for (int p = 0; p < CL; p++) v[p] = ld_cluster_v4(peer[p] + off);
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    u32 x[CL];
+#pragma unroll
+                    for (int p = 0; p < CL; p++) x[p] = (&v[p].x)[e];
+                    reg_network<F, LX>(x, tws, 1u);
+#pragma unroll
+                    for (int p = 0; p < CL; p++) (&v[p].x)[e] = x[p];
+                }
+#pragma unroll
+                for (int p = 0; p < CL; p++) st_cluster_v4(peer[p] + off, v[p]);
+            }
+        }
+        cluster_sync_all();   // every CTA has the exchanged values of its quarter; nobody touches a peer's buffer before the next band
+        if (threadIdx.x == 0 && t + n_clusters < total) {
+            bulk_wait_read();   // band k-1's store has read out the other buffer
+            issue(t + n_clusters, buf ^ 1u);
+        }
+        // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
+        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += BAND_THREADS) {
+            u32 *sp = data + it;
+            u32 x[1 << QA];
+#pragma unroll
+            for (u32 m = 0; m < (1u << QA); m++) x[m] = sp[m * (w << QB)];
+            reg_network<F, QA>(x, tws, (1u << LX) + q);
+#pragma unroll
+            for (u32 m = 0; m < (1u << QA); m++) sp[m * (w << QB)] = x[m];
+        }
+        __syncthreads();
+        // ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB
+        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += BAND_THREADS) {
+            const u32 g = it / w, c = it - g * w;
+            u32 *sp = data + (g << QB) * w + c;
+            u32 x[1 << QB];
+#pragma unroll
+            for (u32 m = 0; m < (1u << QB); m++) x[m] = sp[m * w];
+            reg_network<F, QB>(x, tws, (1u << (LX + QA)) + (q << QA) + g);
+            if (a.final_reduce) {
+#pragma unroll
+                for (u32 m = 0; m < (1u << QB); m++) x[m] = fp_reduce<F>(x[m]);
+            }
+#pragma unroll
+            for (u32 m = 0; m < (1u << QB); m++) sp[m * w] = x[m];
+        }
+        fence_proxy_async_smem();
+        __syncthreads();
+        if (threadIdx.x == 0 && !P3_SKIP(a.skip_store)) {
+            const u32 coset = t >> band_log, T = t & ((1u << band_log) - 1u);
+            bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data, qwords * 4);
+        }
+    }
+    if (threadIdx.x == 0) bulk_wait_all();
 }
 
 // ---- fused middle passes of the two-pass coset LDE (2^(2r) rows, 7 <= r <= 10) ------------------------------------
@@ -1208,6 +1360,60 @@ static int32_t launch_fast(p3gpu_ctx *ctx, const PassArgs &a) {
     }
 }
 
+// Cluster size of the band pass: clusters of 4 and of 8 CTAs (221 KB of shared memory each) both fill 120 of the H100's 132 SMs
+// and stream at the same rate (tools/band_probe, DESIGN 4.1); 4 sends less over distributed shared memory (3/4 of each quarter
+// against 7/8).
+constexpr int BAND_CL = 4;
+static bool band_pass_eligible(const PassArgs &a) {
+    const int r = a.l1 - a.l0;
+    return env_int("P3GPU_NTT_BAND", 1) != 0 && a.l1 == a.log_n && r >= 7 && r <= 10 && a.w % 4 == 0 && a.in_stride % 4 == 0 &&
+           a.out_stride % 4 == 0 && ((reinterpret_cast<uintptr_t>(a.in) | reinterpret_cast<uintptr_t>(a.out)) % 16) == 0 &&
+           (((size_t)a.w * 4) << r) / BAND_CL <= BAND_SLOT_BYTES;
+}
+template <int F, int R_LOG>
+static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
+    constexpr int CL = BAND_CL;
+    const size_t qbytes = (((size_t)a.w * 4) << R_LOG) / CL;
+    const size_t smem = 2 * (qbytes + ((size_t)1 << R_LOG) * sizeof(uint2) + 8);
+    auto kern = ntt_band_pass_kernel<F, R_LOG, CL>;
+    // per instantiation and device: the shared memory limit and the number of clusters that fit at once, for the last size asked
+    static size_t smem_set[64] = {0};
+    static int clusters[64] = {0};
+    const int dev = ctx->device & 63;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = CL; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(BAND_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = ctx->stream;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    if (smem != smem_set[dev]) {
+        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+        cfg.gridDim = dim3(CL * ctx->sm_count);
+        int n = 0;
+        P3_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+        P3_CHECK(n > 0, P3GPU_ECUDA, "ntt: no %d-CTA cluster of the band pass fits the device", CL);
+        clusters[dev] = n;
+        smem_set[dev] = smem;
+    }
+    const size_t bands = (size_t)a.n_cosets << (a.log_n - R_LOG);
+    cfg.gridDim = dim3((unsigned)(CL * std::min<size_t>(bands, (size_t)clusters[dev])));
+    P3_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
+    ctx->launches++;
+    return P3GPU_OK;
+}
+template <int F>
+static int32_t launch_band(p3gpu_ctx *ctx, PassArgs a) {
+    // profiling build only: NOLOAD / NOSTORE skip the quarter's bulk copies, NOBFLY bit 0 steps A and B, bit 1 the exchange
+    a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0);
+    a.skip_load = env_int("P3GPU_NTT_NOLOAD", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
+    switch (a.l1 - a.l0) {
+        case 7: return launch_band_r<F, 7>(ctx, a);
+        case 8: return launch_band_r<F, 8>(ctx, a);
+        case 9: return launch_band_r<F, 9>(ctx, a);
+        default: return launch_band_r<F, 10>(ctx, a);
+    }
+}
+
 // Instances of the fused kernel that have a producer-warp form: every one but the runtime-width instance at r = 10, whose 384
 // consumer threads need 168 registers against the 152 that 416 threads leave them.
 template <int R_LOG, int CT_T> constexpr bool lde_mid_producer() { return R_LOG < 10 || CT_T != 0; }
@@ -1685,8 +1891,7 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
     if (bitrev_rows && (cp_async || pipe_mode() == 0) && run_plan.n_passes == 2 && 2 * r == log_n && r >= 7 && r <= 10 && n_cosets <= 4 &&
         lde_mid_tile_width((u32)w) != 0 && ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) % 16) == 0 &&
         tensor_map_encoder() != nullptr && !env_int("P3GPU_NTT_GENERIC", 0)) {
-        // inverse pass 1 and the fused pass store whole tiles with tensor copies.  Forward pass 2 keeps its register stores: its
-        // rows are contiguous already, and the tensor copies measured 3 % slower there (DESIGN 4.1)
+        // inverse pass 1 and the fused pass store whole tiles with tensor copies
         PassArgs a;
         memset(&a, 0, sizeof a);
         a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = r; a.tma_store = 1;
@@ -1697,8 +1902,11 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
         a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;
         P3_TRY(launch_lde_mid<F>(ctx, a, tw));
         memset(&a, 0, sizeof a);
-        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n;
+        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
         a.tw = tw; a.tw_stride = h; a.in = d_out; a.in_stride = h * w; a.out = d_out; a.out_stride = h * w; a.final_reduce = 1;
+        // forward pass 2 reads and writes contiguous bands of 2^r rows: whole quarter bands as single bulk copies in 4-CTA clusters
+        // (ntt_band_pass_kernel) where a quarter fits a ring slot; P3GPU_NTT_BAND=0 keeps the tile kernel
+        if (band_pass_eligible(a)) return launch_band<F>(ctx, a);
         return launch_pass<F>(ctx, a, (unsigned)n_cosets, 4);
     }
     P3_TRY(run_network<F>(ctx, log_n, w, tw_inv, 0, 1, d_in, 0, 0, (u32 *)coef, 0, 0, 0, 0, nullptr, true, inv_height_scale<F>(h), false));

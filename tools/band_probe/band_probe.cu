@@ -1,0 +1,163 @@
+// Probe for the coset LDE's band pass (ntt_band_pass_kernel): the three numbers its design rests on, measured on the device.
+//   1. in-place streaming of the forward pass 2 buffer (2^21 x 100 u32 = 839 MB read + 839 MB written) as 100 KB 1-D bulk
+//      copies, persistent 4-CTA clusters, a 2-deep ring per CTA (the load of chunk k+1 waits until the store of chunk k-1 has
+//      left its buffer);
+//   2. the DSMEM rate of the radix-4 exchange in 4-CTA clusters: each CTA reads 3/4 of its 100 KB quarter's worth from its peers
+//      and writes 3/4 back, between two cluster barriers, 64 times (the bands a CTA takes at 2^20 x 100, blowup 2);
+//   3. cudaOccupancyMaxActiveClusters for clusters of 4 and 8 CTAs at 221 KB of dynamic shared memory, 512 threads.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 band_probe.cu -o band_probe
+#include <cuda_runtime.h>
+#include <algorithm>
+#include <cstdio>
+#include <vector>
+typedef unsigned u32;
+constexpr int THREADS = 512;
+constexpr u32 W = 100, QROWS = 256, QWORDS = QROWS * W, QBYTES = QWORDS * 4;   // one quarter band: 256 rows x 100 columns
+constexpr size_t SMEM = 2 * (QBYTES + 1024 * 8) + 64;                          // 2 x (quarter + its twiddles) + barriers
+
+#define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("%s: %s\n", #x, cudaGetErrorString(e_)); return 1; } } while (0)
+
+__device__ __forceinline__ u32 sa(const void *p) { return (u32)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_wait(u32 bar, u32 parity) {
+    asm volatile("{ .reg .pred p; WAIT_%=: mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1; @!p bra WAIT_%=; }" ::"r"(bar), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned; barrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+__global__ void __launch_bounds__(THREADS, 1) stream_kernel(u32 *buf, u32 n_chunks) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    u32 *data = reinterpret_cast<u32 *>(smem);
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(smem + SMEM - 64);
+    if (threadIdx.x != 0) return;
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sa(full)));
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sa(full + 1)));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    auto load = [&](u32 c, u32 b) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sa(full + b)), "r"(QBYTES) : "memory");
+        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                     ::"r"(sa(data + b * (QWORDS + 2048))), "l"(buf + (size_t)c * QWORDS), "r"(QBYTES), "r"(sa(full + b)) : "memory");
+    };
+    u32 c = blockIdx.x, k = 0;
+    if (c < n_chunks) load(c, 0);
+    for (; c < n_chunks; c += gridDim.x, k++) {
+        const u32 b = k & 1;
+        if (c + gridDim.x < n_chunks) {
+            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the store of chunk k-1 has left buffer b^1
+            load(c + gridDim.x, b ^ 1);
+        }
+        mbar_wait(sa(full + b), (k >> 1) & 1);
+        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                     ::"l"(buf + (size_t)c * QWORDS), "r"(sa(data + b * (QWORDS + 2048))), "r"(QBYTES) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+// rows j, j + 256, j + 512, j + 768 of a band are row j of the cluster's four quarters; CTA q takes rows [64q, 64q + 64)
+__global__ void __launch_bounds__(THREADS, 1) dsmem_kernel(u32 iters, u32 *sink) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    u32 *data = reinterpret_cast<u32 *>(smem);
+    for (u32 i = threadIdx.x; i < QWORDS; i += THREADS) data[i] = i;
+    u32 q;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(q));
+    u32 peer[4];
+    for (u32 p = 0; p < 4; p++) asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[p]) : "r"(sa(data)), "r"(p));
+    u32 acc = 0;
+    cluster_sync();
+    for (u32 it = 0; it < iters; it++) {
+        for (u32 i = threadIdx.x; i < (QROWS / 4) * W; i += THREADS) {
+            const u32 off = (q * (QROWS / 4) * W + i) * 4;
+            u32 x[4];
+#pragma unroll
+            for (int p = 0; p < 4; p++) asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(x[p]) : "r"(peer[p] + off) : "memory");
+            const u32 t0 = x[0] + x[2], t1 = x[1] + x[3], t2 = x[0] ^ x[2], t3 = x[1] ^ x[3];
+            x[0] = t0 + t1; x[1] = t0 ^ t1; x[2] = t2 + t3; x[3] = t2 ^ t3;
+#pragma unroll
+            for (int p = 0; p < 4; p++) asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(peer[p] + off), "r"(x[p]) : "memory");
+        }
+        cluster_sync();
+        acc += data[(threadIdx.x * 37u + it) % QWORDS];
+        cluster_sync();
+    }
+    if (acc == 0x9e3779b9u) sink[0] = acc;
+}
+
+template <typename K, typename... A>
+static cudaError_t launch_cluster(K kern, u32 grid, u32 cl, A... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(THREADS); cfg.dynamicSmemBytes = SMEM;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cl; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kern, args...);
+}
+
+static int active_clusters(const void *kern, u32 cl, int *out) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cl * 64); cfg.blockDim = dim3(THREADS); cfg.dynamicSmemBytes = SMEM;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cl; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    CK(cudaOccupancyMaxActiveClusters(out, kern, &cfg));
+    return 0;
+}
+
+int main() {
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, 0));
+    printf("device: %s, %d SMs, smem/block optin %zu\n", prop.name, prop.multiProcessorCount, prop.sharedMemPerBlockOptin);
+    CK(cudaFuncSetAttribute(stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+    CK(cudaFuncSetAttribute(dsmem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+    // 3. occupancy
+    int nc4 = 0, nc8 = 0;
+    if (active_clusters((const void *)stream_kernel, 4, &nc4) || active_clusters((const void *)stream_kernel, 8, &nc8)) return 1;
+    printf("dynamic smem %zu B, %d threads: max active clusters: size 4 -> %d (%d SMs), size 8 -> %d (%d SMs)\n", SMEM, THREADS, nc4, 4 * nc4,
+           nc8, 8 * nc8);
+    if (nc4 == 0) return 1;
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    // 1. streaming
+    const u32 n_chunks = (2u << 20) / QROWS;   // 2^21 rows of 100 columns = 8192 quarter bands
+    const size_t bytes = (size_t)n_chunks * QBYTES;
+    u32 *buf;
+    CK(cudaMalloc(&buf, bytes));
+    CK(cudaMemset(buf, 1, bytes));
+    for (u32 cl : {4u, 8u}) {
+        const u32 grid = cl * (cl == 4 ? nc4 : nc8);
+        if (grid == 0) continue;
+        std::vector<float> ts;
+        for (int rep = 0; rep < 12; rep++) {
+            CK(cudaEventRecord(e0));
+            CK(launch_cluster(stream_kernel, grid, cl, buf, n_chunks));
+            CK(cudaEventRecord(e1));
+            CK(cudaEventSynchronize(e1));
+            float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+            if (rep >= 2) ts.push_back(ms);
+        }
+        std::sort(ts.begin(), ts.end());
+        printf("stream in place, cluster %u, %u CTAs: %zu MB read + written: median %.3f ms (min %.3f, max %.3f) = %.0f GB/s\n", cl, grid,
+               bytes >> 20, ts[ts.size() / 2], ts[0], ts.back(), 2.0 * bytes / (ts[ts.size() / 2] * 1e-3) / 1e9);
+    }
+    // 2. DSMEM exchange
+    u32 *sink;
+    CK(cudaMalloc(&sink, 4));
+    const u32 iters = 64, grid = 4 * nc4;
+    std::vector<float> ts;
+    for (int rep = 0; rep < 12; rep++) {
+        CK(cudaEventRecord(e0));
+        CK(launch_cluster(dsmem_kernel, grid, 4, iters, sink));
+        CK(cudaEventRecord(e1));
+        CK(cudaEventSynchronize(e1));
+        float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+        if (rep >= 2) ts.push_back(ms);
+    }
+    std::sort(ts.begin(), ts.end());
+    const double remote = 2.0 * 0.75 * QBYTES * iters * grid;   // bytes crossing between SMs (reads + writes)
+    printf("dsmem radix-4 exchange, %u CTAs x %u bands: median %.3f ms (min %.3f, max %.3f) = %.1f us per band, %.0f GB/s between SMs\n", grid,
+           iters, ts[ts.size() / 2], ts[0], ts.back(), ts[ts.size() / 2] * 1e3 / iters, remote / (ts[ts.size() / 2] * 1e-3) / 1e9);
+    CK(cudaFree(buf)); CK(cudaFree(sink));
+    return 0;
+}

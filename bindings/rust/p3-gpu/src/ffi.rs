@@ -41,6 +41,7 @@ pub const P3GPU_AIR_PREPROCESSED_LOCAL: u32 = 16;
 pub const P3GPU_AIR_PREPROCESSED_NEXT: u32 = 17;
 pub const P3GPU_AIR_PERIODIC: u32 = 18;
 pub const P3GPU_KECCAK_AIR_COLS: usize = 2633;
+pub const P3GPU_BLAKE3_AIR_COLS: usize = 9168;
 
 /// `p3gpu_air_layout`: what a constraint program's leaves may read.
 #[repr(C)]
@@ -174,6 +175,11 @@ unsafe extern "C" {
     // Keccak-f AIR (keccak-air): trace generation and quotient values, P3GPU_KECCAK_AIR_COLS columns
     pub fn p3gpu_keccak_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u64, n_hashes: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_keccak_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
+                                         alpha: *const u32, d_quotient: *mut u32) -> i32;
+
+    // Blake3 AIR (blake3-air): trace generation and quotient values, P3GPU_BLAKE3_AIR_COLS columns
+    pub fn p3gpu_blake3_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, d_trace: *mut u32) -> i32;
+    pub fn p3gpu_blake3_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
                                          alpha: *const u32, d_quotient: *mut u32) -> i32;
 
     // any AIR as a constraint program (symbolic expression DAG -> register program -> quotient kernel)

@@ -243,6 +243,20 @@ int32_t p3gpu_keccak_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uin
 int32_t p3gpu_keccak_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
                                       const uint32_t alpha[4], uint32_t *d_quotient);
 
+/* ---- Blake3 AIR: the AIR of prove_prime_field_31 -o blake-3-permutations (blake3-air/src), BabyBear and KoalaBear ----------
+ * One BLAKE3 compression per row, rows independent (no next-row reads, no selectors), P3GPU_BLAKE3_AIR_COLS columns (columns.rs
+ * Blake3Cols); 9632 constraints of degree 3, so two quotient chunks (log_blowup >= 1). */
+#define P3GPU_BLAKE3_AIR_COLS 9168
+/* generate_trace_rows (blake3-air/src/generation.rs:16-118): d_inputs n_hashes x 24 u32 (16 message words, then 8 chaining-value
+ * words) -> d_trace, n_hashes x P3GPU_BLAKE3_AIR_COLS Montgomery words; row i is compressed with counter i, block_len n_hashes and
+ * flags 0.  P3GPU_EINVAL before any launch: a NULL or non-4-byte-aligned pointer, n_hashes 0, not a power of two or above 2^32;
+ * P3GPU_EUNSUPPORTED: a field other than BabyBear / KoalaBear. */
+int32_t p3gpu_blake3_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, uint32_t *d_trace);
+/* quotient_values of the Blake3 AIR, with the contract of p3gpu_keccak_air_quotient_dev (d_lde: 2^log_lde_height rows x
+ * P3GPU_BLAKE3_AIR_COLS). */
+int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient);
+
 /* ---- any AIR as a constraint program (DESIGN.md section 4.7) ----------------------------------------------------------------
  * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
  * (operands refer only to earlier nodes) plus the list of constrained nodes in assertion order.  The library compiles it once

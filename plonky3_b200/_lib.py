@@ -15,6 +15,7 @@ EOK, EINVAL, EUNSUPPORTED, ECUDA, ENOMEM, ESTATE = 0, -1, -2, -3, -4, -5
 DFT, IDFT, COSET_DFT, COSET_IDFT = 0, 1, 2, 3
 HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_KECCAK = 0, 1, 2
 KECCAK_AIR_COLS = 2633                       # P3GPU_KECCAK_AIR_COLS
+BLAKE3_AIR_COLS = 9168                       # P3GPU_BLAKE3_AIR_COLS
 
 EXPORTS = [
     "p3gpu_ctx_create", "p3gpu_ctx_destroy", "p3gpu_ctx_set_stream", "p3gpu_ctx_use_own_stream", "p3gpu_ctx_sync", "p3gpu_last_error",
@@ -35,6 +36,7 @@ EXPORTS = [
     "p3gpu_air_program_create_layout", "p3gpu_air_quotient_layout_dev",
     "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
     "p3gpu_keccak_air_generate_trace_dev", "p3gpu_keccak_air_quotient_dev",
+    "p3gpu_blake3_air_generate_trace_dev", "p3gpu_blake3_air_quotient_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -138,6 +140,8 @@ def load():
         "p3gpu_challenger_sample_bits": (i32, [vp, vp, cu, sz, vp]),
         "p3gpu_keccak_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
         "p3gpu_keccak_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
+        "p3gpu_blake3_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
+        "p3gpu_blake3_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

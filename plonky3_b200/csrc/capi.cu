@@ -512,6 +512,21 @@ int32_t p3gpu_keccak_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t 
     return keccak_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
 }
 
+// ---- Blake3 AIR: trace generation + quotient (blake3_air.cu) ------------------------------------------
+int32_t p3gpu_blake3_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, uint32_t *d_trace) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && d_trace, P3GPU_EINVAL, "null argument");
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 4 == 0 && reinterpret_cast<uintptr_t>(d_trace) % 4 == 0, P3GPU_EINVAL,
+             "Blake3 AIR trace: misaligned buffer");
+    return blake3_air_generate(ctx, field, d_inputs, n_hashes, d_trace);
+}
+int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return blake3_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+
 // ---- any AIR as a constraint program (air_program.cu) -------------------------------------------------
 int32_t p3gpu_air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
                                  size_t n_constraints, uint32_t width, uint32_t n_public, p3gpu_air_program **out) {

@@ -169,6 +169,10 @@ size_t keccak_air_height(size_t n_hashes);
 int32_t keccak_air_generate(p3gpu_ctx *ctx, int field, const u64 *d_inputs, size_t n_hashes, u32 *d_trace);
 int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
 
+// blake3_air.cu: Blake3 AIR trace generation / quotient
+int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
+int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);
 void challenger_free(p3gpu_ctx *ctx, p3gpu_challenger *ch);

@@ -323,6 +323,30 @@ class Gpu:
         check(self.L.p3gpu_keccak_air_quotient_dev(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    # ------------------------------------------------------------------ Blake3 AIR
+    def blake3_air_generate_trace(self, field, inputs_dev):
+        """(n, 24) contiguous CUDA int32 tensor of u32 words (16 message words, 8 chaining-value words), n a power of two -> the
+        (n, 9168) trace."""
+        import torch
+        assert inputs_dev.is_cuda and inputs_dev.dtype == torch.int32 and inputs_dev.is_contiguous(), "inputs: contiguous CUDA int32 (n, 24)"
+        assert inputs_dev.dim() == 2 and int(inputs_dev.shape[1]) == 24
+        self._use_torch_stream()
+        n = int(inputs_dev.shape[0])
+        out = self._empty((n, _lib.BLAKE3_AIR_COLS))
+        check(self.L.p3gpu_blake3_air_generate_trace_dev(self.h, field, inputs_dev.data_ptr(), n, out.data_ptr()))
+        return out
+
+    def blake3_air_quotient(self, field, lde_dev, log_trace_height, alpha):
+        """Quotient values (2^(log_trace_height + 1), 4) in natural order over GENERATOR * K from the first 2^(log_trace_height + 1)
+        rows of the committed bit-reversed LDE."""
+        m = self._dev(lde_dev); self._use_torch_stream()
+        H = int(m.shape[0]); log_h = H.bit_length() - 1
+        if H != 1 << log_h or int(m.shape[1]) != _lib.BLAKE3_AIR_COLS:
+            raise _lib.P3GpuError(f"LDE of shape {tuple(m.shape)}: need 2^k rows x {_lib.BLAKE3_AIR_COLS}", _lib.EINVAL)
+        q = self._empty((2 << log_trace_height, 4))
+        check(self.L.p3gpu_blake3_air_quotient_dev(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
+
     # ------------------------------------------------------------------ any AIR as a constraint program
     def air_program_create(self, field, nodes, constraints, width, n_public):
         """Compile an expression DAG: nodes (n, 4) uint32 rows (op, a, b, imm), constraints: node indices in assertion order.

@@ -142,8 +142,8 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
 
 def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
     """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
-    call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air or
-    keccak_air.KeccakAir.  `trace`: device (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
+    call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air,
+    keccak_air.KeccakAir or blake3_air.Blake3Air.  `trace`: device (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
 
     `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
     after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is

@@ -1,0 +1,114 @@
+"""Blake3 AIR `prove` of `prove_prime_field_31 -o blake-3-permutations` at 2^18 compressions (a 2^18 x 9168 trace; the reference's
+`-l 20` shape, a 38.5 GB trace with a 77 GB LDE, does not fit on one 80 GB card), new_benchmark_high_arity's FRI parameters, cap
+height 3.  One configuration per process (the trace and its LDE take 29 GB together):
+
+    python tools/blake3_air_prove.py --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
+
+Times trace generation and the quotient kernel alone (CUDA events, median of --kernel-reps launches after a warm-up), and `prove`
+span by span (median of --reps proofs after one warm-up); then verifies the last proof.  Prints one JSON object with the card's name
+and power limit, and the quotient kernel's LDE bytes per second next to the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), named
+as such."""
+import argparse
+import json
+import pathlib
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = pathlib.Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT))
+
+import numpy as np
+import torch
+
+from plonky3_b200.dft import Radix2DitParallel
+from plonky3_b200.field import BabyBear, KoalaBear
+from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
+from plonky3_b200.gpu import default_gpu
+from plonky3_b200.blake3_air import WIDTH, Blake3Air, random_inputs
+from plonky3_b200.merkle_tree import MerkleTreeMmcs
+from plonky3_b200.poseidon2 import default_poseidon2
+from plonky3_b200.uni_stark import KeccakStarkConfig, StarkConfig, prove, verify
+
+DATASHEET_HBM_BYTES_PER_S = 3.35e12          # NVIDIA H100 SXM data sheet, HBM3
+
+
+def _card():
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    return q.stdout.strip() if q.returncode == 0 else torch.cuda.get_device_name(0)
+
+
+def _events_median(fn, reps):
+    fn()
+    times = []
+    for _ in range(reps):
+        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        s.record(); fn(); e.record(); e.synchronize()
+        times.append(s.elapsed_time(e))
+    return statistics.median(times)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--field", choices=["koala-bear", "baby-bear"], default="koala-bear")
+    ap.add_argument("--config", choices=["keccak", "poseidon2"], default="keccak")
+    ap.add_argument("--log-rows", type=int, default=18)
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--kernel-reps", type=int, default=10)
+    a = ap.parse_args()
+    f = KoalaBear if a.field == "koala-bear" else BabyBear
+    gpu = default_gpu(0)
+    if a.config == "keccak":
+        m = MerkleTreeMmcs.keccak(f, cap_height=3, gpu=gpu)
+        config = KeccakStarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, FriParameters.new_benchmark_high_arity(m)))
+    else:
+        p16, p24 = default_poseidon2(f, 16), default_poseidon2(f, 24)
+        m = MerkleTreeMmcs.poseidon2(p16, p24, cap_height=3, gpu=gpu)
+        config = StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, FriParameters.new_benchmark_high_arity(m)), p24, 16)
+    air = Blake3Air(f, gpu)
+    n = 1 << a.log_rows                                          # one compression per row
+    inputs = torch.from_numpy(random_inputs(n).view(np.int32)).cuda()
+    trace = air.generate_trace_rows(inputs)
+    assert tuple(trace.shape) == (1 << a.log_rows, WIDTH)
+    gen_ms = _events_median(lambda: air.generate_trace_rows(inputs), a.kernel_reps)
+    trace_bytes = trace.numel() * 4
+
+    # the quotient kernel alone, on the committed LDE's quotient-domain prefix (2^(log_rows + 1) rows)
+    lde = gpu.coset_lde_batch(f.id, trace, 1, f.generator, bitrev_rows=True)
+    alpha = np.array([f.to_monty(v) for v in (3, 5, 7, 11)], dtype=np.uint32)
+    q_ms = _events_median(lambda: air.quotient_values(lde, a.log_rows, alpha), a.kernel_reps)
+    lde_bytes = lde.numel() * 4
+    del lde
+    torch.cuda.empty_cache()
+
+    prove(config, air, trace)                                    # warm-up: twiddles, constants, allocator
+    spans, totals = {}, []
+    for _ in range(a.reps):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        proof = prove(config, air, trace)
+        torch.cuda.synchronize()
+        totals.append((time.perf_counter() - t0) * 1e3)
+        for s, v in proof.timings_ms.items():
+            spans.setdefault(s, []).append(v)
+    raw = proof.to_postcard()
+    del trace
+    torch.cuda.empty_cache()
+    t0 = time.perf_counter()
+    verify(config, Blake3Air(f), raw)
+    verify_ms = (time.perf_counter() - t0) * 1e3
+    print(json.dumps({
+        "card_and_power_limit": _card(), "field": a.field, "config": a.config, "hashes": n, "trace_rows": 1 << a.log_rows, "width": WIDTH,
+        "trace_generation_ms": round(gen_ms, 3), "trace_bytes_written": trace_bytes,
+        "trace_generation_bytes_per_s": float("%.3g" % (trace_bytes / gen_ms * 1e3)),
+        "quotient_kernel_ms": round(q_ms, 3), "quotient_lde_bytes_read": lde_bytes,
+        "quotient_bytes_per_s": float("%.3g" % (lde_bytes / q_ms * 1e3)),
+        "datasheet_hbm_bytes_per_s": DATASHEET_HBM_BYTES_PER_S,
+        "prove_ms": round(statistics.median(totals), 1), "prove_spans_ms": {s: round(statistics.median(v), 2) for s, v in spans.items()},
+        "peak_allocated_bytes": torch.cuda.max_memory_allocated(),
+        "proof_bytes": len(raw), "verify_ms": round(verify_ms, 1), "verified": True}))
+
+
+if __name__ == "__main__":
+    main()

@@ -278,6 +278,12 @@ class SymbolicAir:
         if self.gpu is None:
             raise _lib.P3GpuError(f"{what} needs a GPU context (no CPU fallback)")
 
+    def _to_device(self, t):
+        """Host tensor `t` on the context's CUDA device (unchanged for a stand-in device without an integer `device`)."""
+        if isinstance(getattr(self.gpu, "device", None), int):
+            return t.to(f"cuda:{self.gpu.device}")
+        return t
+
     def program(self):
         self._need_gpu("quotient evaluation")
         if self._program is None:
@@ -305,9 +311,7 @@ class SymbolicAir:
             p_max = max(len(c) for c in self._periodic)
             q = log_quotient_size - log_degree
             padded = np.array([[c[i % len(c)] for c in self._periodic] for i in range(p_max)], dtype=np.uint64)
-            m = torch.from_numpy(f.to_monty_array(padded).astype(np.uint32).view(np.int32))
-            if isinstance(getattr(self.gpu, "device", None), int):
-                m = m.to(f"cuda:{self.gpu.device}")
+            m = self._to_device(torch.from_numpy(f.to_monty_array(padded).astype(np.uint32).view(np.int32)))
             shift = f.pow(f.generator, n // p_max)                     # GENERATOR^(|K| / (p_max 2^q)), |K| = n 2^q
             self._periodic_tables[key] = self.gpu.coset_lde_batch(f.id, m, q, shift, bitrev_rows=False)
         return self._periodic_tables[key]
@@ -372,3 +376,23 @@ class SymbolicAir:
         for c in self.builder.constraints:
             acc = e.add(e.mul(acc, alpha), vals[c])
         return acc
+
+
+class KernelAir(SymbolicAir):
+    """A SymbolicAir whose prover runs the AIR's own hand-written kernels instead of a constraint program: no public values, no
+    preprocessed columns, no CPU fallback.  A subclass names the AIR in `air_name` and launches its quotient kernel in
+    `_kernel_quotient`."""
+    air_name = ""
+
+    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
+        """uni-stark/src/prover.rs:462-827 on the AIR's hand-written kernel: `trace_lde_dev` holds the trace on the quotient domain in
+        bit-reversed row order (the committed LDE or its prefix, as `_kernel_quotient` says).  Returns (|K|, 4) in natural order."""
+        if len(public_values) != 0:
+            raise ValueError(f"{len(public_values)} public values given, the {self.air_name} AIR has none")
+        if preprocessed_on_quotient_domain is not None:
+            raise ValueError(f"the {self.air_name} AIR has no preprocessed columns")
+        self._need_gpu("quotient evaluation")
+        return self._kernel_quotient(trace_lde_dev, log_degree, alpha)
+
+    def _kernel_quotient(self, trace_lde_dev, log_degree: int, alpha):
+        raise NotImplementedError

@@ -15,6 +15,7 @@
 // 656 contiguous bytes), constraints folded with lazy 64-bit multiply-accumulates against an alpha-power table in shared memory,
 // 3-step shuffle reduction across the row's lanes.
 #include "common.h"
+#include "air_program.cuh"
 #include "hash_core.cuh"
 
 namespace p3 {
@@ -115,19 +116,6 @@ __global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, 
 }
 
 // ---- quotient ----------------------------------------------------------------------------------------------------------
-template <int F> __device__ __forceinline__ void qmac(u64 (&acc)[4], u32 c, const uint4 a) {
-    // acc += c * a (base x EF4), lazily: invariant acc < p * 2^32 (open.cu lazy_mac)
-    const u32 av[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-    for (int d = 0; d < 4; d++) {
-        acc[d] += (u64)c * av[d];
-        u32 hi = (u32)(acc[d] >> 32);
-        const u32 hs = hi - Fp<F>::P;
-        hi = hi < hs ? hi : hs;
-        acc[d] = ((u64)hi << 32) | (u32)acc[d];
-    }
-}
-
 // One column segment of a sharded row block: columns [c0, c1) of the trace are a (rows x (c1 - c0)) row-major matrix at element
 // offset `off` of the block.  c0 and c1 are multiples of 4, so a 16-byte load never straddles two segments.
 struct QSeg { u32 c0, c1; u64 off; };
@@ -220,7 +208,7 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
             u32 post[AIR_W];
             ld16(post);
 #pragma unroll
-            for (int x = 0; x < AIR_W; x++) { qmac<F>(acc, fp_sub<F>(s[x], post[x]), apv[x]); s[x] = post[x]; }
+            for (int x = 0; x < AIR_W; x++) { air_qmac<F>(acc, fp_sub<F>(s[x], post[x]), apv[x]); s[x] = post[x]; }
             apv += 16;
         }
         {
@@ -234,7 +222,7 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
 #pragma unroll
                 for (int t2 = 0; t2 < 4; t2++) {
                     const u32 x3 = sbox<F>(fp_add<F>(s[0], k.part[r + t2]));
-                    qmac<F>(acc, fp_sub<F>(x3, pv[t2]), *apv++);
+                    air_qmac<F>(acc, fp_sub<F>(x3, pv[t2]), *apv++);
                     s[0] = pv[t2];
                     air_internal_layer<F>(s);
                 }
@@ -249,7 +237,7 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
             u32 post[AIR_W];
             ld16(post);
 #pragma unroll
-            for (int x = 0; x < AIR_W; x++) { qmac<F>(acc, fp_sub<F>(s[x], post[x]), apv[x]); s[x] = post[x]; }
+            for (int x = 0; x < AIR_W; x++) { air_qmac<F>(acc, fp_sub<F>(s[x], post[x]), apv[x]); s[x] = post[x]; }
             apv += 16;
         }
     }
@@ -381,12 +369,9 @@ static int32_t quotient_launch(p3gpu_ctx *ctx, int field, int vec_len, const u32
     QSeg *dsegs = reinterpret_cast<QSeg *>(invz + 256);         // SHARDED: behind the largest 1/Z_H table, 16-byte aligned
     Ef4<F> al; for (int d = 0; d < 4; d++) al.c[d] = alpha[d];
     ef_powers_kernel<F><<<(unsigned)(((n_all + 31) / 32 + 63) / 64), 64, 0, ctx->stream>>>(apow, (size_t)n_all, al);
-    // 1 / Z_H on the coset GENERATOR * K (domain.rs:326-360): Z_H(x_i) = g^N * w^(i mod 2^rate_bits) - 1, w of order 2^rate_bits
-    u32 hz[256];
-    const u32 s_pow_n = fp_pow<F>(to_monty<F>(Fp<F>::GEN), (u64)1 << log_n), wr = two_adic_generator<F>(rate_bits);
-    u32 wp = Fp<F>::ONE;
-    for (size_t j = 0; j < nz; j++) { hz[j] = fp_inv<F>(fp_sub<F>(mont_mul<F>(s_pow_n, wp), Fp<F>::ONE)); wp = mont_mul<F>(wp, wr); }
-    P3_CUDA(cudaMemcpyAsync(invz, hz, nz * 4, cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<u32> zh, izh;                                       // Z_H and 1 / Z_H on the coset GENERATOR * K, by i mod 2^rate_bits
+    air_domain<F>(log_h, log_n, 0, zh, izh);
+    P3_CUDA(cudaMemcpyAsync(invz, izh.data(), nz * 4, cudaMemcpyHostToDevice, ctx->stream));
     QuotArgs qa;
     qa.lde = d_lde; qa.q = d_q; qa.apow = apow; qa.invz = invz; qa.log_h = log_h; qa.rate_mask = (unsigned)(nz - 1); qa.vec_len = vec_len;
     qa.segs = nullptr; qa.n_segs = 0; qa.row0 = row0; qa.rows = rows;

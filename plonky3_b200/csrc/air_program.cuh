@@ -179,7 +179,7 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
 
 // ---- per-instruction semantics and per-row quotient, shared by the kernel and host C++ -------------------------------------
 template <int F> __host__ __device__ __forceinline__ void air_qmac(u64 (&acc)[4], u32 c, const uint4 a) {
-    // acc += c * a (base x EF4), lazily: invariant acc < p * 2^32 (open.cu lazy_mac, air.cu qmac)
+    // acc += c * a (base x EF4), lazily: invariant acc < p * 2^32 (open.cu lazy_mac)
     const u32 av[4] = {a.x, a.y, a.z, a.w};
 #pragma unroll
     for (int d = 0; d < 4; d++) {
@@ -212,6 +212,16 @@ struct AirDomain {
     u32 periodic_mask;          // rows of the periodic table - 1 (natural index i reads row i & periodic_mask)
 };
 
+// Arguments of a hand-written AIR quotient kernel (keccak_air.cu, blake3_air.cu), launched by air_hand_quotient (air_program.cu):
+// 2N points of GENERATOR * K, |K| = 2N, read from the first 2N rows of the committed bit-reversed LDE.
+struct AirHandQArgs {
+    const u32 *lde;            // bit-reversed LDE prefix, >= 2^d.log_q rows x the AIR's width
+    const uint4 *apow;         // alpha^(K - 1 - k), k < K
+    u32 *q;                    // 2^d.log_q x 4, natural order
+    AirDomain d;
+    u32 zh[2], izh[2];         // Z_H and 1 / Z_H by i mod 2
+};
+
 // selectors_on_coset (commit/src/domain.rs:321-361) at x_i = g * w_q^i, unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1.
 // zh = Z_H(x_i).  Shared by the constraint-program kernel and the hand-written Keccak AIR kernel (keccak_air.cu).
 template <int F> __host__ __device__ __forceinline__ void air_selectors(const AirDomain &d, u32 i, u32 zh, u32 &first, u32 &last, u32 &trans) {
@@ -222,6 +232,26 @@ template <int F> __host__ __device__ __forceinline__ void air_selectors(const Ai
     last = mont_mul<F>(zh, mont_mul<F>(a, inv_ab));
     trans = b;
 }
+
+#ifdef __CUDACC__
+// ---- device helpers of the hand-written quotient kernels ------------------------------------------------------------------
+template <int F> __device__ __forceinline__ u32 air_bxor(u32 x, u32 y) { return fp_sub<F>(fp_add<F>(x, y), fp_double<F>(mont_mul<F>(x, y))); }   // x + y - 2xy
+template <int F> __device__ __forceinline__ u32 air_bool(u32 x) { return mont_mul<F>(x, fp_sub<F>(x, Fp<F>::ONE)); }                         // x (x - 1)
+
+// The end of a warp's point i: reduce every lane's lazy accumulators, add them over the 32 lanes, multiply by 1 / Z_H(x_i) and let
+// lanes 0..3 store the four coefficients of q[i].
+template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQArgs &a, const u64 (&acc)[4], u32 i, unsigned lane) {
+    u32 r[4];
+#pragma unroll
+    for (int d = 0; d < 4; d++) r[d] = mont_redc<F>(acc[d]);
+#pragma unroll
+    for (int o = 16; o; o >>= 1)
+#pragma unroll
+        for (int d = 0; d < 4; d++) r[d] = fp_add<F>(r[d], __shfl_xor_sync(0xffffffffu, r[d], o));
+    const u32 mine = lane == 0 ? r[0] : lane == 1 ? r[1] : lane == 2 ? r[2] : r[3];
+    if (lane < 4) a.q[4 * (size_t)i + lane] = mont_mul<F>(mine, (i & 1u) ? a.izh[1] : a.izh[0]);
+}
+#endif
 
 // Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),
 // the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).  EXT (a program that reads

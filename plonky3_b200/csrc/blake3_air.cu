@@ -132,33 +132,22 @@ __global__ void __launch_bounds__(32 * B3_GEN_WARPS) blake3_air_generate_kernel(
 constexpr int BQ_WARPS = 16;
 constexpr size_t BQ_SMEM = (size_t)B3_CONSTRAINTS * 16;
 
-struct B3QArgs {
-    const u32 *lde;            // bit-reversed LDE prefix, >= 2^log_q rows x 9168
-    const uint4 *apow;         // alpha^(9631 - k), k < 9632
-    u32 *q;                    // 2^log_q x 4, natural order
-    unsigned log_q;
-    u32 izh[2];                // 1 / Z_H by i mod 2
-};
-
 // a Blake3State's four column bases: row0[j] limbs at r0 + 2j, row1[j] bits at r1 + 32j, row2[j] at r2 + 2j, row3[j] at r3 + 32j
 struct B3View { int r0, r1, r2, r3; };
 __device__ __forceinline__ B3View b3_state(int base) { return {base, base + B3_S_ROW1, base + B3_S_ROW2, base + B3_S_ROW3}; }
 
-template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_quotient_kernel(const B3QArgs a) {
+template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_quotient_kernel(const AirHandQArgs a) {
     extern __shared__ uint4 bq_sm[];
     const uint4 *ap = bq_sm;
     for (int t = threadIdx.x; t < B3_CONSTRAINTS; t += blockDim.x) bq_sm[t] = __ldg(a.apow + t);
     __syncthreads();
     const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const u32 n_pts = 1u << a.log_q;
-    const u32 ONE = Fp<F>::ONE;
+    const u32 n_pts = 1u << a.d.log_q;
     const u32 T16 = to_monty<F>(1u << 16), T17 = fp_double<F>(T16), T32 = mont_mul<F>(T16, T16), T33 = fp_double<F>(T32);
     const u32 wpow = to_monty<F>(1u << (lane & 15u));                  // weight of this lane's bit in its 16-bit limb
     auto add = [](u32 x, u32 y) { return fp_add<F>(x, y); };
     auto sub = [](u32 x, u32 y) { return fp_sub<F>(x, y); };
     auto mul = [](u32 x, u32 y) { return mont_mul<F>(x, y); };
-    auto bxor = [](u32 x, u32 y) { return fp_sub<F>(fp_add<F>(x, y), fp_double<F>(mont_mul<F>(x, y))); };   // x + y - 2xy
-    auto bchk = [ONE](u32 x) { return mont_mul<F>(x, fp_sub<F>(x, ONE)); };                                 // x (x - 1)
     // pack_bits_le of the lane-distributed bits v over [0, 16) and [16, 32): (lo, hi), warp-uniform
     auto pack = [&](u32 v, u32 &lo, u32 &hi) {
         u32 s = mul(v, wpow);
@@ -167,12 +156,12 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
         lo = __shfl_sync(0xffffffffu, s, 0); hi = __shfl_sync(0xffffffffu, s, 16);
     };
     for (u32 i = blockIdx.x * BQ_WARPS + warp; i < n_pts; i += gridDim.x * BQ_WARPS) {
-        const u32 *row = a.lde + (size_t)air_bitrev(i, a.log_q) * B3_COLS;
+        const u32 *row = a.lde + (size_t)air_bitrev(i, a.d.log_q) * B3_COLS;
         auto ld = [row](int c) { return __ldg(row + c); };
         u64 acc[4] = {0, 0, 0, 0};
         auto fold = [&](int k, u32 c) { air_qmac<F>(acc, c, ap[k]); };
         // the initialisation inputs are boolean (k 0..895: column k)
-        for (int c = lane; c < B3_ROW0; c += 32) fold(c, bchk(ld(c)));
+        for (int c = lane; c < B3_ROW0; c += 32) fold(c, air_bool<F>(ld(c)));
         // initial row0 = packed chaining_values[0] (k 896..903), initial row2 = IV (k 904..911)
         {
             u32 mine = 0;
@@ -224,7 +213,7 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
                 const u32 bp = ld(s1.r1 + 32 * j1 + lane), dp = ld(s1.r3 + 32 * j3 + lane);
                 const u32 bo = ld(s2.r1 + 32 * j1 + lane), dout = ld(s2.r3 + 32 * j3 + lane);
                 // booleans of d', b', d'', b'' (the c argument of each xor_32_shift)
-                fold(k + 2 + lane, bchk(dp)); fold(k + 38 + lane, bchk(bp)); fold(k + 74 + lane, bchk(dout)); fold(k + 110 + lane, bchk(bo));
+                fold(k + 2 + lane, air_bool<F>(dp)); fold(k + 38 + lane, air_bool<F>(bp)); fold(k + 74 + lane, air_bool<F>(dout)); fold(k + 110 + lane, air_bool<F>(bo));
                 u32 lo, hi, mine = 0;
                 // add3(a', a, pack(b), m0): acc (acc + 2^32) (acc + 2 2^32), acc16 (acc16 + 2^16) (acc16 + 2 2^16)
                 auto add3 = [&](u32 x0, u32 x1, u32 y0, u32 y1, u32 l, u32 h, u32 z0, u32 z1, int j) {
@@ -241,7 +230,7 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
                 };
                 // xor_32_shift(x, bb, cc, s): x[0] - pack(lo), x[1] - pack(hi) of xor(bb[l], cc[(l - s) mod 32])
                 auto xsh = [&](u32 x0, u32 x1, u32 bb, u32 cc, int s, int j) {
-                    pack(bxor(bb, __shfl_sync(0xffffffffu, cc, (lane - s) & 31u)), lo, hi);
+                    pack(air_bxor<F>(bb, __shfl_sync(0xffffffffu, cc, (lane - s) & 31u)), lo, hi);
                     if (lane == (unsigned)j) mine = sub(x0, lo);
                     if (lane == (unsigned)j + 1) mine = sub(x1, hi);
                 };
@@ -275,29 +264,21 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
                 if (lane == 2 * j) mine = sub(lo, ld(so.r2 + 2 * j));
                 if (lane == 2 * j + 1) mine = sub(hi, ld(so.r2 + 2 * j + 1));
                 // outputs[0] booleans (k + 8 .. 135)
-                fold(k + 8 + 32 * j + lane, bchk(o0));
+                fold(k + 8 + 32 * j + lane, air_bool<F>(o0));
                 // xor_32_shift(row0[j], outputs[0][j], helpers[j], 0): 32 booleans of helpers[j], then two packs (k + 136 + 34 j ..)
-                fold(k + 136 + 34 * j + lane, bchk(h));
-                pack(bxor(o0, h), lo, hi);
+                fold(k + 136 + 34 * j + lane, air_bool<F>(h));
+                pack(air_bxor<F>(o0, h), lo, hi);
                 if (lane == 16 + 2 * j) mine = sub(ld(so.r0 + 2 * j), lo);
                 if (lane == 17 + 2 * j) mine = sub(ld(so.r0 + 2 * j + 1), hi);
                 // outputs[1] = row1 ^ row3, outputs[2] = chaining_values[0] ^ helpers, outputs[3] = chaining_values[1] ^ row3 (k + 272 ..)
-                fold(k + 272 + 32 * j + lane, sub(o1, bxor(r1, r3)));
-                fold(k + 400 + 32 * j + lane, sub(o2, bxor(cv0, h)));
-                fold(k + 528 + 32 * j + lane, sub(o3, bxor(cv1, r3)));
+                fold(k + 272 + 32 * j + lane, sub(o1, air_bxor<F>(r1, r3)));
+                fold(k + 400 + 32 * j + lane, sub(o2, air_bxor<F>(cv0, h)));
+                fold(k + 528 + 32 * j + lane, sub(o3, air_bxor<F>(cv1, r3)));
             }
             if (lane < 8) fold(k + lane, mine);
             else if (lane >= 16 && lane < 24) fold(k + 136 + 34 * ((lane - 16) >> 1) + 32 + (lane & 1u), mine);
         }
-        u32 rr[4];
-#pragma unroll
-        for (int d = 0; d < 4; d++) rr[d] = mont_redc<F>(acc[d]);
-#pragma unroll
-        for (int o = 16; o; o >>= 1)
-#pragma unroll
-            for (int d = 0; d < 4; d++) rr[d] = add(rr[d], __shfl_xor_sync(0xffffffffu, rr[d], o));
-        const u32 out = lane == 0 ? rr[0] : lane == 1 ? rr[1] : lane == 2 ? rr[2] : rr[3];
-        if (lane < 4) a.q[4 * (size_t)i + lane] = mul(out, (i & 1u) ? a.izh[1] : a.izh[0]);
+        air_warp_store<F>(a, acc, i, lane);
     }
 }
 
@@ -317,36 +298,9 @@ int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size
     return field == BABY_BEAR ? b3_generate<BABY_BEAR>(ctx, d_inputs, n_hashes, d_trace) : b3_generate<KOALA_BEAR>(ctx, d_inputs, n_hashes, d_trace);
 }
 
-template <int F> static int32_t b3_quotient(p3gpu_ctx *ctx, const u32 *d_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
-    B3QArgs qa;
-    std::vector<u32> zh, izh;
-    const AirDomain dom = air_domain<F>(log_n + 1, log_n, 0, zh, izh);
-    qa.log_q = dom.log_q;
-    for (int j = 0; j < 2; j++) qa.izh[j] = izh[j];
-    const std::vector<uint4> ap = air_alpha_table<F>(alpha, B3_CONSTRAINTS);
-    void *tab = nullptr;
-    P3_TRY(ctx_scratch2(ctx, ap.size() * 16, &tab));
-    P3_CUDA(cudaMemcpyAsync(tab, ap.data(), ap.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
-    qa.lde = d_lde; qa.apow = static_cast<const uint4 *>(tab); qa.q = d_q;
-    auto kern = blake3_air_quotient_kernel<F>;
-    P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BQ_SMEM));
-    const size_t warps = (size_t)1 << (log_n + 1);
-    const unsigned grid = (unsigned)std::min<size_t>((size_t)ctx->sm_count, (warps + BQ_WARPS - 1) / BQ_WARPS);
-    kern<<<grid, 32 * BQ_WARPS, BQ_SMEM, ctx->stream>>>(qa);
-    ctx->launches++;
-    P3_CUDA(cudaGetLastError());
-    return P3GPU_OK;
-}
-
 int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Blake3 AIR: unsupported field %d", field);
-    const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
-    P3_CHECK(log_n + 1 <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL,
-             "Blake3 AIR quotient: need log_trace_height %u + 1 <= log_lde_height %u <= %u", log_n, log_lde, two_adicity);
-    P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 4 == 0 && reinterpret_cast<uintptr_t>(d_q) % 4 == 0, P3GPU_EINVAL,
-             "Blake3 AIR quotient: misaligned buffer");
-    return field == BABY_BEAR ? b3_quotient<BABY_BEAR>(ctx, d_lde, log_n, alpha, d_q) : b3_quotient<KOALA_BEAR>(ctx, d_lde, log_n, alpha, d_q);
+    return air_hand_quotient(ctx, field, "Blake3", (const void *)blake3_air_quotient_kernel<BABY_BEAR>, (const void *)blake3_air_quotient_kernel<KOALA_BEAR>,
+                             B3_CONSTRAINTS, BQ_WARPS, BQ_SMEM, 0, d_lde, log_lde, log_n, alpha, d_q);
 }
 
 }  // namespace p3

@@ -163,6 +163,11 @@ int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t 
 int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const u32 *d_lde, unsigned log_lde, const u32 *d_pre,
                              unsigned log_pre, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n,
                              const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
+// A hand-written AIR quotient kernel (AirHandQArgs, air_program.cuh) over the 2N points of GENERATOR * K from the first 2N rows of
+// the committed bit-reversed LDE: checks the field, the domain, the alignment and alpha (messages name the AIR), builds the domain
+// and the alpha^(K - 1 - k) table (scratch2), then launches `kern_<field>` on min(SMs, 2N / warps) blocks of `warps` warps.
+int32_t air_hand_quotient(p3gpu_ctx *ctx, int field, const char *name, const void *kern_babybear, const void *kern_koalabear, u32 n_constraints,
+                          unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
 
 // keccak_air.cu: Keccak-f AIR trace generation / quotient
 size_t keccak_air_height(size_t n_hashes);

@@ -111,19 +111,11 @@ constexpr int KQ_WARPS = 12;
 constexpr int KQ_ROW = KA_COLS + KA_NEXT_COLS;                       // staged words per warp
 constexpr size_t KQ_SMEM = (size_t)KA_CONSTRAINTS * 16 + (size_t)KQ_WARPS * KQ_ROW * 4;
 
-struct KaQArgs {
-    const u32 *lde;            // bit-reversed LDE prefix, >= 2^log_q rows x 2633
-    const uint4 *apow;         // alpha^(3181 - k), k < 3182
-    u32 *q;                    // 2^log_q x 4, natural order
-    AirDomain d;
-    u32 zh[2], izh[2];         // Z_H and 1 / Z_H by i mod 2
-};
-
 __device__ __forceinline__ void ka_cp_async4(u32 *dst, const u32 *src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
 }
 
-template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_quotient_kernel(const KaQArgs a) {
+template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_quotient_kernel(const AirHandQArgs a) {
     extern __shared__ uint4 kq_sm[];
     const uint4 *ap = kq_sm;
     for (int t = threadIdx.x; t < KA_CONSTRAINTS; t += blockDim.x) kq_sm[t] = __ldg(a.apow + t);
@@ -137,8 +129,6 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
     auto add = [](u32 x, u32 y) { return fp_add<F>(x, y); };
     auto sub = [](u32 x, u32 y) { return fp_sub<F>(x, y); };
     auto mul = [](u32 x, u32 y) { return mont_mul<F>(x, y); };
-    auto bxor = [](u32 x, u32 y) { return fp_sub<F>(fp_add<F>(x, y), fp_double<F>(mont_mul<F>(x, y))); };   // x + y - 2xy
-    auto bchk = [ONE](u32 x) { return mont_mul<F>(x, fp_sub<F>(x, ONE)); };                                 // x (x - 1)
     // (sum of this half warp's weighted v0, of its weighted v1): the limbs (lane / 16) and 2 + (lane / 16) of a 64-bit word
     auto limbs = [&](u32 v0, u32 v1, u32 &s0, u32 &s1) {
         s0 = mul(v0, wpow); s1 = mul(v1, wpow);
@@ -175,27 +165,27 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
             fold(48 + j, c);
         }
         // export is boolean (248) and zero unless final step (249)
-        if (lane < 2) fold(248 + lane, lane == 0 ? bchk(L[KA_EXPORT]) : mul(nf, L[KA_EXPORT]));
+        if (lane < 2) fold(248 + lane, lane == 0 ? air_bool<F>(L[KA_EXPORT]) : mul(nf, L[KA_EXPORT]));
         // per x: 64 c bools, then 64 c' = xor3(c[x][z], c[x-1][z], c[x+1][z-1]) (k 250..889)
 #pragma unroll 1
         for (int x = 0; x < 5; x++) {
             const u32 *c = L + KA_C + 64 * x, *cm = L + KA_C + 64 * ((x + 4) % 5), *cq = L + KA_C + 64 * ((x + 1) % 5), *cp = L + KA_CP + 64 * x;
             const int k = 250 + 128 * x;
-            fold(k + z0, bchk(c[z0])); fold(k + z1, bchk(c[z1]));
-            fold(k + 64 + z0, sub(cp[z0], bxor(bxor(c[z0], cm[z0]), cq[(z0 + 63) & 63])));
-            fold(k + 64 + z1, sub(cp[z1], bxor(bxor(c[z1], cm[z1]), cq[(z1 + 63) & 63])));
+            fold(k + z0, air_bool<F>(c[z0])); fold(k + z1, air_bool<F>(c[z1]));
+            fold(k + 64 + z0, sub(cp[z0], air_bxor<F>(air_bxor<F>(c[z0], cm[z0]), cq[(z0 + 63) & 63])));
+            fold(k + 64 + z1, sub(cp[z1], air_bxor<F>(air_bxor<F>(c[z1], cm[z1]), cq[(z1 + 63) & 63])));
         }
         // x-outer, y-inner: 64 a' bools, then a[y][x] limb = sum 2^z xor(a'[y][x][z], xor(c[x][z], c'[x][z])) (k 890..2589)
 #pragma unroll 1
         for (int x = 0; x < 5; x++) {
-            const u32 cc0 = bxor(L[KA_C + 64 * x + z0], L[KA_CP + 64 * x + z0]), cc1 = bxor(L[KA_C + 64 * x + z1], L[KA_CP + 64 * x + z1]);
+            const u32 cc0 = air_bxor<F>(L[KA_C + 64 * x + z0], L[KA_CP + 64 * x + z0]), cc1 = air_bxor<F>(L[KA_C + 64 * x + z1], L[KA_CP + 64 * x + z1]);
 #pragma unroll 1
             for (int y = 0; y < 5; y++) {
                 const u32 *apx = L + KA_AP + 64 * (5 * y + x);
                 const int k = 890 + 68 * (5 * x + y);
-                fold(k + z0, bchk(apx[z0])); fold(k + z1, bchk(apx[z1]));
+                fold(k + z0, air_bool<F>(apx[z0])); fold(k + z1, air_bool<F>(apx[z1]));
                 u32 s0, s1;
-                limbs(bxor(apx[z0], cc0), bxor(apx[z1], cc1), s0, s1);
+                limbs(air_bxor<F>(apx[z0], cc0), air_bxor<F>(apx[z1], cc1), s0, s1);
                 const u32 *al = L + KA_A + 4 * (5 * y + x);
                 if ((lane & 15u) == 0) fold(k + 64 + hl, sub(s0, al[hl]));
                 else if ((lane & 15u) == 1) fold(k + 66 + hl, sub(s1, al[2 + hl]));
@@ -226,7 +216,7 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
                     // B[bx][y][z] = a'[bx][(bx + 3y) % 5][(z - R) mod 64] (columns.rs b())
                     auto b = [&](int bx) { const int ax = (bx + 3 * y) % 5; return L[KA_AP + 64 * (5 * bx + ax) + ((z + 64 - KA_R[ax][bx]) & 63)]; };
                     const u32 andn = mul(sub(ONE, b((x + 1) % 5)), b((x + 2) % 5));
-                    v[h] = bxor(andn, b(x));
+                    v[h] = air_bxor<F>(andn, b(x));
                 }
                 u32 s0, s1;
                 limbs(v[0], v[1], s0, s1);
@@ -239,7 +229,7 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
         // a''[0,0] bits: bools (k 3010..3073), their limbs = a''[0][0] (3074..3077), iota: limbs of xor(rc bit, bit) = a''' (3078..3081)
         {
             const u32 b0 = L[KA_APP_BITS + z0], b1 = L[KA_APP_BITS + z1];
-            fold(3010 + z0, bchk(b0)); fold(3010 + z1, bchk(b1));
+            fold(3010 + z0, air_bool<F>(b0)); fold(3010 + z1, air_bool<F>(b1));
             u32 s0, s1;
             limbs(b0, b1, s0, s1);
             if ((lane & 15u) == 0) fold(3074 + hl, sub(s0, L[KA_APP + hl]));
@@ -251,7 +241,7 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
                 if ((rc >> z0) & 1) rc0 = add(rc0, L[KA_STEP + r]);
                 if ((rc >> z1) & 1) rc1 = add(rc1, L[KA_STEP + r]);
             }
-            limbs(bxor(rc0, b0), bxor(rc1, b1), s0, s1);
+            limbs(air_bxor<F>(rc0, b0), air_bxor<F>(rc1, b1), s0, s1);
             if ((lane & 15u) == 0) fold(3078 + hl, sub(s0, L[KA_APPP + hl]));
             else if ((lane & 15u) == 1) fold(3080 + hl, sub(s1, L[KA_APPP + 2 + hl]));
         }
@@ -261,15 +251,7 @@ template <int F> __global__ void __launch_bounds__(32 * KQ_WARPS, 1) keccak_air_
             const u32 out = yx == 0 ? L[KA_APPP + l] : L[KA_APP + 4 * yx + l];
             fold(3082 + j, mul(tnf, sub(out, N[KA_A + 4 * yx + l])));
         }
-        u32 r[4];
-#pragma unroll
-        for (int d = 0; d < 4; d++) r[d] = mont_redc<F>(acc[d]);
-#pragma unroll
-        for (int o = 16; o; o >>= 1)
-#pragma unroll
-            for (int d = 0; d < 4; d++) r[d] = add(r[d], __shfl_xor_sync(0xffffffffu, r[d], o));
-        const u32 mine = lane == 0 ? r[0] : lane == 1 ? r[1] : lane == 2 ? r[2] : r[3];
-        if (lane < 4) a.q[4 * (size_t)i + lane] = mul(mine, (i & 1u) ? a.izh[1] : a.izh[0]);
+        air_warp_store<F>(a, acc, i, lane);
     }
 }
 
@@ -304,35 +286,9 @@ int32_t keccak_air_generate(p3gpu_ctx *ctx, int field, const u64 *d_inputs, size
     return field == BABY_BEAR ? ka_generate<BABY_BEAR>(ctx, d_inputs, n_hashes, d_trace) : ka_generate<KOALA_BEAR>(ctx, d_inputs, n_hashes, d_trace);
 }
 
-template <int F> static int32_t ka_quotient(p3gpu_ctx *ctx, const u32 *d_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
-    KaQArgs qa;
-    std::vector<u32> zh, izh;
-    qa.d = air_domain<F>(log_n + 1, log_n, AIR_USES_NEXT | AIR_USES_SELECTORS, zh, izh);
-    for (int j = 0; j < 2; j++) { qa.zh[j] = zh[j]; qa.izh[j] = izh[j]; }
-    const std::vector<uint4> ap = air_alpha_table<F>(alpha, KA_CONSTRAINTS);
-    void *tab = nullptr;
-    P3_TRY(ctx_scratch2(ctx, ap.size() * 16, &tab));
-    P3_CUDA(cudaMemcpyAsync(tab, ap.data(), ap.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
-    qa.lde = d_lde; qa.apow = static_cast<const uint4 *>(tab); qa.q = d_q;
-    auto kern = keccak_air_quotient_kernel<F>;
-    P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KQ_SMEM));
-    const size_t warps = (size_t)1 << (log_n + 1);
-    const unsigned grid = (unsigned)std::min<size_t>((size_t)ctx->sm_count, (warps + KQ_WARPS - 1) / KQ_WARPS);
-    kern<<<grid, 32 * KQ_WARPS, KQ_SMEM, ctx->stream>>>(qa);
-    ctx->launches++;
-    P3_CUDA(cudaGetLastError());
-    return P3GPU_OK;
-}
-
 int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Keccak AIR: unsupported field %d", field);
-    const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
-    P3_CHECK(log_n + 1 <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL,
-             "Keccak AIR quotient: need log_trace_height %u + 1 <= log_lde_height %u <= %u", log_n, log_lde, two_adicity);
-    P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 4 == 0 && reinterpret_cast<uintptr_t>(d_q) % 4 == 0, P3GPU_EINVAL,
-             "Keccak AIR quotient: misaligned buffer");
-    return field == BABY_BEAR ? ka_quotient<BABY_BEAR>(ctx, d_lde, log_n, alpha, d_q) : ka_quotient<KOALA_BEAR>(ctx, d_lde, log_n, alpha, d_q);
+    return air_hand_quotient(ctx, field, "Keccak", (const void *)keccak_air_quotient_kernel<BABY_BEAR>, (const void *)keccak_air_quotient_kernel<KOALA_BEAR>,
+                             KA_CONSTRAINTS, KQ_WARPS, KQ_SMEM, AIR_USES_NEXT | AIR_USES_SELECTORS, d_lde, log_lde, log_n, alpha, d_q);
 }
 
 }  // namespace p3

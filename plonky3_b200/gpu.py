@@ -304,47 +304,48 @@ class Gpu:
     def keccak_air_generate_trace(self, field, inputs_dev):
         """(n, 25) contiguous CUDA int64 tensor of u64 lanes (input[x + 5 y] = state[x][y]) -> the (H, 2633) trace, padding included."""
         import torch
-        assert inputs_dev.is_cuda and inputs_dev.dtype == torch.int64 and inputs_dev.is_contiguous(), "inputs: contiguous CUDA int64 (n, 25)"
-        assert inputs_dev.dim() == 2 and int(inputs_dev.shape[1]) == 25
-        self._use_torch_stream()
-        n = int(inputs_dev.shape[0])
+        x = self._air_inputs(inputs_dev, torch.int64, 25); self._use_torch_stream()
+        n = int(x.shape[0])
         out = self._empty((self.keccak_air_height(n), _lib.KECCAK_AIR_COLS))
-        check(self.L.p3gpu_keccak_air_generate_trace_dev(self.h, field, inputs_dev.data_ptr() if n else None, n, out.data_ptr()))
+        check(self.L.p3gpu_keccak_air_generate_trace_dev(self.h, field, x.data_ptr() if n else None, n, out.data_ptr()))
         return out
 
     def keccak_air_quotient(self, field, lde_dev, log_trace_height, alpha):
-        """Quotient values (2^(log_trace_height + 1), 4) in natural order over GENERATOR * K from the first 2^(log_trace_height + 1)
-        rows of the committed bit-reversed LDE."""
-        m = self._dev(lde_dev); self._use_torch_stream()
-        H = int(m.shape[0]); log_h = H.bit_length() - 1
-        if H != 1 << log_h or int(m.shape[1]) != _lib.KECCAK_AIR_COLS:
-            raise _lib.P3GpuError(f"LDE of shape {tuple(m.shape)}: need 2^k rows x {_lib.KECCAK_AIR_COLS}", _lib.EINVAL)
-        q = self._empty((2 << log_trace_height, 4))
-        check(self.L.p3gpu_keccak_air_quotient_dev(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
-        return q
+        """`_air_quotient_2n` of the Keccak AIR (2633 columns)."""
+        return self._air_quotient_2n(self.L.p3gpu_keccak_air_quotient_dev, _lib.KECCAK_AIR_COLS, field, lde_dev, log_trace_height, alpha)
 
     # ------------------------------------------------------------------ Blake3 AIR
     def blake3_air_generate_trace(self, field, inputs_dev):
         """(n, 24) contiguous CUDA int32 tensor of u32 words (16 message words, 8 chaining-value words), n a power of two -> the
         (n, 9168) trace."""
         import torch
-        assert inputs_dev.is_cuda and inputs_dev.dtype == torch.int32 and inputs_dev.is_contiguous(), "inputs: contiguous CUDA int32 (n, 24)"
-        assert inputs_dev.dim() == 2 and int(inputs_dev.shape[1]) == 24
-        self._use_torch_stream()
-        n = int(inputs_dev.shape[0])
+        x = self._air_inputs(inputs_dev, torch.int32, 24); self._use_torch_stream()
+        n = int(x.shape[0])
         out = self._empty((n, _lib.BLAKE3_AIR_COLS))
-        check(self.L.p3gpu_blake3_air_generate_trace_dev(self.h, field, inputs_dev.data_ptr(), n, out.data_ptr()))
+        check(self.L.p3gpu_blake3_air_generate_trace_dev(self.h, field, x.data_ptr(), n, out.data_ptr()))
         return out
 
     def blake3_air_quotient(self, field, lde_dev, log_trace_height, alpha):
+        """`_air_quotient_2n` of the Blake3 AIR (9168 columns)."""
+        return self._air_quotient_2n(self.L.p3gpu_blake3_air_quotient_dev, _lib.BLAKE3_AIR_COLS, field, lde_dev, log_trace_height, alpha)
+
+    # ------------------------------------------------------------------ shared by the hand-written Keccak and Blake3 AIRs
+    @staticmethod
+    def _air_inputs(t, dtype, width):
+        """A trace generator's inputs: a contiguous CUDA (n, width) tensor of `dtype`."""
+        assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"inputs: contiguous CUDA {str(dtype).removeprefix('torch.')} (n, {width})"
+        assert t.dim() == 2 and int(t.shape[1]) == width
+        return t
+
+    def _air_quotient_2n(self, entry, width, field, lde_dev, log_trace_height, alpha):
         """Quotient values (2^(log_trace_height + 1), 4) in natural order over GENERATOR * K from the first 2^(log_trace_height + 1)
-        rows of the committed bit-reversed LDE."""
+        rows of the committed bit-reversed LDE of a `width`-column trace; `entry`: the AIR's p3gpu_*_air_quotient_dev."""
         m = self._dev(lde_dev); self._use_torch_stream()
         H = int(m.shape[0]); log_h = H.bit_length() - 1
-        if H != 1 << log_h or int(m.shape[1]) != _lib.BLAKE3_AIR_COLS:
-            raise _lib.P3GpuError(f"LDE of shape {tuple(m.shape)}: need 2^k rows x {_lib.BLAKE3_AIR_COLS}", _lib.EINVAL)
+        if H != 1 << log_h or int(m.shape[1]) != width:
+            raise _lib.P3GpuError(f"LDE of shape {tuple(m.shape)}: need 2^k rows x {width}", _lib.EINVAL)
         q = self._empty((2 << log_trace_height, 4))
-        check(self.L.p3gpu_blake3_air_quotient_dev(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
+        check(entry(self.h, field, m.data_ptr(), log_h, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
     # ------------------------------------------------------------------ any AIR as a constraint program

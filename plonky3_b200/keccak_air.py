@@ -19,7 +19,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .air import SymbolicAir
+from .air import KernelAir
 from .field import Field
 
 NUM_ROUNDS, U64_LIMBS, BITS_PER_LIMB = 24, 4, 16
@@ -187,10 +187,11 @@ def random_inputs(n: int, seed: int = 1) -> np.ndarray:
     return out.reshape(n, 25)
 
 
-class KeccakAir(SymbolicAir):
+class KeccakAir(KernelAir):
     """KeccakAir (keccak-air/src/air.rs) in the surface uni_stark.prove and verify read: width 2633, max_constraint_degree 3 (the
     DAG's), no public values, every column opened at the next point (BaseAir's default main_next_row_columns, which KeccakAir
     keeps).  `gpu`: a plonky3_b200.gpu.Gpu (or None for a verifier-only AIR)."""
+    air_name = "Keccak"
 
     def __init__(self, field: Field, gpu=None):
         super().__init__(field, WIDTH, eval_keccak, gpu=gpu)
@@ -205,17 +206,9 @@ class KeccakAir(SymbolicAir):
         """KeccakAir::generate_random_trace_rows(n, 0): the trace of `random_inputs(n)` (seed 1)."""
         import torch
         self._need_gpu("trace generation")
-        x = torch.from_numpy(random_inputs(n).view(np.int64))
-        if isinstance(getattr(self.gpu, "device", None), int):
-            x = x.to(f"cuda:{self.gpu.device}")
+        x = self._to_device(torch.from_numpy(random_inputs(n).view(np.int64)))
         return self.generate_trace_rows(x)
 
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
-        """uni-stark/src/prover.rs:462-827 on the hand-written kernel: `trace_lde_dev` holds the trace on GENERATOR * K, |K| = 2N, in
-        bit-reversed row order (the committed LDE's prefix).  Returns (2N, 4) in natural order."""
-        if len(public_values) != 0:
-            raise ValueError(f"{len(public_values)} public values given, the Keccak AIR has none")
-        if preprocessed_on_quotient_domain is not None:
-            raise ValueError("the Keccak AIR has no preprocessed columns")
-        self._need_gpu("quotient evaluation")
+    def _kernel_quotient(self, trace_lde_dev, log_degree: int, alpha):
+        """`trace_lde_dev`: the trace on GENERATOR * K, |K| = 2N (the committed LDE's prefix).  Returns (2N, 4)."""
         return self.gpu.keccak_air_quotient(self.field.id, trace_lde_dev, int(log_degree), alpha)

@@ -20,7 +20,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from .air import SymbolicAir
+from .air import KernelAir
 from .field import Field
 
 VECTOR_LEN = 8           # examples/src/airs.rs: P2_VECTOR_LEN = 1 << 3
@@ -83,11 +83,12 @@ def poseidon2_eval(field, constants, vector_len=8):
     return ev, vector_len * cols
 
 
-class VectorizedPoseidon2Air(SymbolicAir):
+class VectorizedPoseidon2Air(KernelAir):
     """VectorizedPoseidon2Air<KoalaBear, ..., WIDTH 16, SBOX_DEGREE 3, SBOX_REGISTERS 0, 4, 20, VECTOR_LEN 8> in the surface
     uni_stark.prove and verify read: width vector_len * (144 + rounds_p), max_constraint_degree 3 (the DAG's), no public values, and
     no transition constraints, so the next row is never opened (verifier.rs:431-440).  `gpu`: a plonky3_b200.gpu.Gpu (or None for a
     verifier-only AIR)."""
+    air_name = "Poseidon2"
 
     def __init__(self, field: Field, constants: RoundConstants, gpu, vector_len: int = VECTOR_LEN):
         eval_fn, width = poseidon2_eval(field, constants, vector_len)
@@ -115,13 +116,7 @@ class VectorizedPoseidon2Air(SymbolicAir):
         self._upload()
         return self.gpu.p2air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1), self.vector_len)
 
-    def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
-        """uni-stark/src/prover.rs:462-827 on the hand-written kernel, on the committed LDE (natural order over the quotient
-        domain)."""
-        if len(public_values) != 0:
-            raise ValueError(f"{len(public_values)} public values given, the Poseidon2 AIR has none")
-        if preprocessed_on_quotient_domain is not None:
-            raise ValueError("the Poseidon2 AIR has no preprocessed columns")
-        self._need_gpu("quotient evaluation")
+    def _kernel_quotient(self, trace_lde_dev, log_degree: int, alpha):
+        """`trace_lde_dev`: the whole committed LDE.  Returns (its height, 4)."""
         self._upload()
         return self.gpu.p2air_quotient(self.field.id, trace_lde_dev, log_degree, alpha, self.vector_len)

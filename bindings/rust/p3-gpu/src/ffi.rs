@@ -182,6 +182,16 @@ unsafe extern "C" {
     pub fn p3gpu_blake3_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
                                          alpha: *const u32, d_quotient: *mut u32) -> i32;
 
+    // Poseidon1 AIR (poseidon1-air, width 16): per-context constants (Poseidon1Constants::to_optimized's output, Montgomery words),
+    // trace generation and quotient values
+    pub fn p3gpu_p1air_set_constants(ctx: *mut P3GpuCtx, field: c_int, initial_full: *const u32, terminal_full: *const u32,
+                                     mds_circ_col: *const u32, first_round_constants: *const u32, m_i: *const u32, partial_rc: *const u32,
+                                     sparse_first_row: *const u32, v: *const u32, rounds_p: c_int) -> i32;
+    pub fn p3gpu_p1air_columns(field: c_int, rounds_p: c_int) -> usize;
+    pub fn p3gpu_p1air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_perms: usize, d_trace: *mut u32) -> i32;
+    pub fn p3gpu_p1air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_lde: *const u32, log_lde_height: c_uint,
+                                    log_trace_height: c_uint, alpha: *const u32, d_quotient: *mut u32) -> i32;
+
     // any AIR as a constraint program (symbolic expression DAG -> register program -> quotient kernel)
     pub fn p3gpu_air_program_create(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize, constraints: *const u32,
                                     n_constraints: usize, width: u32, n_public: u32, out: *mut *mut P3GpuAirProgram) -> i32;

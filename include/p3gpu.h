@@ -257,6 +257,30 @@ int32_t p3gpu_blake3_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uin
 int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
                                       const uint32_t alpha[4], uint32_t *d_quotient);
 
+/* ---- Poseidon1 AIR: the AIR of prove_prime_field_31 -o poseidon-1-permutations (poseidon1-air/src), width 16 -------------------
+ * VectorizedPoseidon1Air<F, 16, SBOX_DEGREE, SBOX_REGISTERS, 4, rounds_p, vector_len>: BabyBear x^7 with one S-box register,
+ * KoalaBear x^3 without.  No next-row reads, no selectors; constraints of degree 3, so two quotient chunks (log_blowup >= 1).
+ * Constants are per context: the arguments of Poseidon1Air::new(full, partial) as Poseidon1Constants::to_optimized returns them,
+ * Montgomery words: initial_full / terminal_full 4 x 16, mds_circ_col 16 (the circulant MDS's first column; its canonical entries
+ * must be below 2^12), first_round_constants 16, m_i 16 x 16 row-major, partial_rc rounds_p - 1 scalars, sparse_first_row and v
+ * rounds_p x 16 each.  rounds_p: 1..32 for BabyBear, a multiple of 4 in 4..32 for KoalaBear.  P3GPU_EINVAL: a NULL pointer, a
+ * non-canonical word, rounds_p out of range; P3GPU_EUNSUPPORTED: a field other than BabyBear / KoalaBear. */
+int32_t p3gpu_p1air_set_constants(p3gpu_ctx *ctx, int field, const uint32_t *initial_full, const uint32_t *terminal_full,
+                                  const uint32_t *mds_circ_col, const uint32_t *first_round_constants, const uint32_t *m_i,
+                                  const uint32_t *partial_rc, const uint32_t *sparse_first_row, const uint32_t *v, int rounds_p);
+/* columns of ONE permutation: 16 + 8 (16 REG + 16) + rounds_p (REG + 1), REG = 1 for BabyBear, 0 for KoalaBear (columns.rs); 0 for
+ * an unknown field */
+size_t p3gpu_p1air_columns(int field, int rounds_p);
+/* generate_vectorized_trace_rows (poseidon1-air/src/generation.rs): d_inputs n_perms x 16 Montgomery words (16-byte aligned) ->
+ * d_trace n_perms x columns, i.e. the (n_perms / vector_len) x (vector_len * columns) row-major trace.  P3GPU_ESTATE: constants
+ * not set, or set for the other field; P3GPU_EINVAL: a NULL or misaligned pointer, n_perms 0. */
+int32_t p3gpu_p1air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_perms, uint32_t *d_trace);
+/* quotient_values of the Poseidon1 AIR with vector_len permutations per row (a power of two <= 32), with the contract of
+ * p3gpu_keccak_air_quotient_dev (d_lde: 2^log_lde_height rows x vector_len * columns; 16-byte aligned for KoalaBear, 8-byte for
+ * BabyBear; the quotient is 2^(log_trace_height + 1) x 4).  P3GPU_ESTATE as for the trace. */
+int32_t p3gpu_p1air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_lde, unsigned log_lde_height,
+                                 unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient);
+
 /* ---- any AIR as a constraint program (DESIGN.md section 4.7) ----------------------------------------------------------------
  * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
  * (operands refer only to earlier nodes) plus the list of constrained nodes in assertion order.  The library compiles it once

@@ -37,6 +37,7 @@ EXPORTS = [
     "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
     "p3gpu_keccak_air_generate_trace_dev", "p3gpu_keccak_air_quotient_dev",
     "p3gpu_blake3_air_generate_trace_dev", "p3gpu_blake3_air_quotient_dev",
+    "p3gpu_p1air_set_constants", "p3gpu_p1air_columns", "p3gpu_p1air_generate_trace_dev", "p3gpu_p1air_quotient_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -142,6 +143,10 @@ def load():
         "p3gpu_keccak_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
         "p3gpu_blake3_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
         "p3gpu_blake3_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
+        "p3gpu_p1air_set_constants": (i32, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]),
+        "p3gpu_p1air_columns": (sz, [ci, ci]),
+        "p3gpu_p1air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
+        "p3gpu_p1air_quotient_dev": (i32, [vp, ci, ci, vp, cu, cu, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

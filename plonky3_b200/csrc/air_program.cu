@@ -187,10 +187,10 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const 
     return air_quotient_launch<KOALA_BEAR>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q);
 }
 
-// ---- hand-written AIR quotient kernels (keccak_air.cu, blake3_air.cu) -----------------------------------------------------
+// ---- hand-written AIR quotient kernels (keccak_air.cu, blake3_air.cu, poseidon1_air.cu) -----------------------------------
 template <int F>
 static int32_t hand_quotient_launch(p3gpu_ctx *ctx, const void *kern, u32 n_constraints, unsigned warps, size_t smem, u32 uses, const u32 *d_lde,
-                                    unsigned log_n, const u32 *alpha, u32 *d_q) {
+                                    unsigned log_n, const u32 *alpha, u32 *d_q, const u32 *consts, unsigned lanes) {
     for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
     AirHandQArgs qa;
     std::vector<u32> zh, izh;
@@ -201,9 +201,11 @@ static int32_t hand_quotient_launch(p3gpu_ctx *ctx, const void *kern, u32 n_cons
     P3_TRY(ctx_scratch2(ctx, ap.size() * 16, &tab));
     P3_CUDA(cudaMemcpyAsync(tab, ap.data(), ap.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
     qa.lde = d_lde; qa.apow = static_cast<const uint4 *>(tab); qa.q = d_q;
+    qa.consts = consts; qa.lanes = lanes;
     P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const size_t points = (size_t)1 << qa.d.log_q;                   // one warp per point, persistent blocks
-    const unsigned grid = (unsigned)std::min<size_t>((size_t)ctx->sm_count, (points + warps - 1) / warps);
+    const size_t points = (size_t)1 << qa.d.log_q;                   // `lanes` lanes per point, persistent blocks
+    const size_t per_block = (size_t)warps * 32 / lanes;
+    const unsigned grid = (unsigned)std::min<size_t>((size_t)ctx->sm_count, (points + per_block - 1) / per_block);
     void *args[] = {&qa};
     P3_CUDA(cudaLaunchKernel(kern, dim3(grid), dim3(32 * warps), args, smem, ctx->stream));
     ctx->launches++;
@@ -211,15 +213,17 @@ static int32_t hand_quotient_launch(p3gpu_ctx *ctx, const void *kern, u32 n_cons
 }
 
 int32_t air_hand_quotient(p3gpu_ctx *ctx, int field, const char *name, const void *kern_babybear, const void *kern_koalabear, u32 n_constraints,
-                          unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
+                          unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q,
+                          const u32 *consts, unsigned lanes) {
     P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "%s AIR: unsupported field %d", name, field);
     const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
     P3_CHECK(log_n + 1 <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL,
              "%s AIR quotient: need log_trace_height %u + 1 <= log_lde_height %u <= %u", name, log_n, log_lde, two_adicity);
     P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 4 == 0 && reinterpret_cast<uintptr_t>(d_q) % 4 == 0, P3GPU_EINVAL,
              "%s AIR quotient: misaligned buffer", name);
-    if (field == BABY_BEAR) return hand_quotient_launch<BABY_BEAR>(ctx, kern_babybear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q);
-    return hand_quotient_launch<KOALA_BEAR>(ctx, kern_koalabear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q);
+    if (field == BABY_BEAR)
+        return hand_quotient_launch<BABY_BEAR>(ctx, kern_babybear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes);
+    return hand_quotient_launch<KOALA_BEAR>(ctx, kern_koalabear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes);
 }
 
 }  // namespace p3

@@ -212,14 +212,16 @@ struct AirDomain {
     u32 periodic_mask;          // rows of the periodic table - 1 (natural index i reads row i & periodic_mask)
 };
 
-// Arguments of a hand-written AIR quotient kernel (keccak_air.cu, blake3_air.cu), launched by air_hand_quotient (air_program.cu):
-// 2N points of GENERATOR * K, |K| = 2N, read from the first 2N rows of the committed bit-reversed LDE.
+// Arguments of a hand-written AIR quotient kernel (keccak_air.cu, blake3_air.cu, poseidon1_air.cu), launched by air_hand_quotient
+// (air_program.cu): 2N points of GENERATOR * K, |K| = 2N, read from the first 2N rows of the committed bit-reversed LDE.
 struct AirHandQArgs {
     const u32 *lde;            // bit-reversed LDE prefix, >= 2^d.log_q rows x the AIR's width
     const uint4 *apow;         // alpha^(K - 1 - k), k < K
     u32 *q;                    // 2^d.log_q x 4, natural order
     AirDomain d;
     u32 zh[2], izh[2];         // Z_H and 1 / Z_H by i mod 2
+    const u32 *consts;         // the AIR's constants on the device, owned by the context (null for AIRs without any)
+    u32 lanes;                 // lanes per point: 32 (one warp per point) or the AIR's vector length
 };
 
 // selectors_on_coset (commit/src/domain.rs:321-361) at x_i = g * w_q^i, unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1.

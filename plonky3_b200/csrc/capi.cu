@@ -108,6 +108,7 @@ void p3gpu_ctx_destroy(p3gpu_ctx *ctx) {
     for (int f = 0; f < 2; f++) if (ctx->fold_table[f]) cudaFree(ctx->fold_table[f]);
     if (ctx->scratch) cudaFree(ctx->scratch);
     if (ctx->scratch2) cudaFree(ctx->scratch2);
+    if (ctx->p1_consts) cudaFree(ctx->p1_consts);
     for (int i = 0; i < 4; i++) if (ctx->pool[i]) cudaFree(ctx->pool[i]);
     if (ctx->xchg_stream) cudaStreamDestroy(ctx->xchg_stream);
     for (int q = 0; q < 16; q++) if (ctx->dma_stream[q]) { cudaStreamDestroy(ctx->dma_stream[q]); cudaEventDestroy(ctx->dma_done[q]); }
@@ -525,6 +526,29 @@ int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t 
     P3_ENTER(ctx);
     P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
     return blake3_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+
+// ---- Poseidon1 AIR: constants, trace generation + quotient (poseidon1_air.cu) -------------------------------
+int32_t p3gpu_p1air_set_constants(p3gpu_ctx *ctx, int field, const uint32_t *initial_full, const uint32_t *terminal_full,
+                                  const uint32_t *mds_circ_col, const uint32_t *first_round_constants, const uint32_t *m_i,
+                                  const uint32_t *partial_rc, const uint32_t *sparse_first_row, const uint32_t *v, int rounds_p) {
+    P3_ENTER(ctx);
+    P3_CHECK(initial_full && terminal_full && mds_circ_col && first_round_constants && m_i && sparse_first_row && v && (partial_rc || rounds_p == 1),
+             P3GPU_EINVAL, "null argument");
+    return p1air_set_constants(ctx, field, initial_full, terminal_full, mds_circ_col, first_round_constants, m_i, partial_rc, sparse_first_row, v,
+                               rounds_p);
+}
+size_t p3gpu_p1air_columns(int field, int rounds_p) { return p1air_columns(field, rounds_p); }
+int32_t p3gpu_p1air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_perms, uint32_t *d_trace) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && d_trace, P3GPU_EINVAL, "null argument");
+    return p1air_generate(ctx, field, d_inputs, n_perms, d_trace);
+}
+int32_t p3gpu_p1air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                 const uint32_t alpha[4], uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return p1air_quotient(ctx, field, vector_len, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
 }
 
 // ---- any AIR as a constraint program (air_program.cu) -------------------------------------------------

@@ -103,6 +103,10 @@ struct p3gpu_ctx {
     p3::Poseidon2Consts *p2_dev = nullptr;  // 4 entries
     alignas(8) unsigned char air_consts[1024];   // Poseidon2 AIR round constants (air.cu: AirConsts)
     int air_set = 0;
+    // Poseidon1 AIR constants (poseidon1_air.cu): a device buffer of this context, written by p3gpu_p1air_set_constants on the
+    // context's stream, freed at destroy; p1_field is the field they were set for (-1: not set)
+    uint32_t *p1_consts = nullptr;
+    int p1_field = -1, p1_rounds_p = 0;
 };
 
 namespace p3 {
@@ -165,9 +169,11 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, cons
                              const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
 // A hand-written AIR quotient kernel (AirHandQArgs, air_program.cuh) over the 2N points of GENERATOR * K from the first 2N rows of
 // the committed bit-reversed LDE: checks the field, the domain, the alignment and alpha (messages name the AIR), builds the domain
-// and the alpha^(K - 1 - k) table (scratch2), then launches `kern_<field>` on min(SMs, 2N / warps) blocks of `warps` warps.
+// and the alpha^(K - 1 - k) table (scratch2), then launches `kern_<field>` on min(SMs, 2N lanes / (32 warps)) blocks of `warps`
+// warps.  `lanes`: lanes per point (32: one warp per point); `consts`: the AIR's device constants, handed to the kernel.
 int32_t air_hand_quotient(p3gpu_ctx *ctx, int field, const char *name, const void *kern_babybear, const void *kern_koalabear, u32 n_constraints,
-                          unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+                          unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q,
+                          const u32 *consts = nullptr, unsigned lanes = 32);
 
 // keccak_air.cu: Keccak-f AIR trace generation / quotient
 size_t keccak_air_height(size_t n_hashes);
@@ -177,6 +183,14 @@ int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigne
 // blake3_air.cu: Blake3 AIR trace generation / quotient
 int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
 int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+
+// poseidon1_air.cu: Poseidon1 AIR constants (per context), trace generation / quotient
+size_t p1air_columns(int field, int rounds_p);          // 0 for an unknown field
+int32_t p1air_set_constants(p3gpu_ctx *ctx, int field, const u32 *initial_full, const u32 *terminal_full, const u32 *mds_circ_col,
+                            const u32 *first_round_constants, const u32 *m_i, const u32 *partial_rc, const u32 *sparse_first_row, const u32 *v,
+                            int rounds_p);
+int32_t p1air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_perms, u32 *d_trace);
+int32_t p1air_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
 
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);

@@ -329,7 +329,38 @@ class Gpu:
         """`_air_quotient_2n` of the Blake3 AIR (9168 columns)."""
         return self._air_quotient_2n(self.L.p3gpu_blake3_air_quotient_dev, _lib.BLAKE3_AIR_COLS, field, lde_dev, log_trace_height, alpha)
 
-    # ------------------------------------------------------------------ shared by the hand-written Keccak and Blake3 AIRs
+    # ------------------------------------------------------------------ Poseidon1 AIR
+    def p1air_set_constants(self, field, initial_full, terminal_full, mds_circ_col, first_round_constants, m_i, partial_rc,
+                            sparse_first_row, v, rounds_p):
+        """Poseidon1Air::new(full, partial) constants (Montgomery words) for this context; see p3gpu_p1air_set_constants."""
+        a = [np.ascontiguousarray(x, dtype=np.uint32).ravel() for x in
+             (initial_full, terminal_full, mds_circ_col, first_round_constants, m_i, partial_rc, sparse_first_row, v)]
+        rp = int(rounds_p)
+        sizes = (64, 64, 16, 16, 256, rp - 1, 16 * rp, 16 * rp)
+        if any(x.size != s for x, s in zip(a, sizes)):
+            raise _lib.P3GpuError(f"Poseidon1 constants of sizes {[x.size for x in a]}: need {list(sizes)}", _lib.EINVAL)
+        check(self.L.p3gpu_p1air_set_constants(self.h, field, *[x.ctypes.data if x.size else None for x in a], rp))
+        self._p1air_cols = int(self.L.p3gpu_p1air_columns(field, rp))
+
+    def p1air_generate_trace(self, field, inputs_dev, vector_len=8):
+        """(n_perms, 16) contiguous CUDA int32 tensor of Montgomery words, n_perms vector_len times a power of two -> the vectorised
+        trace (n_perms / vector_len, vector_len * columns)."""
+        import torch
+        x = self._air_inputs(inputs_dev, torch.int32, 16); self._use_torch_stream()
+        n = int(x.shape[0])
+        rows = n // vector_len
+        if n == 0 or n % vector_len or rows & (rows - 1):
+            raise _lib.P3GpuError(f"{n} permutations: need {vector_len} times a power of two", _lib.EINVAL)
+        out = self._empty((rows, vector_len * self._p1air_cols))
+        check(self.L.p3gpu_p1air_generate_trace_dev(self.h, field, x.data_ptr(), n, out.data_ptr()))
+        return out
+
+    def p1air_quotient(self, field, lde_dev, log_trace_height, alpha, vector_len=8):
+        """`_air_quotient_2n` of the Poseidon1 AIR (vector_len * columns)."""
+        entry = lambda h, f, *rest: self.L.p3gpu_p1air_quotient_dev(h, f, vector_len, *rest)
+        return self._air_quotient_2n(entry, vector_len * self._p1air_cols, field, lde_dev, log_trace_height, alpha)
+
+    # ------------------------------------------------------------------ shared by the hand-written Keccak, Blake3 and Poseidon1 AIRs
     @staticmethod
     def _air_inputs(t, dtype, width):
         """A trace generator's inputs: a contiguous CUDA (n, width) tensor of `dtype`."""

@@ -6,10 +6,10 @@ sequencing (the transcript's sponge itself runs on the device, challenger.py).  
 quotient chunks up to the blowup, preprocessed columns committed once by `setup_preprocessed`, periodic columns.  The AIR evaluates
 its own quotient on the device: a plain SymbolicAir through the constraint-program kernel (p3gpu_air_quotient_dev /
 p3gpu_air_quotient_layout_dev); poseidon2_air.VectorizedPoseidon2Air, the config-5 benchmark's AIR (`prove_prime_field_31 --field
-koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`), and
-keccak_air.KeccakAir through their hand-written kernels.  With `shard=distributed.ShardedTrace(...)` the same lines prove the
-Poseidon2 AIR with the trace's columns split over several GPUs, the shard standing in for the trace commit, the quotient values and
-the trace's row reads of the opening.
+koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`),
+keccak_air.KeccakAir, blake3_air.Blake3Air and poseidon1_air.VectorizedPoseidon1Air through their hand-written kernels.  With
+`shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns split over several GPUs, the
+shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
     alpha <- transcript;  quotient values on GENERATOR * K ................... air.quotient_values (p3gpu_p2air_quotient_dev, ...)
@@ -18,7 +18,8 @@ the trace's row reads of the opening.
     prove_fri: commit phase (fold + commit per round), grind, query openings . p3gpu_fri_fold_dev, p3gpu_challenger_grind,
                                                                                p3gpu_gather_rows_dev / p3gpu_merkle_paths_dev
 
-RoundConstants, VectorizedPoseidon2Air and VECTOR_LEN live in poseidon2_air and are re-exported here.
+RoundConstants, VectorizedPoseidon2Air and VECTOR_LEN live in poseidon2_air and are re-exported here, as are Poseidon1Constants and
+VectorizedPoseidon1Air from poseidon1_air.
 """
 from __future__ import annotations
 
@@ -34,6 +35,7 @@ from .fri import FriParameters, TwoAdicFriFolding, TwoAdicFriPcs, commit_phase
 from .merkle_tree import MerkleTreeMmcs
 from .poseidon2 import Poseidon2
 from .poseidon2_air import VECTOR_LEN, RoundConstants, VectorizedPoseidon2Air  # noqa: F401  (re-exported)
+from .poseidon1_air import Poseidon1Constants, VectorizedPoseidon1Air  # noqa: F401  (re-exported)
 
 
 @dataclass
@@ -143,7 +145,8 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
 def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
     """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
     call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air,
-    keccak_air.KeccakAir or blake3_air.Blake3Air.  `trace`: device (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
+    keccak_air.KeccakAir, blake3_air.Blake3Air or poseidon1_air.VectorizedPoseidon1Air.  `trace`: device (CUDA int32) matrix of
+    height 2^n.  `public_values`: canonical integers.
 
     `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
     after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is

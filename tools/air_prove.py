@@ -3,10 +3,13 @@ cap height 3.  One configuration per process:
 
     python tools/air_prove.py --air keccak --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air blake3 --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
+    python tools/air_prove.py --air poseidon1 --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
 
   keccak   `-o keccak-f-permutations -l 20`: 43,690 hashes, a 2^20 x 2633 trace (the trace and its LDE take 33 GB together)
   blake3   `-o blake-3-permutations` at 2^18 compressions, a 2^18 x 9168 trace (29 GB with its LDE; the reference's `-l 20`
            shape, a 38.5 GB trace with a 77 GB LDE, does not fit on one 80 GB card)
+  poseidon1  `-o poseidon-1-permutations -l 20`: 8 << log_rows permutations, 8 per row, the constants of
+           tests/golden/poseidon1_constants.json; a 2^20 x 1312 trace (KoalaBear, 5.5 GB) or 2^20 x 2384 (BabyBear, 10 GB)
 
 Times trace generation and the quotient kernel alone (CUDA events, median of --kernel-reps launches after a warm-up), and `prove`
 span by span (median of --reps proofs after one warm-up); then verifies the last proof.  Prints one JSON object with the card's name
@@ -27,7 +30,7 @@ sys.path.insert(0, str(ROOT))
 import numpy as np
 import torch
 
-from plonky3_b200 import blake3_air, keccak_air
+from plonky3_b200 import blake3_air, keccak_air, poseidon1_air
 from plonky3_b200.dft import Radix2DitParallel
 from plonky3_b200.field import BabyBear, KoalaBear
 from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
@@ -38,10 +41,27 @@ from plonky3_b200.uni_stark import KeccakStarkConfig, StarkConfig, prove, verify
 
 DATASHEET_HBM_BYTES_PER_S = 3.35e12          # NVIDIA H100 SXM data sheet, HBM3
 
-# --air: (module, AIR class, default --log-rows, hashes of a 2^log_rows trace, input dtype)
+
+def _poseidon1(f, gpu=None):
+    """VectorizedPoseidon1Air with the fixture's constants (the example binary's), optimized as the reference does."""
+    fx = json.loads((ROOT / "tests" / "golden" / "poseidon1_constants.json").read_text())[f.name]
+    return poseidon1_air.VectorizedPoseidon1Air(f, poseidon1_air.Poseidon1Constants.from_fixture(f, fx).to_optimized(), gpu)
+
+
+def _poseidon1_inputs(f, n):
+    """poseidon1_air.random_inputs(f, n), drawn by the C oracle of the same SmallRng: the scalar restatement takes minutes at
+    2^23 permutations."""
+    from oracle import p3_oracle as O
+    return O.SmallRng(1).field(f.id, 16 * n).reshape(n, 16)
+
+
+# --air: (AIR constructor (field, gpu), default --log-rows, hashes of a 2^log_rows trace, inputs (field, n), input dtype)
 AIRS = {
-    "keccak": (keccak_air, keccak_air.KeccakAir, 20, lambda log_rows: (1 << log_rows) // 24, np.int64),   # (24 n).next_power_of_two()
-    "blake3": (blake3_air, blake3_air.Blake3Air, 18, lambda log_rows: 1 << log_rows, np.int32),           # one compression per row
+    "keccak": (lambda f, gpu=None: keccak_air.KeccakAir(f, gpu), 20, lambda log_rows: (1 << log_rows) // 24,   # (24 n).next_power_of_two()
+               lambda f, n: keccak_air.random_inputs(n), np.int64),
+    "blake3": (lambda f, gpu=None: blake3_air.Blake3Air(f, gpu), 18, lambda log_rows: 1 << log_rows,           # one compression per row
+               lambda f, n: blake3_air.random_inputs(n), np.int32),
+    "poseidon1": (_poseidon1, 20, lambda log_rows: 8 << log_rows, _poseidon1_inputs, np.int32),               # 8 permutations per row
 }
 
 
@@ -65,11 +85,11 @@ def main():
     ap.add_argument("--air", choices=sorted(AIRS), required=True)
     ap.add_argument("--field", choices=["koala-bear", "baby-bear"], default="koala-bear")
     ap.add_argument("--config", choices=["keccak", "poseidon2"], default="keccak")
-    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak, 18 for blake3)")
+    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1, 18 for blake3)")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--kernel-reps", type=int, default=10)
     a = ap.parse_args()
-    mod, Air, default_log_rows, hashes, dtype = AIRS[a.air]
+    Air, default_log_rows, hashes, random_inputs, dtype = AIRS[a.air]
     log_rows = default_log_rows if a.log_rows is None else a.log_rows
     f = KoalaBear if a.field == "koala-bear" else BabyBear
     gpu = default_gpu(0)
@@ -82,9 +102,9 @@ def main():
         config = StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, FriParameters.new_benchmark_high_arity(m)), p24, 16)
     air = Air(f, gpu)
     n = hashes(log_rows)
-    inputs = torch.from_numpy(mod.random_inputs(n).view(dtype)).cuda()
+    inputs = torch.from_numpy(random_inputs(f, n).view(dtype)).cuda()
     trace = air.generate_trace_rows(inputs)
-    assert tuple(trace.shape) == (1 << log_rows, mod.WIDTH)
+    assert tuple(trace.shape) == (1 << log_rows, air.width())
     gen_ms = _events_median(lambda: air.generate_trace_rows(inputs), a.kernel_reps)
     trace_bytes = trace.numel() * 4
 
@@ -114,7 +134,7 @@ def main():
     verify_ms = (time.perf_counter() - t0) * 1e3
     print(json.dumps({
         "card_and_power_limit": _card(), "air": a.air, "field": a.field, "config": a.config, "hashes": n, "trace_rows": 1 << log_rows,
-        "width": mod.WIDTH, "trace_generation_ms": round(gen_ms, 3), "trace_bytes_written": trace_bytes,
+        "width": air.width(), "trace_generation_ms": round(gen_ms, 3), "trace_bytes_written": trace_bytes,
         "trace_generation_bytes_per_s": float("%.3g" % (trace_bytes / gen_ms * 1e3)),
         "quotient_kernel_ms": round(q_ms, 3), "quotient_lde_bytes_read": lde_bytes,
         "quotient_bytes_per_s": float("%.3g" % (lde_bytes / q_ms * 1e3)),

@@ -8,6 +8,9 @@ Run once as `python tools/gen_constants.py <Plonky3 checkout>`; outputs are comm
   tests/golden/poseidon2_kat.json  known-answer vectors of the default-constant permutations
                                    (koala-bear/src/poseidon2.rs:614-653, baby-bear/src/poseidon2.rs:599-639)
   tests/golden/two_adic_generators.json  (baby_bear.rs:48-53, koala_bear.rs:73-78)
+  tests/golden/poseidon1_constants.json  width-16 Poseidon1 of both fields (baby-bear/src/poseidon1.rs, koala-bear/src/poseidon1.rs,
+                                   {baby-bear,koala-bear}/src/mds.rs): rounds, S-box degree, the circulant MDS's first column,
+                                   the raw round constants and the known answer for input 0..15
 Only numbers are extracted, no code.
 """
 import json, re, sys, pathlib
@@ -63,7 +66,42 @@ def main():
     (OUT / "plonky3_b200" / "p2_constants.json").write_text(json.dumps(consts))
     (OUT / "tests" / "golden" / "poseidon2_kat.json").write_text(json.dumps(kats, indent=0))
     (OUT / "tests" / "golden" / "two_adic_generators.json").write_text(json.dumps(gens))
-    print({k: (len(v["external_initial"]), len(v["internal"])) for k, v in consts.items()}, {k: len(v) for k, v in gens.items()})
+    p1 = poseidon1()
+    (OUT / "tests" / "golden" / "poseidon1_constants.json").write_text(json.dumps(p1, indent=0))
+    print({k: (len(v["external_initial"]), len(v["internal"])) for k, v in consts.items()}, {k: len(v) for k, v in gens.items()},
+          {k: (v["rounds_f"], v["rounds_p"], v["sbox_degree"]) for k, v in p1.items() if k != "note"})
+
+
+def poseidon1():
+    """The width-16 Poseidon1 instances of prove_prime_field_31 -o poseidon-1-permutations (examples/examples/prove_prime_field_31.rs)."""
+    out = {"note": "width-16 Poseidon1; canonical values; mds_circ_col is the circulant MDS's first COLUMN, "
+                   "first_row_to_first_col of the first row in mds.rs (col[0] = row[0], col[i] = row[16 - i]); "
+                   "round_constants: rounds_f / 2 initial full rounds, rounds_p partial rounds, rounds_f / 2 terminal full rounds"}
+    for fld, d, pfx, half, part in (("baby_bear", "baby-bear", "BABYBEAR", "BABYBEAR_POSEIDON1_HALF_FULL_ROUNDS", "BABYBEAR_POSEIDON1_PARTIAL_ROUNDS_16"),
+                                    ("koala_bear", "koala-bear", "KOALABEAR", "KOALABEAR_POSEIDON_HALF_FULL_ROUNDS",
+                                     "KOALABEAR_POSEIDON_PARTIAL_ROUNDS_16")):
+        src = (REF / d / "src" / "poseidon1.rs").read_text()
+        num = lambda name: int(re.search(rf"pub const {name}: \w+ = (\d+);", src).group(1))
+        rounds_f, rounds_p, degree = 2 * num(half), num(part), num(f"{pfx}_S_BOX_DEGREE")
+        i = src.index(f"pub const {pfx}_POSEIDON1_RC_16")
+        blk = src[i: src.index("]);", i)]
+        rc = ints(re.sub(r"//[^\n]*", "", blk[blk.index("new_2d_array(") + len("new_2d_array("):]))
+        assert len(rc) == 16 * (rounds_f + rounds_p), len(rc)
+        mds = (REF / d / "src" / "mds.rs").read_text()
+        j = mds.index("MATRIX_CIRC_MDS_16_COL")
+        row = ints(mds[mds.index("&[", j) + 1: mds.index("])", j)])
+        assert len(row) == 16
+        col = [row[0]] + [row[16 - k] for k in range(1, 16)]
+        t = src.index("fn test_poseidon_width_16")
+        tb = src[t: src.index("assert_eq!", t)]
+        a = tb.index("new_array(")
+        b = tb.index("new_array(", a + 1)
+        kin, kout = ints(tb[a + 10: tb.index("]);", a)]), ints(tb[b + 10: tb.index("]);", b)])
+        assert kin == list(range(16)) and len(kout) == 16
+        out[fld] = {"width": 16, "rounds_f": rounds_f, "rounds_p": rounds_p, "sbox_degree": degree, "mds_circ_col": col,
+                    "round_constants": [rc[16 * r: 16 * r + 16] for r in range(rounds_f + rounds_p)],
+                    "kat_input": kin, "kat_expected": kout}
+    return out
 
 
 if __name__ == "__main__":

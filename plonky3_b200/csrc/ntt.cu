@@ -29,9 +29,10 @@
 // (radix_2_dit_parallel.rs:245, fri/src/two_adic_pcs.rs:313-318).  No standalone bit-reversal or scaling pass exists.
 // With two equal passes on the cp.async kernel (2^20 rows by default) the LDE is three launches: inverse pass 1, ONE fused
 // pass (ntt_lde_mid_kernel: inverse pass 2 and every coset's forward pass 1, tile by tile through shared memory and registers)
-// and forward pass 2, so the coefficients are written and read once.  Forward pass 2 runs on whole-row bands in 4-CTA clusters
-// (ntt_band_pass_kernel: one bulk copy per quarter band in and out, the two cross-quarter layers over distributed shared memory)
-// where a quarter band fits its ring slot.  Every other LDE runs the four passes as separate launches.
+// and forward pass 2, so the coefficients are written and read once.  Forward pass 2 runs on whole-row bands in 8-CTA clusters
+// (ntt_band_pass_kernel: one bulk copy per eighth of a band in and out, the three cross-CTA layers over distributed shared
+// memory, overlapped with another band's local layers) where an eighth fits its ring slot; matrices of up to 48 columns keep
+// 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  Every other LDE runs the four passes as separate launches.
 // The fused pass runs warp-specialised where its registers allow (all instances but the runtime-width one at r = 10): a producer
 // lane loads each tile with one tensor copy and owns the tile stores and their read-out waits (DESIGN 4.1).
 #include <algorithm>
@@ -538,24 +539,32 @@ ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
 // ---- last pass of the two-pass coset LDE on whole-row bands, in clusters of CL CTAs ------------------------------------
 // The forward networks' second pass (layers [n - R, n)) of coset block `coset` works on bands of 2^R CONTIGUOUS rows: band T is
 // rows T*2^R .. (T+1)*2^R - 1, one contiguous run of 2^R * w words in memory.  A cluster of CL CTAs takes a band, CTA q its rows
-// [q*RQ, (q+1)*RQ), RQ = 2^R / CL (its "quarter" at CL = 4): the quarter comes in as ONE 1-D bulk copy and leaves as ONE, with no
-// row segments, partial sectors or per-thread addresses.
-//   * step X: the band's first log2(CL) layers pair rows 2^R/2 .. RQ apart, i.e. row j of every quarter: one radix-CL step over
-//     distributed shared memory, CTA q taking rows j in [q*RQ/CL, (q+1)*RQ/CL) of the CL quarters (ld/st.shared::cluster), between
-//     two cluster barriers (every peer has its quarter; every peer has its results);
-//   * steps A and B: the remaining layers pair rows inside a quarter: two register steps on the quarter in place (as steps 1 and
-//     2 of ntt_pass_fast_kernel), then the final reduction, and one thread stores the quarter;
-//   * a 2-deep ring: thread 0 loads band k+1 into the other buffer (with its 2^R - 1 twiddles) once band k's exchange is over and
-//     the store of band k-1 has read that buffer out, so the load streams in during steps A and B and the store during the next
-//     band's exchange.
+// [q*RQ, (q+1)*RQ), RQ = 2^R / CL (its "part"): the part comes in as ONE 1-D bulk copy and leaves as ONE, with no row segments,
+// partial sectors or per-thread addresses.
+//   * step X: the band's first log2(CL) layers pair rows 2^R/2 .. RQ apart, i.e. row j of every part: one radix-CL step over
+//     distributed shared memory, CTA q taking rows j in [q*RQ/CL, (q+1)*RQ/CL) of the CL parts (ld/st.shared::cluster);
+//   * steps A and B: the remaining layers pair rows inside a part: two register steps on the part in place (as steps 1 and
+//     2 of ntt_pass_fast_kernel), then the final reduction;
+//   * three warp roles run at once, each on its own band, in "periods" that end with ONE cluster barrier of every thread: in
+//     period k the exchange warps run step X on band k+1, the local warps steps A and B on band k (exchanged in period k-1), and
+//     the copy warp keeps a 3-slot ring (band k in slot k % 3).  The barrier at the end of period k certifies that every peer has
+//     finished exchanging band k+1, that every CTA holds band k+2 (the copy warp waits its `full` mbarrier before arriving), and
+//     that nobody still reads a peer's slot the next period reuses;
+//   * the copy lane stores band k as soon as the local warps are done with it (named barrier 2), arrives on the cluster barrier,
+//     and only then waits until that store has read slot k % 3 out and loads band k+3 there (the thread that commits a bulk group
+//     is the one that can wait for it), so the read-out and the load overlap the next period's work.  Band k+3 is waited on at
+//     the end of period k+1.
 // Threads are laid along columns (item = row * w + column): every warp access to shared memory is a run of consecutive words.
-constexpr int BAND_THREADS = 512;
-constexpr size_t BAND_SLOT_BYTES = 100 * 1024;   // the largest quarter a ring slot takes (2^R/CL rows x w x 4 bytes)
+constexpr int BAND_XWARPS = 6, BAND_LWARPS = 14;   // exchange and local warps (chosen by measurement, DESIGN 4.1), plus the copy warp
+constexpr int BAND_THREADS = 32 * (BAND_XWARPS + BAND_LWARPS + 1), BAND_NARROW_THREADS = 512;
+constexpr size_t BAND_SLOT_BYTES = 50 * 1024;   // the largest part a ring slot takes (2^R/CL rows x w x 4 bytes)
 
 __device__ __forceinline__ u32 cluster_rank() { u32 r; asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned; barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ u32 cluster_map(u32 smem_addr, u32 rank) {
     u32 r;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
@@ -577,6 +586,145 @@ __device__ __forceinline__ void bulk_store(void *gmem, const void *smem, u32 byt
 // a: l0 = log_n - R_LOG, l1 = log_n (rows of a band contiguous), dense in / out blocks of a.n_cosets cosets, w % 4 == 0, 16-byte aligned.
 template <int F, int R_LOG, int CL>
 __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __grid_constant__ PassArgs a) {
+    constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
+    constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
+    constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
+    constexpr u32 NX = 32 * BAND_XWARPS, NL = 32 * BAND_LWARPS;    // threads [0, NX) exchange, [NX, NX + NL) local, then the copy warp
+    static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const u32 w = a.w;
+    const u32 qwords = RQ * w;                                     // one part
+    u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
+    uint2 *tws0 = reinterpret_cast<uint2 *>(data0 + 3 * qwords);
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(tws0 + 3 * R);
+    const u32 full_a = (u32)__cvta_generic_to_shared(full);
+    const u32 q = cluster_rank();
+    const u32 n_clusters = gridDim.x / CL, cid = blockIdx.x / CL;
+    const int band_log = a.log_n - R_LOG;
+    const u32 total = a.n_cosets << band_log;
+    const int n = (int)((total - 1 - cid) / n_clusters) + 1;      // this cluster's bands: cid + k * n_clusters, k < n (grid <= bands)
+
+    auto out_of = [&](u32 k, u32 &coset, u32 &T) { const u32 t = cid + k * n_clusters; coset = t >> band_log; T = t & ((1u << band_log) - 1u); };
+    auto issue = [&](u32 k) {   // copy lane: band k's part and twiddles into ring slot k % 3
+        u32 coset, T;
+        out_of(k, coset, T);
+        const u32 s = k % 3u;
+        const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
+        uint2 *tws = tws0 + s * R;
+        tws[1] = tw[((size_t)1 << a.l0) + T];
+        const u32 bar = full_a + 8 * s;
+        const bool load = !P3_SKIP(a.skip_load);
+        mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
+        if (load) bulk_load(data0 + s * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
+        load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+    };
+    auto wait_full = [&](u32 k) { mbar_wait(full_a + 8 * (k % 3u), (k / 3u) & 1u); };   // band k is slot k % 3's (k / 3)-th load
+
+    const bool copy_warp = threadIdx.x >= NX + NL, copy_lane = threadIdx.x == NX + NL;
+    if (threadIdx.x == 0) {
+        for (u32 s = 0; s < 3; s++) mbar_init(full_a + 8 * s, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (copy_lane)
+        for (int k = 0; k < 3 && k < n; k++) issue(k);
+    if (copy_warp) wait_full(0);
+    cluster_sync_all();   // every CTA of the cluster holds its part of band 0
+    // period k: exchange band k+1, local steps on band k; k = -1 only exchanges band 0
+    for (int k = -1; k < n; k++) {
+        if (threadIdx.x < NX) {
+            // ---- step X on band k+1: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p
+            if (k + 1 < n) {
+                const u32 s = (k + 1) % 3;
+                const uint2 *tws = tws0 + s * R;
+                u32 peer[CL];
+#pragma unroll
+                for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(data0 + s * qwords), (u32)p);
+                // an item is 4 adjacent columns: one 16-byte access per peer needs a quarter of the instructions of word accesses
+                const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (RQ / CL) * (w / 4), base = 16 * q * items;
+                for (u32 it = threadIdx.x; it < items; it += NX) {
+                    const u32 off = base + 16 * it;
+                    uint4 v[CL];
+#pragma unroll
+                    for (int p = 0; p < CL; p++) v[p] = ld_cluster_v4(peer[p] + off);
+#pragma unroll
+                    for (int e = 0; e < 4; e++) {
+                        u32 x[CL];
+#pragma unroll
+                        for (int p = 0; p < CL; p++) x[p] = (&v[p].x)[e];
+                        reg_network<F, LX>(x, tws, 1u);
+#pragma unroll
+                        for (int p = 0; p < CL; p++) (&v[p].x)[e] = x[p];
+                    }
+#pragma unroll
+                    for (int p = 0; p < CL; p++) st_cluster_v4(peer[p] + off, v[p]);
+                }
+            }
+            cluster_sync_all();
+        } else if (!copy_warp) {
+            if (k >= 0) {
+                const u32 s = k % 3, lt = threadIdx.x - NX;
+                u32 *data = data0 + s * qwords;
+                const uint2 *tws = tws0 + s * R;
+                // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
+                for (u32 it = lt; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += NL) {
+                    u32 *sp = data + it;
+                    u32 x[1 << QA];
+#pragma unroll
+                    for (u32 m = 0; m < (1u << QA); m++) x[m] = sp[m * (w << QB)];
+                    reg_network<F, QA>(x, tws, (1u << LX) + q);
+#pragma unroll
+                    for (u32 m = 0; m < (1u << QA); m++) sp[m * (w << QB)] = x[m];
+                }
+                asm volatile("bar.sync 1, %0;" ::"n"(NL) : "memory");
+                // ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB
+                for (u32 it = lt; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += NL) {
+                    const u32 g = it / w, c = it - g * w;
+                    u32 *sp = data + (g << QB) * w + c;
+                    u32 x[1 << QB];
+#pragma unroll
+                    for (u32 m = 0; m < (1u << QB); m++) x[m] = sp[m * w];
+                    reg_network<F, QB>(x, tws, (1u << (LX + QA)) + (q << QA) + g);
+                    if (a.final_reduce) {
+#pragma unroll
+                        for (u32 m = 0; m < (1u << QB); m++) x[m] = fp_reduce<F>(x[m]);
+                    }
+#pragma unroll
+                    for (u32 m = 0; m < (1u << QB); m++) sp[m * w] = x[m];
+                }
+                fence_proxy_async_smem();
+                asm volatile("bar.arrive 2, %0;" ::"n"(NL + 32) : "memory");   // band k may be stored
+            }
+            cluster_sync_all();
+        } else {
+            if (k + 2 < n) wait_full(k + 2);
+            if (k >= 0) {
+                asm volatile("bar.sync 2, %0;" ::"n"(NL + 32) : "memory");
+                if (copy_lane && !P3_SKIP(a.skip_store)) {
+                    u32 coset, T;
+                    out_of(k, coset, T);
+                    bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data0 + (k % 3) * qwords, qwords * 4);
+                }
+            }
+            __syncwarp();
+            cluster_arrive();
+            if (copy_lane && k >= 0 && k + 3 < n) {
+                bulk_wait_read();   // band k's store has read slot k % 3 out
+                issue(k + 3);
+            }
+            __syncwarp();
+            cluster_wait();
+        }
+    }
+    if (copy_lane) bulk_wait_all();
+    cluster_sync_all();   // no CTA exits while a peer may still map its shared memory
+}
+
+// Narrow matrices: the same pass in 4-CTA clusters with a 2-slot ring and no warp roles (every thread exchanges band k, then
+// runs its steps A and B, while thread 0 loads band k+1).  With little work per band the pass is bound by its per-band barriers,
+// and 4-CTA clusters (30 on the H100) take half as many bands each as 8-CTA clusters (15).
+template <int F, int R_LOG, int CL>
+__global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_kernel(const __grid_constant__ PassArgs a) {
     constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
     constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
     constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
@@ -626,7 +774,7 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
             // an item is 4 adjacent columns: one 16-byte access per peer keeps 4x the bytes in flight of word accesses (the exchange
             // is bound by the latency of remote shared memory, not by its bandwidth)
             const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (RQ / CL) * (w / 4), base = 16 * q * items;
-            for (u32 it = threadIdx.x; it < items; it += BAND_THREADS) {
+            for (u32 it = threadIdx.x; it < items; it += BAND_NARROW_THREADS) {
                 const u32 off = base + 16 * it;
                 uint4 v[CL];
 #pragma unroll
@@ -650,7 +798,7 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
             issue(t + n_clusters, buf ^ 1u);
         }
         // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
-        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += BAND_THREADS) {
+        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += BAND_NARROW_THREADS) {
             u32 *sp = data + it;
             u32 x[1 << QA];
 #pragma unroll
@@ -661,7 +809,7 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
         }
         __syncthreads();
         // ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB
-        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += BAND_THREADS) {
+        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += BAND_NARROW_THREADS) {
             const u32 g = it / w, c = it - g * w;
             u32 *sp = data + (g << QB) * w + c;
             u32 x[1 << QB];
@@ -1360,22 +1508,28 @@ static int32_t launch_fast(p3gpu_ctx *ctx, const PassArgs &a) {
     }
 }
 
-// Cluster size of the band pass: clusters of 4 and of 8 CTAs (221 KB of shared memory each) both fill 120 of the H100's 132 SMs
-// and stream at the same rate (tools/band_probe, DESIGN 4.1); 4 sends less over distributed shared memory (3/4 of each quarter
-// against 7/8).
-constexpr int BAND_CL = 4;
+// Cluster size of the band pass: clusters of 8 CTAs fill 120 of the H100's 132 SMs, as clusters of 4 do, and stream at the same
+// rate (tools/band_probe, DESIGN 4.1).  An eighth of a band is small enough for the 3-slot ring that lets the exchange of one band
+// run beside the local steps of another; the price is that 7/8 of each eighth crosses SMs instead of 3/4 of a quarter.
+constexpr int BAND_CL = 8;
 static bool band_pass_eligible(const PassArgs &a) {
     const int r = a.l1 - a.l0;
     return env_int("P3GPU_NTT_BAND", 1) != 0 && a.l1 == a.log_n && r >= 7 && r <= 10 && a.w % 4 == 0 && a.in_stride % 4 == 0 &&
            a.out_stride % 4 == 0 && ((reinterpret_cast<uintptr_t>(a.in) | reinterpret_cast<uintptr_t>(a.out)) % 16) == 0 &&
            (((size_t)a.w * 4) << r) / BAND_CL <= BAND_SLOT_BYTES;
 }
-template <int F, int R_LOG>
+// Widths up to BAND_NARROW_W take ntt_band_pass_narrow_kernel: at 2^20 rows it is the faster one up to 48 columns (0.13 against
+// 0.28 ms at 4, 0.41 against 0.50 at 48), the 8-CTA kernel from 64 (0.56 against 0.65 ms) and at every wider shape (DESIGN 4.1).
+constexpr u32 BAND_NARROW_W = 48;
+template <int F, int R_LOG, bool NARROW>
 static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
-    constexpr int CL = BAND_CL;
+    constexpr int CL = NARROW ? 4 : BAND_CL, SLOTS = NARROW ? 2 : 3;
     const size_t qbytes = (((size_t)a.w * 4) << R_LOG) / CL;
-    const size_t smem = 2 * (qbytes + ((size_t)1 << R_LOG) * sizeof(uint2) + 8);
-    auto kern = ntt_band_pass_kernel<F, R_LOG, CL>;
+    const size_t smem = SLOTS * (qbytes + ((size_t)1 << R_LOG) * sizeof(uint2) + 8);
+    const auto kern = [] {
+        if constexpr (NARROW) return ntt_band_pass_narrow_kernel<F, R_LOG, CL>;
+        else return ntt_band_pass_kernel<F, R_LOG, CL>;
+    }();
     // per instantiation and device: the shared memory limit and the number of clusters that fit at once, for the last size asked
     static size_t smem_set[64] = {0};
     static int clusters[64] = {0};
@@ -1384,7 +1538,7 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = CL; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
     cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(BAND_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = ctx->stream;
+    cfg.blockDim = dim3(NARROW ? BAND_NARROW_THREADS : BAND_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = ctx->stream;
     cfg.attrs = &attr; cfg.numAttrs = 1;
     if (smem != smem_set[dev]) {
         P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
@@ -1403,14 +1557,15 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
 }
 template <int F>
 static int32_t launch_band(p3gpu_ctx *ctx, PassArgs a) {
-    // profiling build only: NOLOAD / NOSTORE skip the quarter's bulk copies, NOBFLY bit 0 steps A and B, bit 1 the exchange
+    // profiling build only: NOLOAD / NOSTORE skip the part's bulk copies, NOBFLY bit 0 steps A and B, bit 1 the exchange
     a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0);
     a.skip_load = env_int("P3GPU_NTT_NOLOAD", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
+    const bool narrow = a.w <= BAND_NARROW_W;
     switch (a.l1 - a.l0) {
-        case 7: return launch_band_r<F, 7>(ctx, a);
-        case 8: return launch_band_r<F, 8>(ctx, a);
-        case 9: return launch_band_r<F, 9>(ctx, a);
-        default: return launch_band_r<F, 10>(ctx, a);
+        case 7: return narrow ? launch_band_r<F, 7, true>(ctx, a) : launch_band_r<F, 7, false>(ctx, a);
+        case 8: return narrow ? launch_band_r<F, 8, true>(ctx, a) : launch_band_r<F, 8, false>(ctx, a);
+        case 9: return narrow ? launch_band_r<F, 9, true>(ctx, a) : launch_band_r<F, 9, false>(ctx, a);
+        default: return narrow ? launch_band_r<F, 10, true>(ctx, a) : launch_band_r<F, 10, false>(ctx, a);
     }
 }
 
@@ -1904,8 +2059,9 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
         memset(&a, 0, sizeof a);
         a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
         a.tw = tw; a.tw_stride = h; a.in = d_out; a.in_stride = h * w; a.out = d_out; a.out_stride = h * w; a.final_reduce = 1;
-        // forward pass 2 reads and writes contiguous bands of 2^r rows: whole quarter bands as single bulk copies in 4-CTA clusters
-        // (ntt_band_pass_kernel) where a quarter fits a ring slot; P3GPU_NTT_BAND=0 keeps the tile kernel
+        // forward pass 2 reads and writes contiguous bands of 2^r rows: eighths of bands as single bulk copies in 8-CTA clusters
+        // (ntt_band_pass_kernel; up to 48 columns ntt_band_pass_narrow_kernel) where an eighth fits a ring slot; P3GPU_NTT_BAND=0
+        // keeps the tile kernel
         if (band_pass_eligible(a)) return launch_band<F>(ctx, a);
         return launch_pass<F>(ctx, a, (unsigned)n_cosets, 4);
     }

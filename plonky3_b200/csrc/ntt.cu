@@ -32,7 +32,10 @@
 // and forward pass 2, so the coefficients are written and read once.  Forward pass 2 runs on whole-row bands in 8-CTA clusters
 // (ntt_band_pass_kernel: one bulk copy per eighth of a band in and out, the three cross-CTA layers over distributed shared
 // memory, overlapped with another band's local layers) where an eighth fits its ring slot; matrices of up to 48 columns keep
-// 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  Every other LDE runs the four passes as separate launches.
+// 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  Inverse pass 1 runs on the same kernel where a part fits
+// (100 columns at 2^20 rows, 100-200 at 2^18), its "bands" being the strided units of rows 2^10 apart, each part moved by one 3-D
+// tensor copy.
+// Every other LDE runs the four passes as separate launches.
 // The fused pass runs warp-specialised where its registers allow (all instances but the runtime-width one at r = 10): a producer
 // lane loads each tile with one tensor copy and owns the tile stores and their read-out waits (DESIGN 4.1).
 #include <algorithm>
@@ -582,21 +585,41 @@ __device__ __forceinline__ void bulk_store(void *gmem, const void *smem, u32 byt
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gmem), "r"((u32)__cvta_generic_to_shared(smem)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// a strided unit's part through a 3-D tensor map (column, unit, row of the unit): see make_unit_tensor_map
+__device__ __forceinline__ void tma_load_part(const CUtensorMap *map, void *smem, u32 unit, u32 row0, u32 bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                 ::"r"((u32)__cvta_generic_to_shared(smem)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(0), "r"(unit), "r"(row0), "r"(bar)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_part(const CUtensorMap *map, const void *smem, u32 unit, u32 row0) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(reinterpret_cast<unsigned long long>(map)), "r"((u32)__cvta_generic_to_shared(smem)), "r"(0), "r"(unit), "r"(row0) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
 
 // a: l0 = log_n - R_LOG, l1 = log_n (rows of a band contiguous), dense in / out blocks of a.n_cosets cosets, w % 4 == 0, 16-byte aligned.
-template <int F, int R_LOG, int CL>
-__global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __grid_constant__ PassArgs a) {
+// STRIDED: the first pass of a network instead (l0 = 0, l1 = R_LOG, one block, no pitch).  Its "band" T is the strided unit of rows
+// T + 2^(log_n - R_LOG) * i, i < 2^R_LOG, so the same network runs on the unit's index i.  CTA q's part, rows i in [q*RQ, (q+1)*RQ),
+// comes in as ONE 3-D tensor copy (imap) and leaves as ONE 3-D tensor store (omap); every unit uses the same twiddles Z[1..2^R),
+// loaded once with slot 0's first load.  The network is linear, so the scale by a.scale is applied where the values leave step B, on
+// the 14 local warps: in step X it made the 6 exchange warps the ones that set the period (DESIGN 4.1).  The ring has a fourth slot,
+// which the one twiddle table leaves room for.
+template <int F, int R_LOG, int CL, bool STRIDED>
+__global__ void __launch_bounds__(BAND_THREADS, 1)
+ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap) {
     constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
     constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
     constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
     constexpr u32 NX = 32 * BAND_XWARPS, NL = 32 * BAND_LWARPS;    // threads [0, NX) exchange, [NX, NX + NL) local, then the copy warp
+    constexpr u32 NS = STRIDED ? 4 : 3;                            // ring slots
+    constexpr u32 TW_SLOTS = STRIDED ? 1 : NS;                     // twiddle tables: one per ring slot, or the one all units share
     static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const u32 w = a.w;
     const u32 qwords = RQ * w;                                     // one part
     u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
-    uint2 *tws0 = reinterpret_cast<uint2 *>(data0 + 3 * qwords);
-    unsigned long long *full = reinterpret_cast<unsigned long long *>(tws0 + 3 * R);
+    uint2 *tws0 = reinterpret_cast<uint2 *>(data0 + NS * qwords);
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(tws0 + TW_SLOTS * R);
     const u32 full_a = (u32)__cvta_generic_to_shared(full);
     const u32 q = cluster_rank();
     const u32 n_clusters = gridDim.x / CL, cid = blockIdx.x / CL;
@@ -605,29 +628,37 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
     const int n = (int)((total - 1 - cid) / n_clusters) + 1;      // this cluster's bands: cid + k * n_clusters, k < n (grid <= bands)
 
     auto out_of = [&](u32 k, u32 &coset, u32 &T) { const u32 t = cid + k * n_clusters; coset = t >> band_log; T = t & ((1u << band_log) - 1u); };
-    auto issue = [&](u32 k) {   // copy lane: band k's part and twiddles into ring slot k % 3
+    auto issue = [&](u32 k) {   // copy lane: band k's part and twiddles into ring slot k % NS
         u32 coset, T;
         out_of(k, coset, T);
-        const u32 s = k % 3u;
-        const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
-        uint2 *tws = tws0 + s * R;
-        tws[1] = tw[((size_t)1 << a.l0) + T];
+        const u32 s = k % NS;
         const u32 bar = full_a + 8 * s;
         const bool load = !P3_SKIP(a.skip_load);
-        mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
-        if (load) bulk_load(data0 + s * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
-        load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+        if constexpr (STRIDED) {
+            const bool tw = k == 0;
+            if (tw) tws0[1] = a.tw[1];
+            mbar_expect_tx(bar, (load ? qwords * 4 : 0) + (tw ? 8 * (R - 2) : 0));
+            if (load) tma_load_part(&imap, data0 + s * qwords, T, q * RQ, bar);
+            if (tw) load_tile_twiddles(tws0, a.tw, 0, 0, R_LOG, bar);
+        } else {
+            const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
+            uint2 *tws = tws0 + s * R;
+            tws[1] = tw[((size_t)1 << a.l0) + T];
+            mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
+            if (load) bulk_load(data0 + s * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
+            load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+        }
     };
-    auto wait_full = [&](u32 k) { mbar_wait(full_a + 8 * (k % 3u), (k / 3u) & 1u); };   // band k is slot k % 3's (k / 3)-th load
+    auto wait_full = [&](u32 k) { mbar_wait(full_a + 8 * (k % NS), (k / NS) & 1u); };   // band k is slot k % NS's (k / NS)-th load
 
     const bool copy_warp = threadIdx.x >= NX + NL, copy_lane = threadIdx.x == NX + NL;
     if (threadIdx.x == 0) {
-        for (u32 s = 0; s < 3; s++) mbar_init(full_a + 8 * s, 1);
+        for (u32 s = 0; s < NS; s++) mbar_init(full_a + 8 * s, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     if (copy_lane)
-        for (int k = 0; k < 3 && k < n; k++) issue(k);
+        for (int k = 0; k < (int)NS && k < n; k++) issue(k);
     if (copy_warp) wait_full(0);
     cluster_sync_all();   // every CTA of the cluster holds its part of band 0
     // period k: exchange band k+1, local steps on band k; k = -1 only exchanges band 0
@@ -635,8 +666,8 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
         if (threadIdx.x < NX) {
             // ---- step X on band k+1: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p
             if (k + 1 < n) {
-                const u32 s = (k + 1) % 3;
-                const uint2 *tws = tws0 + s * R;
+                const u32 s = (k + 1) % NS;
+                const uint2 *tws = tws0 + (STRIDED ? 0 : s * R);
                 u32 peer[CL];
 #pragma unroll
                 for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(data0 + s * qwords), (u32)p);
@@ -663,9 +694,9 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
             cluster_sync_all();
         } else if (!copy_warp) {
             if (k >= 0) {
-                const u32 s = k % 3, lt = threadIdx.x - NX;
+                const u32 s = k % NS, lt = threadIdx.x - NX;
                 u32 *data = data0 + s * qwords;
-                const uint2 *tws = tws0 + s * R;
+                const uint2 *tws = tws0 + (STRIDED ? 0 : s * R);
                 // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
                 for (u32 it = lt; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += NL) {
                     u32 *sp = data + it;
@@ -685,6 +716,10 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
 #pragma unroll
                     for (u32 m = 0; m < (1u << QB); m++) x[m] = sp[m * w];
                     reg_network<F, QB>(x, tws, (1u << (LX + QA)) + (q << QA) + g);
+                    if (STRIDED && a.has_scale) {
+#pragma unroll
+                        for (u32 m = 0; m < (1u << QB); m++) x[m] = shoup_mul<F>(x[m], a.scale);
+                    }
                     if (a.final_reduce) {
 #pragma unroll
                         for (u32 m = 0; m < (1u << QB); m++) x[m] = fp_reduce<F>(x[m]);
@@ -703,14 +738,15 @@ __global__ void __launch_bounds__(BAND_THREADS, 1) ntt_band_pass_kernel(const __
                 if (copy_lane && !P3_SKIP(a.skip_store)) {
                     u32 coset, T;
                     out_of(k, coset, T);
-                    bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data0 + (k % 3) * qwords, qwords * 4);
+                    if constexpr (STRIDED) tma_store_part(&omap, data0 + (k % NS) * qwords, T, q * RQ);
+                    else bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data0 + (k % NS) * qwords, qwords * 4);
                 }
             }
             __syncwarp();
             cluster_arrive();
-            if (copy_lane && k >= 0 && k + 3 < n) {
-                bulk_wait_read();   // band k's store has read slot k % 3 out
-                issue(k + 3);
+            if (copy_lane && k >= 0 && k + (int)NS < n) {
+                bulk_wait_read();   // band k's store has read slot k % NS out
+                issue(k + NS);
             }
             __syncwarp();
             cluster_wait();
@@ -1521,15 +1557,24 @@ static bool band_pass_eligible(const PassArgs &a) {
 // Widths up to BAND_NARROW_W take ntt_band_pass_narrow_kernel: at 2^20 rows it is the faster one up to 48 columns (0.13 against
 // 0.28 ms at 4, 0.41 against 0.50 at 48), the 8-CTA kernel from 64 (0.56 against 0.65 ms) and at every wider shape (DESIGN 4.1).
 constexpr u32 BAND_NARROW_W = 48;
-template <int F, int R_LOG, bool NARROW>
+static int32_t make_unit_tensor_map(const u32 *base, u32 w, int log_n, int r, u32 rows, CUtensorMap *tm);
+template <int F, int R_LOG, bool NARROW, bool STRIDED = false>
 static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
+    static_assert(!(NARROW && STRIDED), "the strided first pass runs in 8-CTA clusters only");
     constexpr int CL = NARROW ? 4 : BAND_CL, SLOTS = NARROW ? 2 : 3;
     const size_t qbytes = (((size_t)a.w * 4) << R_LOG) / CL;
-    const size_t smem = SLOTS * (qbytes + ((size_t)1 << R_LOG) * sizeof(uint2) + 8);
+    const size_t tw_bytes = ((size_t)1 << R_LOG) * sizeof(uint2);
+    const size_t smem = STRIDED ? 4 * (qbytes + 8) + tw_bytes : SLOTS * (qbytes + tw_bytes + 8);
     const auto kern = [] {
         if constexpr (NARROW) return ntt_band_pass_narrow_kernel<F, R_LOG, CL>;
-        else return ntt_band_pass_kernel<F, R_LOG, CL>;
+        else return ntt_band_pass_kernel<F, R_LOG, CL, STRIDED>;
     }();
+    CUtensorMap imap, omap;
+    memset(&imap, 0, sizeof imap); memset(&omap, 0, sizeof omap);
+    if constexpr (STRIDED) {
+        P3_TRY(make_unit_tensor_map(a.in, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &imap));
+        P3_TRY(make_unit_tensor_map(a.out, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &omap));
+    }
     // per instantiation and device: the shared memory limit and the number of clusters that fit at once, for the last size asked
     static size_t smem_set[64] = {0};
     static int clusters[64] = {0};
@@ -1551,7 +1596,8 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
     }
     const size_t bands = (size_t)a.n_cosets << (a.log_n - R_LOG);
     cfg.gridDim = dim3((unsigned)(CL * std::min<size_t>(bands, (size_t)clusters[dev])));
-    P3_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
+    if constexpr (NARROW) P3_CUDA(cudaLaunchKernelEx(&cfg, kern, a));
+    else P3_CUDA(cudaLaunchKernelEx(&cfg, kern, a, imap, omap));
     ctx->launches++;
     return P3GPU_OK;
 }
@@ -1566,6 +1612,30 @@ static int32_t launch_band(p3gpu_ctx *ctx, PassArgs a) {
         case 8: return narrow ? launch_band_r<F, 8, true>(ctx, a) : launch_band_r<F, 8, false>(ctx, a);
         case 9: return narrow ? launch_band_r<F, 9, true>(ctx, a) : launch_band_r<F, 9, false>(ctx, a);
         default: return narrow ? launch_band_r<F, 10, true>(ctx, a) : launch_band_r<F, 10, false>(ctx, a);
+    }
+}
+
+// The first pass of a network (l0 = 0, r = l1 layers) on strided units (ntt_band_pass_kernel<..., STRIDED>): one block, no pitch, a
+// part (2^r / 8 rows of w words) that fits a ring slot, and w within the 256-element tensor box; P3GPU_NTT_BAND=0 keeps the tile
+// kernel.  Below BAND_FIRST_MIN_W columns the tile kernel is the faster one, or no gain was measured (DESIGN 4.1).
+constexpr u32 BAND_FIRST_MIN_W = 100;
+static bool band_first_pass_eligible(const PassArgs &a) {
+    const int r = a.l1 - a.l0;
+    return env_int("P3GPU_NTT_BAND", 1) != 0 && a.l0 == 0 && r >= 7 && r <= 10 && a.n_cosets <= 1 && a.in_stride == 0 &&
+           a.out_stride == 0 && !a.in_bitrev && !a.out_bitrev && a.out_sh == 0 && a.out_add == 0 && a.w % 4 == 0 &&
+           a.w >= BAND_FIRST_MIN_W && a.w <= 256 && ((reinterpret_cast<uintptr_t>(a.in) | reinterpret_cast<uintptr_t>(a.out)) % 16) == 0 &&
+           (((size_t)a.w * 4) << r) / BAND_CL <= BAND_SLOT_BYTES;
+}
+template <int F>
+static int32_t launch_band_first(p3gpu_ctx *ctx, PassArgs a) {
+    a.n_cosets = 1;
+    a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0);
+    a.skip_load = env_int("P3GPU_NTT_NOLOAD", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
+    switch (a.l1) {
+        case 7: return launch_band_r<F, 7, false, true>(ctx, a);
+        case 8: return launch_band_r<F, 8, false, true>(ctx, a);
+        case 9: return launch_band_r<F, 9, false, true>(ctx, a);
+        default: return launch_band_r<F, 10, false, true>(ctx, a);
     }
 }
 
@@ -1662,6 +1732,20 @@ static int32_t make_pass_tensor_map(const PassArgs &a, const u32 *base, bool til
         strides[0] = pitch; strides[1] = pitch << gs_log; strides[2] = pitch; strides[3] = pitch << r;
     }
     const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
+    return P3GPU_OK;
+}
+
+// 3-D view of one dense 2^log_n x w block for the strided band pass: (column, unit L, i) at row L + 2^(log_n - r) * i; the box
+// (w, 1, rows) is one part, `rows` dense rows of w words in shared memory.  w % 4 == 0, w <= 256, base 16-byte aligned.
+static int32_t make_unit_tensor_map(const u32 *base, u32 w, int log_n, int r, u32 rows, CUtensorMap *tm) {
+    TensorMapEncodeFn enc = tensor_map_encoder();
+    P3_CHECK(enc != nullptr, P3GPU_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    const cuuint64_t pitch = (cuuint64_t)w * 4;
+    cuuint64_t dims[3] = {w, 1ull << (log_n - r), 1ull << r}, strides[2] = {pitch, pitch << (log_n - r)};
+    cuuint32_t box[3] = {w, 1, rows}, es[3] = {1, 1, 1};
+    const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, const_cast<u32 *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
     return P3GPU_OK;
@@ -2046,12 +2130,14 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
     if (bitrev_rows && (cp_async || pipe_mode() == 0) && run_plan.n_passes == 2 && 2 * r == log_n && r >= 7 && r <= 10 && n_cosets <= 4 &&
         lde_mid_tile_width((u32)w) != 0 && ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) % 16) == 0 &&
         tensor_map_encoder() != nullptr && !env_int("P3GPU_NTT_GENERIC", 0)) {
-        // inverse pass 1 and the fused pass store whole tiles with tensor copies
+        // inverse pass 1 runs on strided units (ntt_band_pass_kernel<..., STRIDED>) where it is eligible, else on the tile kernel;
+        // both it and the fused pass store whole tiles or parts with tensor copies
         PassArgs a;
         memset(&a, 0, sizeof a);
         a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = r; a.tma_store = 1;
         a.tw = tw_inv; a.in = d_in; a.out = (u32 *)coef; a.has_scale = 1; a.scale = inv_height_scale<F>(h);
-        P3_TRY(launch_pass<F>(ctx, a, 1, 4));
+        if (band_first_pass_eligible(a)) P3_TRY(launch_band_first<F>(ctx, a));
+        else P3_TRY(launch_pass<F>(ctx, a, 1, 4));
         memset(&a, 0, sizeof a);
         a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
         a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;

@@ -4,8 +4,12 @@
 //      left its buffer);
 //   2. the DSMEM rate of the radix-4 exchange in 4-CTA clusters: each CTA reads 3/4 of its 100 KB quarter's worth from its peers
 //      and writes 3/4 back, between two cluster barriers, 64 times (the bands a CTA takes at 2^20 x 100, blowup 2);
-//   3. cudaOccupancyMaxActiveClusters for clusters of 4 and 8 CTAs at 221 KB of dynamic shared memory, 512 threads.
+//   3. cudaOccupancyMaxActiveClusters for clusters of 4 and 8 CTAs at 221 KB of dynamic shared memory, 512 threads;
+//   4. the first pass's strided units (2^20 x 100: unit L = rows L + 1024 i, i < 1024), 15 clusters of 8 CTAs, a 3-slot ring, no
+//      arithmetic: CTA q moves rows i in [128q, 128q + 128) of each unit from one 419 MB buffer to another, either as ONE 3-D tensor
+//      copy in and ONE 3-D tensor store out per part, or as 128 1-D bulk copies of 400 bytes each way (4 per lane of one warp).
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 band_probe.cu -o band_probe
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cstdio>
@@ -81,6 +85,82 @@ __global__ void __launch_bounds__(THREADS, 1) dsmem_kernel(u32 iters, u32 *sink)
         cluster_sync();
     }
     if (acc == 0x9e3779b9u) sink[0] = acc;
+}
+
+// 4. strided units: 2^SU_LOG units of 2^SU_LOG rows (row L + 2^SU_LOG * i), SU_RQ rows of each per CTA, 3-slot ring per CTA
+constexpr int SU_LOG = 10;
+constexpr u32 SU_CL = 8, SU_RQ = (1u << SU_LOG) / SU_CL, SU_PWORDS = SU_RQ * W, SU_PBYTES = SU_PWORDS * 4;
+constexpr size_t SU_SMEM = 3 * (size_t)SU_PBYTES + 8192 + 64;   // as the band pass's ring: 3 parts + twiddles + barriers
+
+template <bool TENSOR>
+__global__ void __launch_bounds__(32, 1) strided_kernel(const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap,
+                                                        const u32 *src, u32 *dst) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    u32 *data = reinterpret_cast<u32 *>(smem);
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(smem + SU_SMEM - 64);
+    u32 q;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(q));
+    const u32 n_clusters = gridDim.x / SU_CL, cid = blockIdx.x / SU_CL, lane = threadIdx.x;
+    const u32 n = ((1u << SU_LOG) - 1 - cid) / n_clusters + 1;
+    if (lane == 0) {
+        for (int s = 0; s < 3; s++) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(sa(full + s)), "r"(TENSOR ? 1 : 32));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    auto load = [&](u32 k) {
+        const u32 s = k % 3, L = cid + k * n_clusters;
+        u32 *part = data + s * SU_PWORDS;
+        if (TENSOR) {
+            if (lane != 0) return;
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sa(full + s)), "r"(SU_PBYTES) : "memory");
+            asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                         ::"r"(sa(part)), "l"(reinterpret_cast<unsigned long long>(&imap)), "r"(0), "r"(L), "r"(q * SU_RQ), "r"(sa(full + s)) : "memory");
+        } else {
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sa(full + s)), "r"(SU_PBYTES / 32) : "memory");
+            for (u32 j = lane; j < SU_RQ; j += 32)
+                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                             ::"r"(sa(part + j * W)), "l"(src + ((size_t)L + ((size_t)(q * SU_RQ + j) << SU_LOG)) * W), "r"(W * 4), "r"(sa(full + s)) : "memory");
+        }
+    };
+    auto store = [&](u32 k) {
+        const u32 s = k % 3, L = cid + k * n_clusters;
+        const u32 *part = data + s * SU_PWORDS;
+        if (TENSOR) {
+            if (lane != 0) return;
+            asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                         ::"l"(reinterpret_cast<unsigned long long>(&omap)), "r"(sa(part)), "r"(0), "r"(L), "r"(q * SU_RQ) : "memory");
+        } else {
+            for (u32 j = lane; j < SU_RQ; j += 32)
+                asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+                             ::"l"(dst + ((size_t)L + ((size_t)(q * SU_RQ + j) << SU_LOG)) * W), "r"(sa(part + j * W)), "r"(W * 4) : "memory");
+        }
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    };
+    for (u32 k = 0; k < 3 && k < n; k++) load(k);
+    for (u32 k = 0; k < n; k++) {
+        mbar_wait(sa(full + k % 3), (k / 3) & 1);
+        cluster_sync();   // the band pass's one cluster barrier per period
+        store(k);
+        if (k + 3 < n) {
+            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // this lane's stores have read slot k % 3 out
+            __syncwarp();
+            load(k + 3);
+        }
+    }
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    cluster_sync();
+}
+
+typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
+                             const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// (column, unit L, i) over a 2^(2 SU_LOG) x W matrix: row L + 2^SU_LOG * i; box (W, 1, SU_RQ) = one part, dense in shared memory
+static int unit_map(EncodeFn enc, void *base, CUtensorMap *tm) {
+    cuuint64_t dims[3] = {W, 1ull << SU_LOG, 1ull << SU_LOG}, strides[2] = {(cuuint64_t)W * 4, ((cuuint64_t)W * 4) << SU_LOG};
+    cuuint32_t box[3] = {W, 1, SU_RQ}, es[3] = {1, 1, 1};
+    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 3, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { printf("cuTensorMapEncodeTiled: %d\n", (int)r); return 1; }
+    return 0;
 }
 
 template <typename K, typename... A>
@@ -159,5 +239,45 @@ int main() {
     printf("dsmem radix-4 exchange, %u CTAs x %u bands: median %.3f ms (min %.3f, max %.3f) = %.1f us per band, %.0f GB/s between SMs\n", grid,
            iters, ts[ts.size() / 2], ts[0], ts.back(), ts[ts.size() / 2] * 1e3 / iters, remote / (ts[ts.size() / 2] * 1e-3) / 1e9);
     CK(cudaFree(buf)); CK(cudaFree(sink));
+    // 4. strided units, buffer to buffer
+    EncodeFn enc = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    CK(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void **)&enc, cudaEnableDefault, &qres));
+    if (qres != cudaDriverEntryPointSuccess || enc == nullptr) { printf("no cuTensorMapEncodeTiled\n"); return 1; }
+    const size_t sbytes = ((size_t)W * 4) << (2 * SU_LOG);
+    u32 *src, *dst;
+    CK(cudaMalloc(&src, sbytes)); CK(cudaMalloc(&dst, sbytes));
+    CK(cudaMemset(src, 1, sbytes)); CK(cudaMemset(dst, 0, sbytes));
+    CUtensorMap imap, omap;
+    if (unit_map(enc, src, &imap) || unit_map(enc, dst, &omap)) return 1;
+    for (int tensor = 1; tensor >= 0; tensor--) {
+        const void *kern = tensor ? (const void *)strided_kernel<true> : (const void *)strided_kernel<false>;
+        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SU_SMEM));
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(15 * SU_CL); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = SU_SMEM;
+        cudaLaunchAttribute attr;
+        attr.id = cudaLaunchAttributeClusterDimension;
+        attr.val.clusterDim.x = SU_CL; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+        cfg.attrs = &attr; cfg.numAttrs = 1;
+        std::vector<float> st;
+        for (int rep = 0; rep < 22; rep++) {
+            CK(cudaEventRecord(e0));
+            if (tensor) CK(cudaLaunchKernelEx(&cfg, strided_kernel<true>, imap, omap, (const u32 *)src, dst));
+            else CK(cudaLaunchKernelEx(&cfg, strided_kernel<false>, imap, omap, (const u32 *)src, dst));
+            CK(cudaEventRecord(e1));
+            CK(cudaEventSynchronize(e1));
+            float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+            if (rep >= 2) st.push_back(ms);
+        }
+        std::vector<u32> chk(4096);
+        CK(cudaMemcpy(chk.data(), dst + sbytes / 4 - chk.size(), chk.size() * 4, cudaMemcpyDeviceToHost));
+        const bool copied = std::all_of(chk.begin(), chk.end(), [](u32 v) { return v == 0x01010101u; });
+        CK(cudaMemset(dst, 0, sbytes));
+        std::sort(st.begin(), st.end());
+        printf("strided units 2^%d x %u, 15 x %u CTAs, %s: %zu MB read + %zu MB written: median %.3f ms (min %.3f, max %.3f) = %.0f GB/s%s\n",
+               2 * SU_LOG, W, SU_CL, tensor ? "3-D tensor copies" : "1-D row copies", sbytes >> 20, sbytes >> 20, st[st.size() / 2], st[0],
+               st.back(), 2.0 * sbytes / (st[st.size() / 2] * 1e-3) / 1e9, copied ? "" : " (COPY WRONG)");
+    }
+    CK(cudaFree(src)); CK(cudaFree(dst));
     return 0;
 }

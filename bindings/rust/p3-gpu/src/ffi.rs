@@ -166,6 +166,7 @@ unsafe extern "C" {
     pub fn p3gpu_p2air_set_constants(ctx: *mut P3GpuCtx, field: c_int, beginning_full: *const u32, partial: *const u32, rounds_p: c_int,
                                      ending_full: *const u32) -> i32;
     pub fn p3gpu_p2air_columns(rounds_p: c_int) -> usize;
+    pub fn p3gpu_p2air_field_columns(field: c_int, rounds_p: c_int) -> usize;
     pub fn p3gpu_p2air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_perms: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_p2air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_lde: *const u32, log_lde_height: c_uint,
                                     log_trace_height: c_uint, alpha: *const u32, d_quotient: *mut u32) -> i32;

@@ -204,25 +204,35 @@ int32_t p3gpu_pcs_commit(p3gpu_ctx *ctx, int field, int hash, const uint32_t *h_
                          uint32_t *h_cap, size_t *cap_len);
 
 /* ---- Poseidon2 AIR (SURVEY.md 8f ranks 2-3): the AIR of prove_prime_field_31 -o poseidon-2-permutations ---------------
- * VectorizedPoseidon2Air<KoalaBear, width 16, S-box degree 3, 0 S-box registers, 4 + rounds_p + 4 rounds> (poseidon2-air/src/
- * air.rs, vectorized.rs).  Only the KoalaBear instance is built (BabyBear's degree-7 S-box needs register columns).
- * RoundConstants::new (poseidon2-air/src/constants.rs:47-57): 4 x 16 beginning, rounds_p partial, 4 x 16 ending, Montgomery. */
+ * VectorizedPoseidon2Air<F, width 16, SBOX_DEGREE, SBOX_REGISTERS, 4 + rounds_p + 4 rounds> (poseidon2-air/src/air.rs,
+ * vectorized.rs) in the example's two instances: KoalaBear (S-box degree 3, no S-box register) and BabyBear (degree 7 with one
+ * register: the committed x^3).  Constraints of degree 3, no next-row reads, no selectors: two quotient chunks.
+ * RoundConstants::new (poseidon2-air/src/constants.rs:47-57): 4 x 16 beginning, rounds_p partial, 4 x 16 ending, Montgomery.
+ * Constants are per context, stored with the field they were set for.  rounds_p: a multiple of 4 in 4..32 for KoalaBear, 1..32
+ * for BabyBear.  P3GPU_EINVAL: a NULL pointer, a non-canonical word, rounds_p out of range; P3GPU_EUNSUPPORTED: another field.
+ * The entry points below return P3GPU_ESTATE when the constants are not set, or were set for the other field. */
 int32_t p3gpu_p2air_set_constants(p3gpu_ctx *ctx, int field, const uint32_t *beginning_full, const uint32_t *partial, int rounds_p,
                                   const uint32_t *ending_full);
-/* columns of ONE permutation: 16 inputs + 4*16 + rounds_p + 4*16 (columns.rs:11-48) */
+/* columns of ONE KoalaBear permutation: 16 inputs + 4*16 + rounds_p + 4*16 (columns.rs:11-48) */
 size_t p3gpu_p2air_columns(int rounds_p);
+/* columns of ONE permutation of the field's instance: 16 + 8 (16 REG + 16) + rounds_p (REG + 1), REG = 1 for BabyBear, 0 for
+ * KoalaBear (columns.rs); 0 for an unknown field */
+size_t p3gpu_p2air_field_columns(int field, int rounds_p);
 /* generate_vectorized_trace_rows (poseidon2-air/src/generation.rs:14-70): d_inputs n_perms x 16 -> d_trace n_perms x columns,
  * i.e. the (n_perms / VECTOR_LEN) x (VECTOR_LEN * columns) row-major trace. */
 int32_t p3gpu_p2air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_perms, uint32_t *d_trace);
 /* quotient_values (uni-stark/src/prover.rs:462-827) of that AIR over the quotient domain GENERATOR * K with |K| = the LDE height
  * (log_quotient_degree == log_blowup: the truncation fast path of get_evaluations_on_domain, two_adic_pcs.rs:376-385).
- * d_lde: the committed trace LDE, 2^log_lde_height rows in bit-reversed order, vector_len * columns wide.
- * d_quotient: 2^log_lde_height EF4 values in NATURAL order (what commit_quotient / split_evals consume). */
+ * d_lde: the committed trace LDE, 2^log_lde_height rows in bit-reversed order, vector_len * columns wide; 16-byte aligned for
+ * KoalaBear, 8-byte for BabyBear.
+ * d_quotient: 2^log_lde_height EF4 values in NATURAL order (what commit_quotient / split_evals consume), 16-byte aligned. */
 int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_lde, unsigned log_lde_height,
                                  unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient);
 /* Columns [col0, col1) of the trace p3gpu_p2air_generate_trace_dev writes for the same inputs (n_perms a multiple of
  * vector_len): d_out is the dense (n_perms / vector_len) x (col1 - col0) matrix — one rank's column block of a sharded prove,
- * built without the full trace.  The window may cut a permutation. */
+ * built without the full trace.  The window may cut a permutation.  KoalaBear only, as is p3gpu_p2air_quotient_sharded_dev:
+ * the sharded quotient reads 16-byte units of 4-column segments, and a BabyBear permutation (298 columns) starts mid-unit every
+ * other time; both return P3GPU_EUNSUPPORTED for BabyBear. */
 int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms,
                                             size_t col0, size_t col1, uint32_t *d_out);
 

@@ -26,7 +26,7 @@ EXPORTS = [
     "p3gpu_merkle_total_digests", "p3gpu_merkle_commit_dev", "p3gpu_merkle_commit", "p3gpu_merkle_from_digests_dev",
     "p3gpu_fri_fold_dev", "p3gpu_fri_fold", "p3gpu_ef_axpy_dev", "p3gpu_fri_commit_phase_dev", "p3gpu_pcs_commit_dev",
     "p3gpu_open_inv_denoms_dev", "p3gpu_columnwise_dot_dev", "p3gpu_rowwise_dot_dev", "p3gpu_open_reduce_dev",
-    "p3gpu_pcs_commit", "p3gpu_p2air_set_constants", "p3gpu_p2air_columns", "p3gpu_p2air_generate_trace_dev", "p3gpu_p2air_quotient_dev",
+    "p3gpu_pcs_commit", "p3gpu_p2air_set_constants", "p3gpu_p2air_columns", "p3gpu_p2air_field_columns", "p3gpu_p2air_generate_trace_dev", "p3gpu_p2air_quotient_dev",
     "p3gpu_challenger_new", "p3gpu_challenger_free", "p3gpu_challenger_clone", "p3gpu_challenger_observe_dev", "p3gpu_challenger_observe",
     "p3gpu_challenger_sample", "p3gpu_challenger_grind", "p3gpu_gather_rows_dev", "p3gpu_merkle_paths_dev",
     "p3gpu_ipc_export", "p3gpu_ipc_import", "p3gpu_ipc_close", "p3gpu_memset_dev", "p3gpu_peer_barrier_dev",
@@ -106,6 +106,7 @@ def load():
         "p3gpu_pcs_commit": (i32, [vp, ci, ci, vp, sz, sz, cu, cu, vp, vp, vp, vp, vp, vp]),
         "p3gpu_p2air_set_constants": (i32, [vp, ci, vp, vp, ci, vp]),
         "p3gpu_p2air_columns": (sz, [ci]),
+        "p3gpu_p2air_field_columns": (sz, [ci, ci]),
         "p3gpu_p2air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
         "p3gpu_p2air_quotient_dev": (i32, [vp, ci, ci, vp, cu, cu, vp, vp]),
         "p3gpu_challenger_new": (i32, [vp, ci, ci, ci, C.POINTER(vp)]),

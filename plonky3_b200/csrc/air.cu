@@ -1,11 +1,15 @@
 // Poseidon2 AIR on the device (SURVEY.md section 8f ranks 2 and 3): trace generation and quotient evaluation for
-// VectorizedPoseidon2Air<KoalaBear, WIDTH 16, S-box degree 3, 0 S-box registers, 4 + 20 + 4 rounds, VECTOR_LEN permutations per row>
-// — the AIR of `prove_prime_field_31 --field koala-bear --objective poseidon-2-permutations` (BASELINE config 5,
-// examples/examples/prove_prime_field_31.rs:150-165).
+// VectorizedPoseidon2Air<F, WIDTH 16, SBOX_DEGREE, SBOX_REGISTERS, 4 + rounds_p + 4 rounds, VECTOR_LEN permutations per row>
+// — the AIR of `prove_prime_field_31 --objective poseidon-2-permutations` (examples/examples/prove_prime_field_31.rs), in its
+// two instances:
+//   KoalaBear (BASELINE config 5): x^3 S-box, no register, 20 partial rounds, 164 columns per permutation
+//   BabyBear: x^7 S-box with one register (the committed x^3; the S-box output is x3^2 x), 13 partial rounds, 298 columns
 //
-//   trace generation   poseidon2-air/src/generation.rs:14-70,184-253: one permutation -> 164 columns
-//                      inputs[16] | 4 x post[16] | rounds_p x post_sbox | 4 x post[16]; a vectorised row is VECTOR_LEN of them
-//   constraints        poseidon2-air/src/air.rs:173-296 (one assert_eq per post / post_sbox column, all of degree 3, no selectors),
+//   trace generation   poseidon2-air/src/generation.rs:14-70,184-253: one permutation ->
+//                      inputs[16] | 4 x {sbox[16 REG], post[16]} | rounds_p x {sbox[REG], post_sbox} | 4 x {sbox[16 REG], post[16]};
+//                      a vectorised row is VECTOR_LEN of them (REG = p2_reg<F>(), columns.rs)
+//   constraints        poseidon2-air/src/air.rs:173-296, all of degree 3, no selectors: per full round the 16 register checks
+//                      x3 - x^3 (REG = 1), then one assert_eq per post; per partial round the register check, then post_sbox;
 //                      vectorised poseidon2-air/src/vectorized.rs:297-311
 //   quotient           uni-stark/src/prover.rs:462-827: fold the constraints with powers of alpha (the first asserted constraint
 //                      gets the highest power, uni-stark/src/folder.rs), multiply by 1/Z_H (commit/src/domain.rs:321-361)
@@ -27,6 +31,11 @@ struct AirConsts {
 static_assert(sizeof(AirConsts) <= 1024, "kernel parameter budget");
 
 constexpr int AIR_W = 16;
+// S-box registers per S-box: the instance is a compile-time property of the field
+template <int F> __host__ __device__ constexpr int p2_reg() { return F == BABY_BEAR ? 1 : 0; }
+// columns / constraints of one permutation: 16 inputs + 8 full rounds x 16 (REG + 1) + rounds_p (REG + 1) (columns.rs)
+__host__ __device__ constexpr size_t p2_cols(int reg, int rp) { return 16 + (size_t)(8 * AIR_W + rp) * (reg + 1); }
+__host__ __device__ constexpr int p2_constraints(int reg, int rp) { return (8 * AIR_W + rp) * (reg + 1); }
 
 template <int F> __device__ __forceinline__ void air_internal_layer(u32 (&s)[AIR_W]) {
     u32 part = s[1];
@@ -48,9 +57,12 @@ template <int F> __device__ __forceinline__ void air_internal_layer(u32 (&s)[AIR
 // still evaluated (its later columns depend on all earlier rounds); only the stores are filtered.
 struct GenWindow { size_t col0, col1; unsigned vec_len; };
 
+// REG = 1 (BabyBear): a full round is written as its 16 registers, then its 16 posts; the partial rounds' (register, post_sbox)
+// pairs go through the tile 16 rounds (32 words per permutation) at a time.
 template <int F, bool WINDOW>
 __global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, size_t n_perms, u32 *trace, const __grid_constant__ AirConsts k,
                                                              const GenWindow win) {
+    constexpr int REG = p2_reg<F>();
     __shared__ u32 tiles[4][32 * 33];
     u32 *tile = tiles[threadIdx.x >> 5];
     const unsigned lane = threadIdx.x & 31u;
@@ -58,7 +70,7 @@ __global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, 
     if (p0 >= n_perms) return;
     const size_t p = p0 + lane;
     const bool live = p < n_perms;
-    const size_t cols = 144 + (size_t)k.rounds_p;
+    const size_t cols = REG ? p2_cols(REG, k.rounds_p) : 144 + (size_t)k.rounds_p;
     const unsigned n_warp = (unsigned)min((size_t)32, n_perms - p0);
     // write `n` values per permutation (held as tile[perm * (n + 1) + i]) to columns [off, off + n) of the warp's rows
     auto flush = [&](unsigned n, size_t off) {
@@ -91,27 +103,60 @@ __global__ void __launch_bounds__(128) p2air_generate_kernel(const u32 *inputs, 
     size_t off = 0;
     put16(off); off += 16;
     mds_light<F, AIR_W>(s);
-#pragma unroll 1
-    for (int r = 0; r < 4; r++) {
+    if constexpr (REG) {
+        // x^7 through the committed register x3 = x^3: the S-box output is x3^2 x
+        auto full = [&](const u32 *rc) {
 #pragma unroll
-        for (int i = 0; i < AIR_W; i++) s[i] = sbox<F>(fp_add<F>(s[i], k.beg[r * 16 + i]));
-        mds_light<F, AIR_W>(s);
-        put16(off); off += 16;
-    }
-    const unsigned rp = (unsigned)k.rounds_p;
+            for (int i = 0; i < AIR_W; i++) {
+                const u32 x = fp_add<F>(s[i], rc[i]), x3 = mont_mul<F>(mont_mul<F>(x, x), x);
+                tile[lane * 17 + i] = x3;
+                s[i] = mont_mul<F>(mont_mul<F>(x3, x3), x);
+            }
+            flush(16, off); off += 16;
+            mds_light<F, AIR_W>(s);
+            put16(off); off += 16;
+        };
 #pragma unroll 1
-    for (unsigned r = 0; r < rp; r++) {
-        s[0] = sbox<F>(fp_add<F>(s[0], k.part[r]));
-        tile[lane * (rp + 1) + r] = s[0];
-        air_internal_layer<F>(s);
-    }
-    flush(rp, off); off += rp;
+        for (int r = 0; r < 4; r++) full(k.beg + r * 16);
+        const unsigned rp = (unsigned)k.rounds_p;
 #pragma unroll 1
-    for (int r = 0; r < 4; r++) {
+        for (unsigned r0 = 0; r0 < rp; r0 += 16) {
+            const unsigned n = 2 * min(16u, rp - r0);
+#pragma unroll 1
+            for (unsigned r = r0; r < r0 + n / 2; r++) {
+                const u32 x = fp_add<F>(s[0], k.part[r]), x3 = mont_mul<F>(mont_mul<F>(x, x), x);
+                s[0] = mont_mul<F>(mont_mul<F>(x3, x3), x);
+                tile[lane * (n + 1) + 2 * (r - r0)] = x3;
+                tile[lane * (n + 1) + 2 * (r - r0) + 1] = s[0];
+                air_internal_layer<F>(s);
+            }
+            flush(n, off); off += n;
+        }
+#pragma unroll 1
+        for (int r = 0; r < 4; r++) full(k.end + r * 16);
+    } else {
+#pragma unroll 1
+        for (int r = 0; r < 4; r++) {
 #pragma unroll
-        for (int i = 0; i < AIR_W; i++) s[i] = sbox<F>(fp_add<F>(s[i], k.end[r * 16 + i]));
-        mds_light<F, AIR_W>(s);
-        put16(off); off += 16;
+            for (int i = 0; i < AIR_W; i++) s[i] = sbox<F>(fp_add<F>(s[i], k.beg[r * 16 + i]));
+            mds_light<F, AIR_W>(s);
+            put16(off); off += 16;
+        }
+        const unsigned rp = (unsigned)k.rounds_p;
+#pragma unroll 1
+        for (unsigned r = 0; r < rp; r++) {
+            s[0] = sbox<F>(fp_add<F>(s[0], k.part[r]));
+            tile[lane * (rp + 1) + r] = s[0];
+            air_internal_layer<F>(s);
+        }
+        flush(rp, off); off += rp;
+#pragma unroll 1
+        for (int r = 0; r < 4; r++) {
+#pragma unroll
+            for (int i = 0; i < AIR_W; i++) s[i] = sbox<F>(fp_add<F>(s[i], k.end[r * 16 + i]));
+            mds_light<F, AIR_W>(s);
+            put16(off); off += 16;
+        }
     }
 }
 
@@ -135,17 +180,74 @@ struct QuotArgs {
     size_t row0, rows;   // the block is memory rows [row0, row0 + rows) of the bit-reversed LDE
 };
 
+// The BabyBear instance (REG = 1): one permutation's constraints folded into acc, c its first column, apv its alpha-power row.
+// A permutation is 298 words = 1192 bytes, so every permutation starts 8-byte aligned: 8-byte loads throughout, and a partial
+// round's (register, post_sbox) pair is one load.  Each register check is folded before the post check that follows it, in the
+// constraint order of air.rs.
+template <int F>
+__device__ __forceinline__ void p2_fold_reg(const u32 *c, const uint4 *apv, const AirConsts &k, u64 (&acc)[4]) {
+    const uint2 *c2 = reinterpret_cast<const uint2 *>(c);
+    auto ld16 = [&](u32 (&dst)[AIR_W]) {
+#pragma unroll
+        for (int x = 0; x < 8; x++) { const uint2 w = __ldg(c2 + x); dst[2 * x] = w.x; dst[2 * x + 1] = w.y; }
+        c2 += 8;
+    };
+    auto cube = [](u32 x) { return mont_mul<F>(mont_mul<F>(x, x), x); };
+    u32 s[AIR_W];
+    ld16(s);
+    mds_light<F, AIR_W>(s);
+    auto full = [&](const u32 *rc) {
+        u32 w[AIR_W];
+        ld16(w);                                                    // the 16 registers
+#pragma unroll
+        for (int x = 0; x < AIR_W; x++) {
+            const u32 t = fp_add<F>(s[x], rc[x]);
+            air_qmac<F>(acc, fp_sub<F>(w[x], cube(t)), apv[x]);
+            s[x] = mont_mul<F>(mont_mul<F>(w[x], w[x]), t);
+        }
+        mds_light<F, AIR_W>(s);
+        ld16(w);                                                    // the 16 posts
+#pragma unroll
+        for (int x = 0; x < AIR_W; x++) { air_qmac<F>(acc, fp_sub<F>(s[x], w[x]), apv[AIR_W + x]); s[x] = w[x]; }
+        apv += 2 * AIR_W;
+    };
+#pragma unroll 1
+    for (int r = 0; r < 4; r++) full(k.beg + r * 16);
+#pragma unroll 1
+    for (int r = 0; r < k.rounds_p; r++) {
+        const uint2 w = __ldg(c2++);                                // (register, post_sbox)
+        const u32 t = fp_add<F>(s[0], k.part[r]);
+        air_qmac<F>(acc, fp_sub<F>(w.x, cube(t)), apv[0]);
+        air_qmac<F>(acc, fp_sub<F>(mont_mul<F>(mont_mul<F>(w.x, w.x), t), w.y), apv[1]);
+        apv += 2;
+        s[0] = w.y;
+        air_internal_layer<F>(s);
+    }
+#pragma unroll 1
+    for (int r = 0; r < 4; r++) full(k.end + r * 16);
+}
+
 // SHARDED = false: the whole LDE, one thread per (natural index i, permutation v), reads memory row bitrev(i), writes q[i].
 // SHARDED = true: one rank's row block of the row-sharded commit, one thread per (block row m, permutation v); memory row
 // row0 + m is natural index i = bitrev(row0 + m), so it takes 1/Z_H entry i & rate_mask and writes q[m].  The block is read in
 // place through the segment table (the chunk-major layout p3gpu_commit_sharded_dev leaves), never copied into a dense matrix.
+// The BabyBear instance is dense only (p2_fold_reg per permutation).
+// Threads per block: 128 for KoalaBear.  BabyBear's alpha table is 36 KB at vector_len 8; at 128 threads six blocks fill the SM's
+// shared memory and leave L1 almost nothing, while every lane's 8-byte loads walk its own 1192-byte permutation and need L1 to keep
+// the rest of each 32-byte sector.  512 threads share one table across 16 rows instead of 4.
+template <int F> constexpr int p2q_block() { return p2_reg<F>() ? 512 : 128; }
+
 template <int F, bool SHARDED>
-__global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, const __grid_constant__ AirConsts k) {
+__global__ void __launch_bounds__(p2q_block<F>()) p2air_quotient_kernel(const QuotArgs a, const __grid_constant__ AirConsts k) {
+    constexpr int REG = p2_reg<F>();
+    static_assert(!(REG && SHARDED), "the sharded quotient reads 16-byte units: KoalaBear only");
     // alpha powers, one padded row per permutation of the vector: constraint kk of permutation v (global index j = v * nc + kk,
-    // multiplied by alpha^(n_all - 1 - j)) sits at ap[v * (nc + 1) + kk].  The row stride of nc + 1 = 149 entries (596 words = 20
-    // mod 32 banks) spreads the 8 permutations a warp works on over disjoint banks; without the pad they collide 4 ways (ncu).
+    // multiplied by alpha^(n_all - 1 - j)) sits at ap[v * (nc + 1) + kk].  A quarter warp's 8 lanes are the 8 permutations of one
+    // row, reading the same kk; 16-byte entries at a row stride of nc + 1 put lane v on banks 4 (v (nc + 1) mod 8) + 0..3, disjoint
+    // for the 8 lanes exactly when nc + 1 is odd.  KoalaBear: nc + 1 = 149 (596 words = 20 mod 32); without the pad they collide 4
+    // ways (ncu).  BabyBear: nc + 1 = 283 (1132 words = 12 mod 32), odd as well, so the same formula holds.
     extern __shared__ uint4 ap[];
-    const int nc = 128 + k.rounds_p, n_all = nc * a.vec_len;
+    const int nc = REG ? p2_constraints(REG, k.rounds_p) : 128 + k.rounds_p, n_all = nc * a.vec_len;
     for (int t = threadIdx.x; t < n_all; t += blockDim.x) {
         const int j = n_all - 1 - t;
         ap[(j / nc) * (nc + 1) + (j % nc)] = __ldg(reinterpret_cast<const uint4 *>(a.apow) + t);
@@ -160,7 +262,12 @@ __global__ void __launch_bounds__(128) p2air_quotient_kernel(const QuotArgs a, c
     const int v = (int)(t % lanes);
     const bool live = SHARDED ? i < a.rows : i < ((size_t)1 << a.log_h);
     u64 acc[4] = {0, 0, 0, 0};
-    if (live) {
+    if constexpr (REG) {
+        if (live) {
+            const size_t m = (size_t)(__brevll((unsigned long long)i) >> (64 - a.log_h));
+            p2_fold_reg<F>(a.lde + (m * lanes + v) * p2_cols(REG, k.rounds_p), ap + v * (nc + 1), k, acc);
+        }
+    } else if (live) {
         const size_t cols = 144 + (size_t)k.rounds_p;
         const size_t m = SHARDED ? i : (size_t)(__brevll((unsigned long long)i) >> (64 - a.log_h));
         const u32 *c = a.lde + (m * lanes + v) * cols;
@@ -269,26 +376,46 @@ template <int F> __global__ void ef_powers_kernel(u32 *pw, size_t n, const Ef4<F
 }
 
 static int32_t air_consts(p3gpu_ctx *ctx, int field, const AirConsts **out) {
-    P3_CHECK(field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Poseidon2 AIR: only the KoalaBear instance (degree-3 S-box, no S-box registers) is built");
-    P3_CHECK(ctx->air_set, P3GPU_ESTATE, "Poseidon2 AIR round constants not set (p3gpu_p2air_set_constants)");
+    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Poseidon2 AIR: unsupported field %d", field);
+    P3_CHECK(ctx->air_field >= 0, P3GPU_ESTATE, "Poseidon2 AIR round constants not set (p3gpu_p2air_set_constants)");
+    P3_CHECK(ctx->air_field == field, P3GPU_ESTATE, "Poseidon2 AIR round constants were set for field %d, not %d", ctx->air_field, field);
     *out = reinterpret_cast<const AirConsts *>(ctx->air_consts);
     return P3GPU_OK;
 }
 
+// The row-sharded entry points read the trace in 16-byte units of 4-column segments; a BabyBear permutation is 298 columns, so
+// every odd one starts in the middle of a unit.
+int32_t air_sharded_field(int field) {
+    P3_CHECK(field != BABY_BEAR, P3GPU_EUNSUPPORTED,
+             "Poseidon2 AIR (BabyBear): no sharded prove: its 298-column permutations do not start on the 4-column units the sharded "
+             "kernels read");
+    return P3GPU_OK;
+}
+
+size_t air_columns(int field, int rounds_p) {
+    if (field != BABY_BEAR && field != KOALA_BEAR) return 0;
+    return p2_cols(field == BABY_BEAR ? p2_reg<BABY_BEAR>() : p2_reg<KOALA_BEAR>(), rounds_p);
+}
+
 int32_t air_set_constants(p3gpu_ctx *ctx, int field, const u32 *beg, const u32 *part, int rounds_p, const u32 *end) {
-    P3_CHECK(field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Poseidon2 AIR: only the KoalaBear instance (degree-3 S-box, no S-box registers) is built");
-    P3_CHECK(rounds_p >= 4 && rounds_p <= 32 && rounds_p % 4 == 0, P3GPU_EINVAL, "rounds_p %d must be a multiple of 4 in 4..32", rounds_p);
+    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Poseidon2 AIR: unsupported field %d", field);
+    // KoalaBear's quotient reads partial rounds four at a time with 16-byte loads; BabyBear's reads (register, post_sbox) pairs
+    if (field == KOALA_BEAR)
+        P3_CHECK(rounds_p >= 4 && rounds_p <= 32 && rounds_p % 4 == 0, P3GPU_EINVAL, "rounds_p %d must be a multiple of 4 in 4..32", rounds_p);
+    else
+        P3_CHECK(rounds_p >= 1 && rounds_p <= 32, P3GPU_EINVAL, "Poseidon2 AIR (BabyBear): rounds_p %d outside 1..32", rounds_p);
     static_assert(sizeof(AirConsts) <= sizeof(ctx->air_consts), "context storage for the AIR constants");
+    const u32 P = field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
     AirConsts k;
     memset(&k, 0, sizeof k);
     for (int i = 0; i < 64; i++) {
-        P3_CHECK(beg[i] < Fp<KOALA_BEAR>::P && end[i] < Fp<KOALA_BEAR>::P, P3GPU_EINVAL, "round constant not in canonical Montgomery range");
+        P3_CHECK(beg[i] < P && end[i] < P, P3GPU_EINVAL, "round constant not in canonical Montgomery range");
         k.beg[i] = beg[i]; k.end[i] = end[i];
     }
-    for (int i = 0; i < rounds_p; i++) { P3_CHECK(part[i] < Fp<KOALA_BEAR>::P, P3GPU_EINVAL, "round constant not in canonical Montgomery range"); k.part[i] = part[i]; }
+    for (int i = 0; i < rounds_p; i++) { P3_CHECK(part[i] < P, P3GPU_EINVAL, "round constant not in canonical Montgomery range"); k.part[i] = part[i]; }
     k.rounds_p = rounds_p;
     memcpy(ctx->air_consts, &k, sizeof k);
-    ctx->air_set = 1;
+    ctx->air_field = field;
     return P3GPU_OK;
 }
 
@@ -296,7 +423,9 @@ int32_t air_generate_trace(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_
     const AirConsts *k;
     P3_TRY(air_consts(ctx, field, &k));
     if (n_perms == 0) return P3GPU_OK;
-    p2air_generate_kernel<KOALA_BEAR, false><<<(unsigned)((n_perms + 127) / 128), 128, 0, ctx->stream>>>(d_inputs, n_perms, d_trace, *k, GenWindow{});
+    const unsigned grid = (unsigned)((n_perms + 127) / 128);
+    if (field == BABY_BEAR) p2air_generate_kernel<BABY_BEAR, false><<<grid, 128, 0, ctx->stream>>>(d_inputs, n_perms, d_trace, *k, GenWindow{});
+    else p2air_generate_kernel<KOALA_BEAR, false><<<grid, 128, 0, ctx->stream>>>(d_inputs, n_perms, d_trace, *k, GenWindow{});
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
@@ -345,16 +474,21 @@ int32_t shard_col_segments(unsigned world, const size_t *col_starts, size_t rows
 }
 
 // alpha powers + 1/Z_H tables into scratch2, then one quotient launch (the whole LDE, or one row block with its segment table)
-template <bool SHARDED>
+// (F, SHARDED) = (BABY_BEAR, true) is refused before this: the C ABI calls air_sharded_field first.
+template <int F, bool SHARDED>
 static int32_t quotient_launch(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q,
                                const std::vector<size_t> *segs, size_t row0, size_t rows) {
-    constexpr int F = KOALA_BEAR;
+    constexpr int REG = p2_reg<F>();
     const AirConsts *k;
     P3_TRY(air_consts(ctx, field, &k));
     P3_CHECK(vec_len >= 1 && vec_len <= 32 && (vec_len & (vec_len - 1)) == 0, P3GPU_EINVAL, "vector length %d must be a power of two <= 32", vec_len);
     P3_CHECK(log_h >= log_n && log_h <= Fp<F>::TWO_ADICITY && log_h - log_n <= 8, P3GPU_EINVAL, "bad domain sizes 2^%u / 2^%u", log_h, log_n);
-    P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 16 == 0 && reinterpret_cast<uintptr_t>(d_q) % 16 == 0, P3GPU_EINVAL, "quotient: buffers must be 16-byte aligned");
-    const int nc = 128 + k->rounds_p, n_all = nc * vec_len;
+    if constexpr (REG)                                              // the kernel's 8-byte LDE loads, 16-byte quotient stores
+        P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 8 == 0 && reinterpret_cast<uintptr_t>(d_q) % 16 == 0, P3GPU_EINVAL,
+                 "quotient: the LDE must be 8-byte aligned, the quotient 16-byte aligned");
+    else
+        P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 16 == 0 && reinterpret_cast<uintptr_t>(d_q) % 16 == 0, P3GPU_EINVAL, "quotient: buffers must be 16-byte aligned");
+    const int nc = p2_constraints(REG, k->rounds_p), n_all = nc * vec_len;
     const unsigned rate_bits = log_h - log_n;
     const size_t nz = (size_t)1 << rate_bits;
     const size_t n_segs = SHARDED ? segs->size() / 3 : 0;
@@ -385,14 +519,16 @@ static int32_t quotient_launch(p3gpu_ctx *ctx, int field, int vec_len, const u32
     const size_t smem = (size_t)vec_len * (nc + 1) * 16 + n_segs * sizeof(QSeg);
     auto kern = p2air_quotient_kernel<F, SHARDED>;
     if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<(unsigned)((threads + 127) / 128), 128, smem, ctx->stream>>>(qa, *k);
+    constexpr int block = p2q_block<F>();
+    kern<<<(unsigned)((threads + block - 1) / block), block, smem, ctx->stream>>>(qa, *k);
     ctx->launches += 2;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
 
 int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    return quotient_launch<false>(ctx, field, vec_len, d_lde, log_h, log_n, alpha, d_q, nullptr, 0, 0);
+    if (field == BABY_BEAR) return quotient_launch<BABY_BEAR, false>(ctx, field, vec_len, d_lde, log_h, log_n, alpha, d_q, nullptr, 0, 0);
+    return quotient_launch<KOALA_BEAR, false>(ctx, field, vec_len, d_lde, log_h, log_n, alpha, d_q, nullptr, 0, 0);
 }
 
 int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned world, unsigned rank, const u32 *d_block, const size_t *col_starts,
@@ -401,7 +537,7 @@ int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned wo
     P3_CHECK(world >= 1 && rank < world && rows * world == H, P3GPU_EINVAL, "LDE height 2^%u does not split over %u ranks", log_h, world);
     std::vector<size_t> segs;
     P3_TRY(shard_col_segments(world, col_starts, rows, segs));
-    return quotient_launch<true>(ctx, field, vec_len, d_block, log_h, log_n, alpha, d_q, &segs, (size_t)rank * rows, rows);
+    return quotient_launch<KOALA_BEAR, true>(ctx, field, vec_len, d_block, log_h, log_n, alpha, d_q, &segs, (size_t)rank * rows, rows);
 }
 
 }  // namespace p3

@@ -480,6 +480,7 @@ int32_t p3gpu_p2air_set_constants(p3gpu_ctx *ctx, int field, const uint32_t *beg
     return air_set_constants(ctx, field, beginning_full, partial, rounds_p, ending_full);
 }
 size_t p3gpu_p2air_columns(int rounds_p) { return 144 + (size_t)rounds_p; }
+size_t p3gpu_p2air_field_columns(int field, int rounds_p) { return air_columns(field, rounds_p); }
 int32_t p3gpu_p2air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_perms, uint32_t *d_trace) {
     P3_ENTER(ctx);
     P3_CHECK(d_inputs && d_trace, P3GPU_EINVAL, "null argument");
@@ -494,6 +495,7 @@ int32_t p3gpu_p2air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, cons
 int32_t p3gpu_p2air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms, size_t col0,
                                             size_t col1, uint32_t *d_out) {
     P3_ENTER(ctx);
+    P3_TRY(air_sharded_field(field));
     P3_CHECK(d_inputs && (d_out || col0 == col1), P3GPU_EINVAL, "null argument");
     return air_generate_trace_cols(ctx, field, vector_len, d_inputs, n_perms, col0, col1, d_out);
 }
@@ -753,6 +755,7 @@ int32_t p3gpu_peer_exchange_dev(p3gpu_ctx *ctx, const p3gpu_peer_group *grp, uin
 int32_t p3gpu_p2air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
                                          unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient_slice) {
     P3_ENTER(ctx);
+    P3_TRY(air_sharded_field(field));
     P3_TRY(check_group(grp, true));
     P3_CHECK(col_starts && alpha && d_quotient_slice, P3GPU_EINVAL, "null argument");
     return air_quotient_sharded(ctx, field, vector_len, grp->world, grp->rank, grp->rows[grp->rank], col_starts, log_lde_height, log_trace_height,

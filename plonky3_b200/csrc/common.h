@@ -102,7 +102,7 @@ struct p3gpu_ctx {
     p3::Poseidon2Consts p2_host[2][2];
     p3::Poseidon2Consts *p2_dev = nullptr;  // 4 entries
     alignas(8) unsigned char air_consts[1024];   // Poseidon2 AIR round constants (air.cu: AirConsts)
-    int air_set = 0;
+    int air_field = -1;                          // the field they were set for (-1: not set)
     // Poseidon1 AIR constants (poseidon1_air.cu): a device buffer of this context, written by p3gpu_p1air_set_constants on the
     // context's stream, freed at destroy; p1_field is the field they were set for (-1: not set)
     uint32_t *p1_consts = nullptr;
@@ -149,9 +149,11 @@ int32_t peer_barrier(p3gpu_ctx *ctx, unsigned world, unsigned rank, void *const 
 int32_t peer_allgather(p3gpu_ctx *ctx, unsigned world, unsigned rank, void *const *tables, const u32 *d_src, size_t words);
 
 // air.cu: Poseidon2 AIR trace generation / quotient (SURVEY 8f ranks 2-3)
+size_t air_columns(int field, int rounds_p);            // 0 for an unknown field
 int32_t air_set_constants(p3gpu_ctx *ctx, int field, const u32 *beg, const u32 *part, int rounds_p, const u32 *end);
 int32_t air_generate_trace(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_perms, u32 *d_trace);
 int32_t air_quotient(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_lde, unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q);
+int32_t air_sharded_field(int field);                   // P3GPU_EUNSUPPORTED for BabyBear: the sharded entry points are KoalaBear-only
 int32_t air_generate_trace_cols(p3gpu_ctx *ctx, int field, int vec_len, const u32 *d_inputs, size_t n_perms, size_t col0, size_t col1, u32 *d_out);
 int32_t shard_col_segments(unsigned world, const size_t *col_starts, size_t rows, std::vector<size_t> &segs);   // (c0, c1, offset) triples
 int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned world, unsigned rank, const u32 *d_block, const size_t *col_starts,

@@ -508,10 +508,14 @@ def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public
     """uni_stark.prove of the Poseidon2 AIR with the trace sharded by column block over the ranks of `grp` (rank g holds columns
     [col_starts[g], col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  Every rank returns the same Proof, byte for
     byte the one `uni_stark.prove` writes for the whole trace on one GPU; its timings_ms are each span's maximum over the ranks."""
+    from .field import KoalaBear
     from .uni_stark import VectorizedPoseidon2Air, get_log_num_quotient_chunks, prove
     pcs = config.pcs
     assert grp.gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
     assert isinstance(air, VectorizedPoseidon2Air), "the sharded quotient kernel evaluates the Poseidon2 AIR only"
+    if air.field.id != KoalaBear.id:
+        # the sharded quotient kernel reads 16-byte units of 4-column segments; BabyBear's 298-column permutations start mid-unit
+        raise ValueError(f"prove_sharded: the Poseidon2 AIR over {air.field.name} has no sharded prove (KoalaBear only)")
     assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
     assert get_log_num_quotient_chunks(air) == pcs.fri.log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
     proof = prove(config, air, trace_block, shard=ShardedTrace(grp, col_starts))

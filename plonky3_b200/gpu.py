@@ -268,7 +268,7 @@ class Gpu:
         c = np.ascontiguousarray(ending_full, dtype=np.uint32).ravel()
         assert a.size == 64 and c.size == 64
         check(self.L.p3gpu_p2air_set_constants(self.h, field, a.ctypes.data, b.ctypes.data, b.size, c.ctypes.data))
-        self._air_cols = int(self.L.p3gpu_p2air_columns(b.size))
+        self._air_cols = int(self.L.p3gpu_p2air_field_columns(field, b.size))
 
     def p2air_generate_trace(self, field, inputs_dev, vector_len=8):
         """(n_perms, 16) CUDA tensor -> vectorised trace (n_perms / vector_len, vector_len * columns)."""

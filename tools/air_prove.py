@@ -4,12 +4,15 @@ cap height 3.  One configuration per process:
     python tools/air_prove.py --air keccak --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air blake3 --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air poseidon1 --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
+    python tools/air_prove.py --air poseidon2 --field baby-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
 
   keccak   `-o keccak-f-permutations -l 20`: 43,690 hashes, a 2^20 x 2633 trace (the trace and its LDE take 33 GB together)
   blake3   `-o blake-3-permutations` at 2^18 compressions, a 2^18 x 9168 trace (29 GB with its LDE; the reference's `-l 20`
            shape, a 38.5 GB trace with a 77 GB LDE, does not fit on one 80 GB card)
   poseidon1  `-o poseidon-1-permutations -l 20`: 8 << log_rows permutations, 8 per row, the constants of
            tests/golden/poseidon1_constants.json; a 2^20 x 1312 trace (KoalaBear, 5.5 GB) or 2^20 x 2384 (BabyBear, 10 GB)
+  poseidon2  `-o poseidon-2-permutations -l 20`: 8 << log_rows permutations, 8 per row, the example's RoundConstants::from_rng on
+           SmallRng(1) (13 partial rounds for BabyBear, 20 for KoalaBear); a 2^20 x 2384 trace (BabyBear, 10 GB) or 2^20 x 1312
 
 Times trace generation and the quotient kernel alone (CUDA events, median of --kernel-reps launches after a warm-up), and `prove`
 span by span (median of --reps proofs after one warm-up); then verifies the last proof.  Prints one JSON object with the card's name
@@ -30,7 +33,7 @@ sys.path.insert(0, str(ROOT))
 import numpy as np
 import torch
 
-from plonky3_b200 import blake3_air, keccak_air, poseidon1_air
+from plonky3_b200 import blake3_air, keccak_air, poseidon1_air, poseidon2_air
 from plonky3_b200.dft import Radix2DitParallel
 from plonky3_b200.field import BabyBear, KoalaBear
 from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
@@ -48,11 +51,22 @@ def _poseidon1(f, gpu=None):
     return poseidon1_air.VectorizedPoseidon1Air(f, poseidon1_air.Poseidon1Constants.from_fixture(f, fx).to_optimized(), gpu)
 
 
-def _poseidon1_inputs(f, n):
+def _smallrng_inputs(f, n):
     """poseidon1_air.random_inputs(f, n), drawn by the C oracle of the same SmallRng: the scalar restatement takes minutes at
     2^23 permutations."""
     from oracle import p3_oracle as O
     return O.SmallRng(1).field(f.id, 16 * n).reshape(n, 16)
+
+
+def _poseidon2(f, gpu=None):
+    """VectorizedPoseidon2Air with the example binary's constants: RoundConstants::from_rng(SmallRng::seed_from_u64(1)), drawn by
+    the C oracle of the same SmallRng."""
+    from oracle import p3_oracle as O
+    rp = 13 if f is BabyBear else 20
+    c = O.air_from_rng(f.id, O.SmallRng(1), rp)
+    consts = poseidon2_air.RoundConstants(np.array(c.beg, dtype=np.uint32).reshape(4, 16), np.array(c.part, dtype=np.uint32)[:rp],
+                                          np.array(c.end, dtype=np.uint32).reshape(4, 16))
+    return poseidon2_air.VectorizedPoseidon2Air(f, consts, gpu)
 
 
 # --air: (AIR constructor (field, gpu), default --log-rows, hashes of a 2^log_rows trace, inputs (field, n), input dtype)
@@ -61,7 +75,8 @@ AIRS = {
                lambda f, n: keccak_air.random_inputs(n), np.int64),
     "blake3": (lambda f, gpu=None: blake3_air.Blake3Air(f, gpu), 18, lambda log_rows: 1 << log_rows,           # one compression per row
                lambda f, n: blake3_air.random_inputs(n), np.int32),
-    "poseidon1": (_poseidon1, 20, lambda log_rows: 8 << log_rows, _poseidon1_inputs, np.int32),               # 8 permutations per row
+    "poseidon1": (_poseidon1, 20, lambda log_rows: 8 << log_rows, _smallrng_inputs, np.int32),               # 8 permutations per row
+    "poseidon2": (_poseidon2, 20, lambda log_rows: 8 << log_rows, _smallrng_inputs, np.int32),               # the same SmallRng(1) draw
 }
 
 
@@ -85,7 +100,7 @@ def main():
     ap.add_argument("--air", choices=sorted(AIRS), required=True)
     ap.add_argument("--field", choices=["koala-bear", "baby-bear"], default="koala-bear")
     ap.add_argument("--config", choices=["keccak", "poseidon2"], default="keccak")
-    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1, 18 for blake3)")
+    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1/2, 18 for blake3)")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--kernel-reps", type=int, default=10)
     a = ap.parse_args()

@@ -42,6 +42,7 @@ pub const P3GPU_AIR_PREPROCESSED_NEXT: u32 = 17;
 pub const P3GPU_AIR_PERIODIC: u32 = 18;
 pub const P3GPU_KECCAK_AIR_COLS: usize = 2633;
 pub const P3GPU_BLAKE3_AIR_COLS: usize = 9168;
+pub const P3GPU_SHA256_AIR_COLS: usize = 7728;
 
 /// `p3gpu_air_layout`: what a constraint program's leaves may read.
 #[repr(C)]
@@ -181,6 +182,11 @@ unsafe extern "C" {
     // Blake3 AIR (blake3-air): trace generation and quotient values, P3GPU_BLAKE3_AIR_COLS columns
     pub fn p3gpu_blake3_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_blake3_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
+                                         alpha: *const u32, d_quotient: *mut u32) -> i32;
+
+    // SHA-256 AIR (sha256-air): trace generation and quotient values, P3GPU_SHA256_AIR_COLS columns
+    pub fn p3gpu_sha256_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, d_trace: *mut u32) -> i32;
+    pub fn p3gpu_sha256_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
                                          alpha: *const u32, d_quotient: *mut u32) -> i32;
 
     // Poseidon1 AIR (poseidon1-air, width 16): per-context constants (Poseidon1Constants::to_optimized's output, Montgomery words),

@@ -267,6 +267,20 @@ int32_t p3gpu_blake3_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uin
 int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
                                       const uint32_t alpha[4], uint32_t *d_quotient);
 
+/* ---- SHA-256 AIR (sha256-air/src), BabyBear and KoalaBear ------------------------------------------------------------------
+ * One SHA-256 compression per row, rows independent (no next-row reads, no selectors, no public values), P3GPU_SHA256_AIR_COLS
+ * columns (columns.rs Sha256Cols); 8096 constraints of degree 3, so two quotient chunks (log_blowup >= 1). */
+#define P3GPU_SHA256_AIR_COLS 7728
+/* generate_trace_rows (sha256-air/src/generation.rs): d_inputs n_hashes x 24 u32 (the 16-word block, then the 8-word chaining
+ * state) -> d_trace, n_hashes x P3GPU_SHA256_AIR_COLS Montgomery words.  P3GPU_EINVAL before any launch: a NULL or
+ * non-4-byte-aligned pointer, n_hashes 0, not a power of two or above 2^32; P3GPU_EUNSUPPORTED: a field other than BabyBear /
+ * KoalaBear. */
+int32_t p3gpu_sha256_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, uint32_t *d_trace);
+/* quotient_values of the SHA-256 AIR, with the contract of p3gpu_keccak_air_quotient_dev (d_lde: 2^log_lde_height rows x
+ * P3GPU_SHA256_AIR_COLS). */
+int32_t p3gpu_sha256_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient);
+
 /* ---- Poseidon1 AIR: the AIR of prove_prime_field_31 -o poseidon-1-permutations (poseidon1-air/src), width 16 -------------------
  * VectorizedPoseidon1Air<F, 16, SBOX_DEGREE, SBOX_REGISTERS, 4, rounds_p, vector_len>: BabyBear x^7 with one S-box register,
  * KoalaBear x^3 without.  No next-row reads, no selectors; constraints of degree 3, so two quotient chunks (log_blowup >= 1).

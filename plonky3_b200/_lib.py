@@ -16,6 +16,7 @@ DFT, IDFT, COSET_DFT, COSET_IDFT = 0, 1, 2, 3
 HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_KECCAK = 0, 1, 2
 KECCAK_AIR_COLS = 2633                       # P3GPU_KECCAK_AIR_COLS
 BLAKE3_AIR_COLS = 9168                       # P3GPU_BLAKE3_AIR_COLS
+SHA256_AIR_COLS = 7728                       # P3GPU_SHA256_AIR_COLS
 
 EXPORTS = [
     "p3gpu_ctx_create", "p3gpu_ctx_destroy", "p3gpu_ctx_set_stream", "p3gpu_ctx_use_own_stream", "p3gpu_ctx_sync", "p3gpu_last_error",
@@ -37,6 +38,7 @@ EXPORTS = [
     "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
     "p3gpu_keccak_air_generate_trace_dev", "p3gpu_keccak_air_quotient_dev",
     "p3gpu_blake3_air_generate_trace_dev", "p3gpu_blake3_air_quotient_dev",
+    "p3gpu_sha256_air_generate_trace_dev", "p3gpu_sha256_air_quotient_dev",
     "p3gpu_p1air_set_constants", "p3gpu_p1air_columns", "p3gpu_p1air_generate_trace_dev", "p3gpu_p1air_quotient_dev",
 ]
 
@@ -144,6 +146,8 @@ def load():
         "p3gpu_keccak_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
         "p3gpu_blake3_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
         "p3gpu_blake3_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
+        "p3gpu_sha256_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),
+        "p3gpu_sha256_air_quotient_dev": (i32, [vp, ci, vp, cu, cu, vp, vp]),
         "p3gpu_p1air_set_constants": (i32, [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci]),
         "p3gpu_p1air_columns": (sz, [ci, ci]),
         "p3gpu_p1air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),

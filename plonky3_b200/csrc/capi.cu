@@ -530,6 +530,21 @@ int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t 
     return blake3_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
 }
 
+// ---- SHA-256 AIR: trace generation + quotient (sha256_air.cu) -----------------------------------------
+int32_t p3gpu_sha256_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, uint32_t *d_trace) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && d_trace, P3GPU_EINVAL, "null argument");
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 4 == 0 && reinterpret_cast<uintptr_t>(d_trace) % 4 == 0, P3GPU_EINVAL,
+             "SHA-256 AIR trace: misaligned buffer");
+    return sha256_air_generate(ctx, field, d_inputs, n_hashes, d_trace);
+}
+int32_t p3gpu_sha256_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
+                                      const uint32_t alpha[4], uint32_t *d_quotient) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
+    return sha256_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+
 // ---- Poseidon1 AIR: constants, trace generation + quotient (poseidon1_air.cu) -------------------------------
 int32_t p3gpu_p1air_set_constants(p3gpu_ctx *ctx, int field, const uint32_t *initial_full, const uint32_t *terminal_full,
                                   const uint32_t *mds_circ_col, const uint32_t *first_round_constants, const uint32_t *m_i,

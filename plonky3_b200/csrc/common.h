@@ -186,6 +186,10 @@ int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigne
 int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
 int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
 
+// sha256_air.cu: SHA-256 AIR trace generation / quotient
+int32_t sha256_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
+int32_t sha256_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+
 // poseidon1_air.cu: Poseidon1 AIR constants (per context), trace generation / quotient
 size_t p1air_columns(int field, int rounds_p);          // 0 for an unknown field
 int32_t p1air_set_constants(p3gpu_ctx *ctx, int field, const u32 *initial_full, const u32 *terminal_full, const u32 *mds_circ_col,

@@ -329,6 +329,21 @@ class Gpu:
         """`_air_quotient_2n` of the Blake3 AIR (9168 columns)."""
         return self._air_quotient_2n(self.L.p3gpu_blake3_air_quotient_dev, _lib.BLAKE3_AIR_COLS, field, lde_dev, log_trace_height, alpha)
 
+    # ------------------------------------------------------------------ SHA-256 AIR
+    def sha256_air_generate_trace(self, field, inputs_dev):
+        """(n, 24) contiguous CUDA int32 tensor of u32 words (the 16-word block, the 8-word chaining state), n a power of two -> the
+        (n, 7728) trace."""
+        import torch
+        x = self._air_inputs(inputs_dev, torch.int32, 24); self._use_torch_stream()
+        n = int(x.shape[0])
+        out = self._empty((n, _lib.SHA256_AIR_COLS))
+        check(self.L.p3gpu_sha256_air_generate_trace_dev(self.h, field, x.data_ptr(), n, out.data_ptr()))
+        return out
+
+    def sha256_air_quotient(self, field, lde_dev, log_trace_height, alpha):
+        """`_air_quotient_2n` of the SHA-256 AIR (7728 columns)."""
+        return self._air_quotient_2n(self.L.p3gpu_sha256_air_quotient_dev, _lib.SHA256_AIR_COLS, field, lde_dev, log_trace_height, alpha)
+
     # ------------------------------------------------------------------ Poseidon1 AIR
     def p1air_set_constants(self, field, initial_full, terminal_full, mds_circ_col, first_round_constants, m_i, partial_rc,
                             sparse_first_row, v, rounds_p):

@@ -7,7 +7,8 @@ quotient chunks up to the blowup, preprocessed columns committed once by `setup_
 its own quotient on the device: a plain SymbolicAir through the constraint-program kernel (p3gpu_air_quotient_dev /
 p3gpu_air_quotient_layout_dev); poseidon2_air.VectorizedPoseidon2Air, the config-5 benchmark's AIR (`prove_prime_field_31 --field
 koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`),
-keccak_air.KeccakAir, blake3_air.Blake3Air and poseidon1_air.VectorizedPoseidon1Air through their hand-written kernels.  With
+keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air and poseidon1_air.VectorizedPoseidon1Air through their
+hand-written kernels.  With
 `shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns split over several GPUs, the
 shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
 
@@ -145,8 +146,8 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
 def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
     """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
     call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air,
-    keccak_air.KeccakAir, blake3_air.Blake3Air or poseidon1_air.VectorizedPoseidon1Air.  `trace`: device (CUDA int32) matrix of
-    height 2^n.  `public_values`: canonical integers.
+    keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air or poseidon1_air.VectorizedPoseidon1Air.  `trace`: device
+    (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.
 
     `preprocessed`: setup_preprocessed's prover data, required iff the AIR has preprocessed columns; its commitment is observed
     after the trace's, and the preprocessed trace is opened last (at zeta, and zeta * omega unless preprocessed_next_row_columns() is

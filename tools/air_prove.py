@@ -3,12 +3,14 @@ cap height 3.  One configuration per process:
 
     python tools/air_prove.py --air keccak --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air blake3 --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
+    python tools/air_prove.py --air sha256 --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air poseidon1 --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air poseidon2 --field baby-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
 
   keccak   `-o keccak-f-permutations -l 20`: 43,690 hashes, a 2^20 x 2633 trace (the trace and its LDE take 33 GB together)
   blake3   `-o blake-3-permutations` at 2^18 compressions, a 2^18 x 9168 trace (29 GB with its LDE; the reference's `-l 20`
            shape, a 38.5 GB trace with a 77 GB LDE, does not fit on one 80 GB card)
+  sha256   sha256-air's Sha256Air at 2^18 compressions, a 2^18 x 7728 trace (8.1 GB; its LDE 16.2 GB)
   poseidon1  `-o poseidon-1-permutations -l 20`: 8 << log_rows permutations, 8 per row, the constants of
            tests/golden/poseidon1_constants.json; a 2^20 x 1312 trace (KoalaBear, 5.5 GB) or 2^20 x 2384 (BabyBear, 10 GB)
   poseidon2  `-o poseidon-2-permutations -l 20`: 8 << log_rows permutations, 8 per row, the example's RoundConstants::from_rng on
@@ -33,7 +35,7 @@ sys.path.insert(0, str(ROOT))
 import numpy as np
 import torch
 
-from plonky3_b200 import blake3_air, keccak_air, poseidon1_air, poseidon2_air
+from plonky3_b200 import blake3_air, keccak_air, poseidon1_air, poseidon2_air, sha256_air
 from plonky3_b200.dft import Radix2DitParallel
 from plonky3_b200.field import BabyBear, KoalaBear
 from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
@@ -75,6 +77,8 @@ AIRS = {
                lambda f, n: keccak_air.random_inputs(n), np.int64),
     "blake3": (lambda f, gpu=None: blake3_air.Blake3Air(f, gpu), 18, lambda log_rows: 1 << log_rows,           # one compression per row
                lambda f, n: blake3_air.random_inputs(n), np.int32),
+    "sha256": (lambda f, gpu=None: sha256_air.Sha256Air(f, gpu), 18, lambda log_rows: 1 << log_rows,         # one compression per row
+               lambda f, n: sha256_air.random_inputs(n), np.int32),
     "poseidon1": (_poseidon1, 20, lambda log_rows: 8 << log_rows, _smallrng_inputs, np.int32),               # 8 permutations per row
     "poseidon2": (_poseidon2, 20, lambda log_rows: 8 << log_rows, _smallrng_inputs, np.int32),               # the same SmallRng(1) draw
 }
@@ -100,7 +104,7 @@ def main():
     ap.add_argument("--air", choices=sorted(AIRS), required=True)
     ap.add_argument("--field", choices=["koala-bear", "baby-bear"], default="koala-bear")
     ap.add_argument("--config", choices=["keccak", "poseidon2"], default="keccak")
-    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1/2, 18 for blake3)")
+    ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1/2, 18 for blake3 and sha256)")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--kernel-reps", type=int, default=10)
     a = ap.parse_args()

@@ -147,6 +147,34 @@ __device__ __forceinline__ void radix_step(u32 *data, const uint2 *tws, int r, i
     __syncthreads();
 }
 
+__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+__device__ __forceinline__ void cp_async8(void *smem, const void *gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+__device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
+
+// The twiddles of a tile of 2^r rows of the pass over layers [l0, l0 + r), row tile T (the top l0 row bits): layer l0 + lam uses the
+// 2^lam contiguous heap entries from Z[2^(l0+lam) + T*2^lam], staged in shared memory as tws[2^lam + q] = Z[2^(l0+lam) + T*2^lam + q],
+// so that tws is the heap of the tile's own r-layer network (tws[0] unused).  Every thread of the CTA copies entries
+// threadIdx.x + 1, + THREADS, ... < 2^r; ASYNC: as cp.async copies in the caller's current group.  (load_tile_twiddles: the same
+// table as bulk copies.)  l0 is taken by reference so that a kernel parameter passed there is read where it is used, as a
+// constant-bank operand, not held in a register across the copy loop (whose asm statements keep the compiler from hoisting it).
+template <int THREADS, bool ASYNC>
+__device__ __forceinline__ void stage_tile_twiddles(uint2 *tws, const uint2 *tw, const int &l0, u32 T, u32 R) {
+    for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {
+        const int lam = 31 - __clz(k);
+        const uint2 *src = tw + ((size_t)1 << (l0 + lam)) + ((size_t)T << lam) + (k - (1u << lam));
+        if constexpr (ASYNC) cp_async8(tws + k, src);
+        else tws[k] = *src;
+    }
+}
+
 template <int F, int LOG_CT, int THREADS, bool VEC>
 __global__ void __launch_bounds__(THREADS) ntt_pass_kernel(const PassArgs a) {
     constexpr u32 CT = 1u << LOG_CT;
@@ -168,12 +196,7 @@ __global__ void __launch_bounds__(THREADS) ntt_pass_kernel(const PassArgs a) {
     const u32 ibase = (a.l0 == 0 ? 0u : (T << (a.log_n - a.l0))) | L;
     const int brsh = 32 - a.log_n;
 
-    // stage this tile's R-1 twiddles: tws[2^lam + ql] = Z[2^(l0+lam) + T*2^lam + ql]
-    for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {
-        const int lam = 31 - __clz(k);
-        const u32 ql = k - (1u << lam);
-        tws[k] = tw[((size_t)1 << (a.l0 + lam)) + ((size_t)T << lam) + ql];
-    }
+    stage_tile_twiddles<THREADS, false>(tws, tw, a.l0, T, R);
     // gather the tile
     if (VEC) {
         constexpr u32 CV = CT >= 4 ? CT / 4 : 1;
@@ -266,18 +289,6 @@ __device__ __forceinline__ void reg_network(u32 (&x)[1 << Q], const uint2 *tws, 
     reg_layer<F, Q, 0>(x, tws, node);
 }
 
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async8(void *smem, const void *gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async4(void *smem, const void *gmem) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
 // Tile stores through the tensor copy engine: the tile's writers make their shared-memory writes visible to the async proxy,
 // meet at a barrier, and one thread stores the whole tile with ONE 5-D tensor copy (box = the padded tile layout: see
 // make_pass_tensor_map).  The copy drains to HBM while the SM computes; a buffer is rewritten only after
@@ -327,9 +338,9 @@ __device__ __forceinline__ void tma_load_tile(const CUtensorMap *map, void *smem
                  ::"r"((u32)__cvta_generic_to_shared(smem)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(0), "r"(0), "r"(c3), "r"(c4),
                    "r"(bar) : "memory");
 }
-// a tile's twiddles tws[2^lam + q] = Z[2^(l0+lam) + T*2^lam + q], 1 <= lam < r: one bulk copy per layer on `bar`, 8 * (2^r - 2)
-// bytes.  Layer 0's single 8-byte entry tws[1] = Z[2^l0 + T] is too small for a bulk copy: the producer writes it itself, before
-// its arrive on bar.
+// a tile's twiddle table of stage_tile_twiddles, layers 1 <= lam < r: one bulk copy per layer on `bar`, 8 * (2^r - 2) bytes.
+// Layer 0's single 8-byte entry tws[1] = Z[2^l0 + T] is too small for a bulk copy: the producer writes it itself, before its
+// arrive on bar.
 __device__ __forceinline__ void load_tile_twiddles(uint2 *tws, const uint2 *tw, int l0, u32 T, int r, u32 bar) {
 #pragma unroll 1
     for (int lam = 1; lam < r; lam++) bulk_load(tws + (1u << lam), tw + ((size_t)1 << (l0 + lam)) + ((size_t)T << lam), 8u << lam, bar);
@@ -380,20 +391,12 @@ ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
         cw = min(CT, a.w - col);
         ibase = (a.l0 == 0 ? 0u : (T << (a.log_n - a.l0))) | L;
     };
-    auto issue_twiddles = [&](u32 coset, u32 T, uint2 *tws) {
-        const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
-        for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {
-            const int lam = 31 - __clz(k);
-            const u32 ql = k - (1u << lam);
-            cp_async8(tws + k, tw + ((size_t)1 << (a.l0 + lam)) + ((size_t)T << lam) + ql);
-        }
-    };
     auto issue = [&](u32 t, u32 buf) {
         u32 coset, col, cw, T, ibase;
         decode(t, coset, col, cw, T, ibase);
         u32 *data = data0 + buf * buf_words;
         const u32 *in = a.in + (size_t)coset * a.in_stride + col;
-        if (!shared_tw || a.n_cosets > 1) issue_twiddles(coset, T, tws0 + buf * R);
+        if (!shared_tw || a.n_cosets > 1) stage_tile_twiddles<THREADS, true>(tws0 + buf * R, a.tw + (size_t)coset * a.tw_stride, a.l0, T, R);
         // chunk = 16 bytes (4 columns) when aligned, else one element
         const u32 cpr = vec16 ? (cw >> 2) : cw;                  // chunks per row segment
         const u32 rs = (THREADS / cpr) & ~(E2 - 1u);             // rows per sweep: a multiple of E2 keeps the shared address linear
@@ -440,7 +443,7 @@ ntt_pass_fast_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
 #else
 #define P3_STAMP(slot) do { } while (0)
 #endif
-    if (shared_tw && a.n_cosets == 1) issue_twiddles(0, 0, tws0);   // once per CTA, lands with the first tile's group
+    if (shared_tw && a.n_cosets == 1) stage_tile_twiddles<THREADS, true>(tws0, a.tw, a.l0, 0, R);   // once per CTA, lands with the first tile's group
     if (NBUF == 2) issue(t, 0);
     for (u32 k = 0; t < total; t += gridDim.x, k++) {
         const u32 buf = NBUF == 2 ? (k & 1u) : 0u;
@@ -597,6 +600,102 @@ __device__ __forceinline__ void tma_store_part(const CUtensorMap *map, const voi
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
 
+// The band's layers as both band kernels split them: LX cross-CTA layers (step X), then QA (step A) and QB (step B) local layers
+// on each CTA's part of RQ rows.
+template <int R_LOG, int CL> struct BandShape {
+    static constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;
+    static constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;
+    static constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
+    static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
+};
+
+// The steps of one band on the CTA's part `part` (w columns) with the band's twiddles `tws`, run by THREADS threads of which the
+// caller is thread t.  A kernel's profiling build skips them with P3GPU_NTT_NOBFLY (bit 1: step X, bit 0: steps A and B).
+// ---- step X: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p.  An item is 4 adjacent columns: one 16-byte access
+// per peer needs a quarter of the instructions of word accesses and keeps 4x the bytes in flight (the exchange is bound by the
+// latency of remote shared memory, not by its bandwidth).
+template <int F, int R_LOG, int CL, u32 THREADS>
+__device__ __forceinline__ void band_step_x(const PassArgs &a, u32 *part, const uint2 *tws, u32 w, u32 q, u32 t) {
+    using S = BandShape<R_LOG, CL>;
+    u32 peer[CL];
+#pragma unroll
+    for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(part), (u32)p);
+    const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (S::RQ / CL) * (w / 4), base = 16 * q * items;
+    for (u32 it = t; it < items; it += THREADS) {
+        const u32 off = base + 16 * it;
+        uint4 v[CL];
+#pragma unroll
+        for (int p = 0; p < CL; p++) v[p] = ld_cluster_v4(peer[p] + off);
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            u32 x[CL];
+#pragma unroll
+            for (int p = 0; p < CL; p++) x[p] = (&v[p].x)[e];
+            reg_network<F, S::LX>(x, tws, 1u);
+#pragma unroll
+            for (int p = 0; p < CL; p++) (&v[p].x)[e] = x[p];
+        }
+#pragma unroll
+        for (int p = 0; p < CL; p++) st_cluster_v4(peer[p] + off, v[p]);
+    }
+}
+// ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
+template <int F, int R_LOG, int CL, u32 THREADS>
+__device__ __forceinline__ void band_step_a(const PassArgs &a, u32 *part, const uint2 *tws, u32 w, u32 q, u32 t) {
+    using S = BandShape<R_LOG, CL>;
+    for (u32 it = t; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << S::QB); it += THREADS) {
+        u32 *sp = part + it;
+        u32 x[1 << S::QA];
+#pragma unroll
+        for (u32 m = 0; m < (1u << S::QA); m++) x[m] = sp[m * (w << S::QB)];
+        reg_network<F, S::QA>(x, tws, (1u << S::LX) + q);
+#pragma unroll
+        for (u32 m = 0; m < (1u << S::QA); m++) sp[m * (w << S::QB)] = x[m];
+    }
+}
+// ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB; then the scale by a.scale (SCALE and a.has_scale) and the
+// final reduction (a.final_reduce)
+template <int F, int R_LOG, int CL, u32 THREADS, bool SCALE>
+__device__ __forceinline__ void band_step_b(const PassArgs &a, u32 *part, const uint2 *tws, u32 w, u32 q, u32 t) {
+    using S = BandShape<R_LOG, CL>;
+    for (u32 it = t; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << S::QA); it += THREADS) {
+        const u32 g = it / w, c = it - g * w;
+        u32 *sp = part + (g << S::QB) * w + c;
+        u32 x[1 << S::QB];
+#pragma unroll
+        for (u32 m = 0; m < (1u << S::QB); m++) x[m] = sp[m * w];
+        reg_network<F, S::QB>(x, tws, (1u << (S::LX + S::QA)) + (q << S::QA) + g);
+        if (SCALE && a.has_scale) {
+#pragma unroll
+            for (u32 m = 0; m < (1u << S::QB); m++) x[m] = shoup_mul<F>(x[m], a.scale);
+        }
+        if (a.final_reduce) {
+#pragma unroll
+            for (u32 m = 0; m < (1u << S::QB); m++) x[m] = fp_reduce<F>(x[m]);
+        }
+#pragma unroll
+        for (u32 m = 0; m < (1u << S::QB); m++) sp[m * w] = x[m];
+    }
+}
+// A contiguous band's part (not STRIDED): CTA q's RQ rows of band T of coset block `coset` come in as ONE bulk copy into `part`,
+// the band's twiddles as load_tile_twiddles' copies into `tws`, both on mbarrier `bar`; they leave as ONE bulk copy.
+template <int R_LOG, int CL>
+__device__ __forceinline__ void band_load_part(const PassArgs &a, u32 *part, uint2 *tws, u32 coset, u32 T, u32 q, u32 bar) {
+    using S = BandShape<R_LOG, CL>;
+    const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
+    const u32 qwords = S::RQ * a.w;
+    tws[1] = tw[((size_t)1 << a.l0) + T];
+    const bool load = !P3_SKIP(a.skip_load);
+    mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (S::R - 2));
+    if (load) bulk_load(part, a.in + (size_t)coset * a.in_stride + ((size_t)T * S::R + q * S::RQ) * a.w, qwords * 4, bar);
+    load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+}
+template <int R_LOG, int CL>
+__device__ __forceinline__ void band_store_part(const PassArgs &a, const u32 *part, u32 coset, u32 T, u32 q) {
+    using S = BandShape<R_LOG, CL>;
+    bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * S::R + q * S::RQ) * a.w, part, S::RQ * a.w * 4);
+}
+
 // a: l0 = log_n - R_LOG, l1 = log_n (rows of a band contiguous), dense in / out blocks of a.n_cosets cosets, w % 4 == 0, 16-byte aligned.
 // STRIDED: the first pass of a network instead (l0 = 0, l1 = R_LOG, one block, no pitch).  Its "band" T is the strided unit of rows
 // T + 2^(log_n - R_LOG) * i, i < 2^R_LOG, so the same network runs on the unit's index i.  CTA q's part, rows i in [q*RQ, (q+1)*RQ),
@@ -607,13 +706,10 @@ __device__ __forceinline__ void tma_store_part(const CUtensorMap *map, const voi
 template <int F, int R_LOG, int CL, bool STRIDED>
 __global__ void __launch_bounds__(BAND_THREADS, 1)
 ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap) {
-    constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
-    constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
-    constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
+    constexpr u32 RQ = BandShape<R_LOG, CL>::RQ, R = 1u << R_LOG;
     constexpr u32 NX = 32 * BAND_XWARPS, NL = 32 * BAND_LWARPS;    // threads [0, NX) exchange, [NX, NX + NL) local, then the copy warp
     constexpr u32 NS = STRIDED ? 4 : 3;                            // ring slots
     constexpr u32 TW_SLOTS = STRIDED ? 1 : NS;                     // twiddle tables: one per ring slot, or the one all units share
-    static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const u32 w = a.w;
     const u32 qwords = RQ * w;                                     // one part
@@ -633,20 +729,14 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
         out_of(k, coset, T);
         const u32 s = k % NS;
         const u32 bar = full_a + 8 * s;
-        const bool load = !P3_SKIP(a.skip_load);
         if constexpr (STRIDED) {
-            const bool tw = k == 0;
+            const bool load = !P3_SKIP(a.skip_load), tw = k == 0;
             if (tw) tws0[1] = a.tw[1];
             mbar_expect_tx(bar, (load ? qwords * 4 : 0) + (tw ? 8 * (R - 2) : 0));
             if (load) tma_load_part(&imap, data0 + s * qwords, T, q * RQ, bar);
             if (tw) load_tile_twiddles(tws0, a.tw, 0, 0, R_LOG, bar);
         } else {
-            const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
-            uint2 *tws = tws0 + s * R;
-            tws[1] = tw[((size_t)1 << a.l0) + T];
-            mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
-            if (load) bulk_load(data0 + s * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
-            load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+            band_load_part<R_LOG, CL>(a, data0 + s * qwords, tws0 + s * R, coset, T, q, bar);
         }
     };
     auto wait_full = [&](u32 k) { mbar_wait(full_a + 8 * (k % NS), (k / NS) & 1u); };   // band k is slot k % NS's (k / NS)-th load
@@ -664,32 +754,9 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
     // period k: exchange band k+1, local steps on band k; k = -1 only exchanges band 0
     for (int k = -1; k < n; k++) {
         if (threadIdx.x < NX) {
-            // ---- step X on band k+1: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p
-            if (k + 1 < n) {
+            if (k + 1 < n) {   // step X on band k+1
                 const u32 s = (k + 1) % NS;
-                const uint2 *tws = tws0 + (STRIDED ? 0 : s * R);
-                u32 peer[CL];
-#pragma unroll
-                for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(data0 + s * qwords), (u32)p);
-                // an item is 4 adjacent columns: one 16-byte access per peer needs a quarter of the instructions of word accesses
-                const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (RQ / CL) * (w / 4), base = 16 * q * items;
-                for (u32 it = threadIdx.x; it < items; it += NX) {
-                    const u32 off = base + 16 * it;
-                    uint4 v[CL];
-#pragma unroll
-                    for (int p = 0; p < CL; p++) v[p] = ld_cluster_v4(peer[p] + off);
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        u32 x[CL];
-#pragma unroll
-                        for (int p = 0; p < CL; p++) x[p] = (&v[p].x)[e];
-                        reg_network<F, LX>(x, tws, 1u);
-#pragma unroll
-                        for (int p = 0; p < CL; p++) (&v[p].x)[e] = x[p];
-                    }
-#pragma unroll
-                    for (int p = 0; p < CL; p++) st_cluster_v4(peer[p] + off, v[p]);
-                }
+                band_step_x<F, R_LOG, CL, NX>(a, data0 + s * qwords, tws0 + (STRIDED ? 0 : s * R), w, q, threadIdx.x);
             }
             cluster_sync_all();
         } else if (!copy_warp) {
@@ -697,36 +764,9 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
                 const u32 s = k % NS, lt = threadIdx.x - NX;
                 u32 *data = data0 + s * qwords;
                 const uint2 *tws = tws0 + (STRIDED ? 0 : s * R);
-                // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
-                for (u32 it = lt; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += NL) {
-                    u32 *sp = data + it;
-                    u32 x[1 << QA];
-#pragma unroll
-                    for (u32 m = 0; m < (1u << QA); m++) x[m] = sp[m * (w << QB)];
-                    reg_network<F, QA>(x, tws, (1u << LX) + q);
-#pragma unroll
-                    for (u32 m = 0; m < (1u << QA); m++) sp[m * (w << QB)] = x[m];
-                }
+                band_step_a<F, R_LOG, CL, NL>(a, data, tws, w, q, lt);
                 asm volatile("bar.sync 1, %0;" ::"n"(NL) : "memory");
-                // ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB
-                for (u32 it = lt; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += NL) {
-                    const u32 g = it / w, c = it - g * w;
-                    u32 *sp = data + (g << QB) * w + c;
-                    u32 x[1 << QB];
-#pragma unroll
-                    for (u32 m = 0; m < (1u << QB); m++) x[m] = sp[m * w];
-                    reg_network<F, QB>(x, tws, (1u << (LX + QA)) + (q << QA) + g);
-                    if (STRIDED && a.has_scale) {
-#pragma unroll
-                        for (u32 m = 0; m < (1u << QB); m++) x[m] = shoup_mul<F>(x[m], a.scale);
-                    }
-                    if (a.final_reduce) {
-#pragma unroll
-                        for (u32 m = 0; m < (1u << QB); m++) x[m] = fp_reduce<F>(x[m]);
-                    }
-#pragma unroll
-                    for (u32 m = 0; m < (1u << QB); m++) sp[m * w] = x[m];
-                }
+                band_step_b<F, R_LOG, CL, NL, STRIDED>(a, data, tws, w, q, lt);
                 fence_proxy_async_smem();
                 asm volatile("bar.arrive 2, %0;" ::"n"(NL + 32) : "memory");   // band k may be stored
             }
@@ -739,7 +779,7 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
                     u32 coset, T;
                     out_of(k, coset, T);
                     if constexpr (STRIDED) tma_store_part(&omap, data0 + (k % NS) * qwords, T, q * RQ);
-                    else bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data0 + (k % NS) * qwords, qwords * 4);
+                    else band_store_part<R_LOG, CL>(a, data0 + (k % NS) * qwords, coset, T, q);
                 }
             }
             __syncwarp();
@@ -756,18 +796,15 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
     cluster_sync_all();   // no CTA exits while a peer may still map its shared memory
 }
 
-// Narrow matrices: the same pass in 4-CTA clusters with a 2-slot ring and no warp roles (every thread exchanges band k, then
+// Narrow matrices: the same pass and steps in 4-CTA clusters with a 2-slot ring and no warp roles (every thread exchanges band k, then
 // runs its steps A and B, while thread 0 loads band k+1).  With little work per band the pass is bound by its per-band barriers,
 // and 4-CTA clusters (30 on the H100) take half as many bands each as 8-CTA clusters (15).
 template <int F, int R_LOG, int CL>
 __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_kernel(const __grid_constant__ PassArgs a) {
-    constexpr int LX = CL == 8 ? 3 : CL == 4 ? 2 : 1;            // cross-CTA layers
-    constexpr int QB = (R_LOG - LX + 1) / 2, QA = R_LOG - LX - QB;  // local layers: step A, then step B
-    constexpr u32 RQ = 1u << (R_LOG - LX), R = 1u << R_LOG;
-    static_assert(CL == 1 << LX && QA >= 1, "band pass: cluster size");
+    constexpr u32 NT = BAND_NARROW_THREADS, R = 1u << R_LOG;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const u32 w = a.w;
-    const u32 qwords = RQ * w;                                     // one quarter
+    const u32 qwords = BandShape<R_LOG, CL>::RQ * w;               // one quarter
     u32 *data0 = reinterpret_cast<u32 *>(smem_raw);
     uint2 *tws0 = reinterpret_cast<uint2 *>(data0 + 2 * qwords);
     unsigned long long *full = reinterpret_cast<unsigned long long *>(tws0 + 2 * R);
@@ -778,15 +815,7 @@ __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_k
     const u32 total = a.n_cosets << band_log;
 
     auto issue = [&](u32 t, u32 buf) {   // thread 0: band t's quarter and twiddles into ring slot buf
-        const u32 coset = t >> band_log, T = t & ((1u << band_log) - 1u);
-        const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
-        uint2 *tws = tws0 + buf * R;
-        tws[1] = tw[((size_t)1 << a.l0) + T];
-        const u32 bar = full_a + 8 * buf;
-        const bool load = !P3_SKIP(a.skip_load);
-        mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
-        if (load) bulk_load(data0 + buf * qwords, a.in + (size_t)coset * a.in_stride + ((size_t)T * R + q * RQ) * w, qwords * 4, bar);
-        load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
+        band_load_part<R_LOG, CL>(a, data0 + buf * qwords, tws0 + buf * R, t >> band_log, t & ((1u << band_log) - 1u), q, full_a + 8 * buf);
     };
 
     u32 t = blockIdx.x / CL;
@@ -802,69 +831,18 @@ __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_k
         const uint2 *tws = tws0 + buf * R;
         mbar_wait(full_a + 8 * buf, (k >> 1) & 1u);
         cluster_sync_all();   // every CTA of the cluster holds its quarter of band t
-        // ---- step X: rows j + p*RQ, p < CL, j in CTA q's share; x[p] lives in CTA p
-        {
-            u32 peer[CL];
-#pragma unroll
-            for (int p = 0; p < CL; p++) peer[p] = cluster_map((u32)__cvta_generic_to_shared(data), (u32)p);
-            // an item is 4 adjacent columns: one 16-byte access per peer keeps 4x the bytes in flight of word accesses (the exchange
-            // is bound by the latency of remote shared memory, not by its bandwidth)
-            const u32 items = P3_SKIP(a.skip_bfly & 2) ? 0 : (RQ / CL) * (w / 4), base = 16 * q * items;
-            for (u32 it = threadIdx.x; it < items; it += BAND_NARROW_THREADS) {
-                const u32 off = base + 16 * it;
-                uint4 v[CL];
-#pragma unroll
-                for (int p = 0; p < CL; p++) v[p] = ld_cluster_v4(peer[p] + off);
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    u32 x[CL];
-#pragma unroll
-                    for (int p = 0; p < CL; p++) x[p] = (&v[p].x)[e];
-                    reg_network<F, LX>(x, tws, 1u);
-#pragma unroll
-                    for (int p = 0; p < CL; p++) (&v[p].x)[e] = x[p];
-                }
-#pragma unroll
-                for (int p = 0; p < CL; p++) st_cluster_v4(peer[p] + off, v[p]);
-            }
-        }
+        band_step_x<F, R_LOG, CL, NT>(a, data, tws, w, q, threadIdx.x);
         cluster_sync_all();   // every CTA has the exchanged values of its quarter; nobody touches a peer's buffer before the next band
         if (threadIdx.x == 0 && t + n_clusters < total) {
             bulk_wait_read();   // band k-1's store has read out the other buffer
             issue(t + n_clusters, buf ^ 1u);
         }
-        // ---- step A: item (g, c) holds local rows g + m * 2^QB, m < 2^QA (layers LX .. LX+QA-1 of block q)
-        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QB); it += BAND_NARROW_THREADS) {
-            u32 *sp = data + it;
-            u32 x[1 << QA];
-#pragma unroll
-            for (u32 m = 0; m < (1u << QA); m++) x[m] = sp[m * (w << QB)];
-            reg_network<F, QA>(x, tws, (1u << LX) + q);
-#pragma unroll
-            for (u32 m = 0; m < (1u << QA); m++) sp[m * (w << QB)] = x[m];
-        }
+        band_step_a<F, R_LOG, CL, NT>(a, data, tws, w, q, threadIdx.x);
         __syncthreads();
-        // ---- step B: item (g, c) holds local rows g * 2^QB + m, m < 2^QB
-        for (u32 it = threadIdx.x; it < (P3_SKIP(a.skip_bfly & 1) ? 0 : w << QA); it += BAND_NARROW_THREADS) {
-            const u32 g = it / w, c = it - g * w;
-            u32 *sp = data + (g << QB) * w + c;
-            u32 x[1 << QB];
-#pragma unroll
-            for (u32 m = 0; m < (1u << QB); m++) x[m] = sp[m * w];
-            reg_network<F, QB>(x, tws, (1u << (LX + QA)) + (q << QA) + g);
-            if (a.final_reduce) {
-#pragma unroll
-                for (u32 m = 0; m < (1u << QB); m++) x[m] = fp_reduce<F>(x[m]);
-            }
-#pragma unroll
-            for (u32 m = 0; m < (1u << QB); m++) sp[m * w] = x[m];
-        }
+        band_step_b<F, R_LOG, CL, NT, false>(a, data, tws, w, q, threadIdx.x);
         fence_proxy_async_smem();
         __syncthreads();
-        if (threadIdx.x == 0 && !P3_SKIP(a.skip_store)) {
-            const u32 coset = t >> band_log, T = t & ((1u << band_log) - 1u);
-            bulk_store(a.out + (size_t)coset * a.out_stride + ((size_t)T * R + q * RQ) * w, data, qwords * 4);
-        }
+        if (threadIdx.x == 0 && !P3_SKIP(a.skip_store)) band_store_part<R_LOG, CL>(a, data, t >> band_log, t & ((1u << band_log) - 1u), q);
     }
     if (threadIdx.x == 0) bulk_wait_all();
 }
@@ -921,11 +899,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
     auto issue = [&](u32 t, u32 buf) {
         const u32 ctile = t % a.n_ctiles, T = __brev(t / a.n_ctiles) >> (32 - R_LOG);
         const u32 col = ctile * CT, cw = min(CT, a.w - col);
-        uint2 *tws = twi0 + buf * R;
-        for (u32 k = threadIdx.x + 1; k < R; k += THREADS) {   // tws[2^lam + q] = Z_inv[2^(r+lam) + T*2^lam + q]
-            const int lam = 31 - __clz(k);
-            cp_async8(tws + k, a.tw + ((size_t)1 << (R_LOG + lam)) + ((size_t)T << lam) + (k - (1u << lam)));
-        }
+        stage_tile_twiddles<THREADS, true>(twi0 + buf * R, a.tw, R_LOG, T, R);   // the inverse heap's layers [r, 2r)
         const u32 cpr = cw >> 2;                         // 16-byte chunks per row segment
         const u32 rs = (THREADS / cpr) & ~(E2 - 1u);     // rows per sweep, >= E2 because THREADS >= 4 * E1 * cpr
         if (threadIdx.x < rs * cpr) {
@@ -1207,14 +1181,9 @@ __global__ void __launch_bounds__(NGROUP * GTHREADS + 32, 1) ntt_pass_pipe_kerne
             {
                 const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
                 uint2 *tws = tws0 + b * R;
-                tws[1] = tw[((size_t)1 << a.l0) + T];   // layer lam = 0 has a single 8-byte entry: too small for a bulk copy
+                tws[1] = tw[((size_t)1 << a.l0) + T];
                 mbar_expect_tx(twfull_bar(b), 8u * (R - 2u));
-#pragma unroll 1
-                for (int lam = 1; lam < R_LOG; lam++) {
-                    const uint2 *src = tw + ((size_t)1 << (a.l0 + lam)) + ((size_t)T << lam);
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"((u32)__cvta_generic_to_shared(tws + (1u << lam))), "l"(src), "r"(8u << lam), "r"(twfull_bar(b)) : "memory");
-                }
+                load_tile_twiddles(tws, tw, a.l0, T, R_LOG, twfull_bar(b));
             }
             // tensor coordinates: (column, 0, 0, c3, c4); see make_pass_tensor_map
             // tiled input: column tile ct, block cb is the 8-column matrix number ct * in_blocks + cb (blocks fold into dim 4)
@@ -1228,9 +1197,7 @@ __global__ void __launch_bounds__(NGROUP * GTHREADS + 32, 1) ntt_pass_pipe_kerne
                 mbar_expect_tx(full_bar(s), BOX_BYTES);
                 const int cc0 = a.in_tiled ? 0 : (int)(ct * CT);
                 const int cc4 = a.in_tiled ? c4 + (int)((ct * a.in_blocks) << blk_sh) : c4;
-                asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-                             ::"r"((u32)__cvta_generic_to_shared(stages + (size_t)s * STAGE_WORDS)), "l"(reinterpret_cast<unsigned long long>(&tmap)),
-                               "r"(cc0), "r"(0), "r"(0), "r"(c3), "r"(cc4), "r"(full_bar(s)) : "memory");
+                tma_load_tile(&tmap, stages + (size_t)s * STAGE_WORDS, cc0, c3, cc4, full_bar(s));
             }
         }
         return;
@@ -1332,7 +1299,7 @@ __global__ void __launch_bounds__(NGROUP * GTHREADS + 32, 1) ntt_pass_pipe_kerne
                     u32 gn = g + dg, cn = c + dc;
                     if (cn >= cw) { cn -= cw; gn++; }
                     if (gn >= E1) {   // last shared-memory read of this thread for this stage: hand it back to the producer
-                        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                        fence_proxy_async_smem();
                         mbar_arrive(empty_bar(s));
                         released = true;
                     }
@@ -1358,7 +1325,7 @@ __global__ void __launch_bounds__(NGROUP * GTHREADS + 32, 1) ntt_pass_pipe_kerne
                     g = gn; c = cn;
                 }
                 if (!released) {   // threads without a step-2 item (ragged tile)
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    fence_proxy_async_smem();
                     mbar_arrive(empty_bar(s));
                 }
             }
@@ -1457,13 +1424,41 @@ static int32_t get_twiddles(p3gpu_ctx *ctx, int log_n, int added_bits, u32 shift
     return P3GPU_OK;
 }
 
+// Kernel KERN's dynamic shared-memory limit (at least the default 48 KB) for launches of `smem` bytes, set on ctx's device when
+// the previous launch of KERN there asked for another size.  *changed (if given) says so, for whatever the caller derives from
+// the size.
+template <auto KERN> static int32_t set_smem_limit(p3gpu_ctx *ctx, size_t smem, bool *changed = nullptr) {
+    static size_t set[64] = {0};   // per instance and device
+    size_t &last = set[ctx->device & 63];
+    if (changed) *changed = smem != last;
+    if (smem != last) {
+        P3_CUDA(cudaFuncSetAttribute(KERN, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+        last = smem;
+    }
+    return P3GPU_OK;
+}
+
+// Grid of persistent kernel KERN over `items` work items: as many CTAs of `block` threads and `smem` bytes per SM as the register
+// file, shared memory (227 KB, 1 KB reserved per CTA) and `cap` allow, at least one, and no more CTAs than items.
+template <auto KERN> static int32_t persistent_grid(p3gpu_ctx *ctx, size_t block, size_t smem, size_t cap, size_t items, size_t *grid) {
+    static int num_regs = 0;   // per instance; benign race (same value)
+    if (num_regs == 0) {
+        cudaFuncAttributes fa;
+        P3_CUDA(cudaFuncGetAttributes(&fa, KERN));
+        num_regs = std::max(fa.numRegs, 16);
+    }
+    const size_t per_sm = std::min({cap, (227 * 1024) / (smem + 1024), 65536 / (block * (size_t)num_regs)});
+    *grid = std::min(items, std::max<size_t>(per_sm, 1) * (size_t)ctx->sm_count);
+    return P3GPU_OK;
+}
+
 template <int F, int LOG_CT, bool VEC>
 static int32_t launch_pass_ct(p3gpu_ctx *ctx, const PassArgs &a) {
     constexpr int THREADS = 256;
     const int r = a.l1 - a.l0;
     const size_t smem = (((size_t)1 << r) << LOG_CT) * 4 + ((size_t)1 << r) * sizeof(uint2);
-    auto kern = ntt_pass_kernel<F, LOG_CT, THREADS, VEC>;
-    if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    constexpr auto kern = ntt_pass_kernel<F, LOG_CT, THREADS, VEC>;
+    P3_TRY(set_smem_limit<kern>(ctx, smem));
     const size_t tiles = ((size_t)1 << (a.log_n - r)) * a.n_ctiles * a.n_cosets;
     P3_CHECK(tiles < (1ull << 31), P3GPU_EINVAL, "ntt: grid too large");
     kern<<<(unsigned)tiles, THREADS, smem, ctx->stream>>>(a);
@@ -1490,27 +1485,14 @@ static int32_t launch_fast_rct(p3gpu_ctx *ctx, PassArgs a) {
         P3_TRY(make_pass_tensor_map(a, a.out, false, a.out_stride, ct, false, Q2, &omap));
     }
     const size_t smem = NBUF * buf_words * 4 + NBUF * ((size_t)1 << R_LOG) * sizeof(uint2);
-    auto kern = ntt_pass_fast_kernel<F, R_LOG, CT_T, THREADS, NBUF>;
+    constexpr auto kern = ntt_pass_fast_kernel<F, R_LOG, CT_T, THREADS, NBUF>;
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: tile does not fit shared memory");
-    static size_t smem_set[64] = {0};   // per instantiation and device: raise the dynamic shared memory limit once per size
-    if (smem > 48 * 1024 && smem > smem_set[ctx->device & 63]) {
-        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        smem_set[ctx->device & 63] = smem;
-    }
+    P3_TRY(set_smem_limit<kern>(ctx, smem));
     const size_t tiles = ((size_t)1 << (a.log_n - R_LOG)) * a.n_ctiles * a.n_cosets;
     P3_CHECK(tiles < (1ull << 31), P3GPU_EINVAL, "ntt: grid too large");
     // persistent grid: one CTA per SM (more when the tile is small enough for several to be resident)
-    size_t per_sm = std::min<size_t>(NBUF == 1 ? 2048 / THREADS : 2, (227 * 1024) / (smem + 1024));
-    static int num_regs = 0;   // per instantiation; benign race (same value)
-    if (num_regs == 0) {
-        cudaFuncAttributes fa;
-        P3_CUDA(cudaFuncGetAttributes(&fa, kern));
-        num_regs = std::max(fa.numRegs, 16);
-    }
-    const size_t by_regs = 65536 / ((size_t)THREADS * (size_t)num_regs);   // register file of the SM
-    if (per_sm > by_regs) per_sm = by_regs;
-    if (per_sm < 1) per_sm = 1;
-    const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
+    size_t grid;
+    P3_TRY(persistent_grid<kern>(ctx, THREADS, smem, NBUF == 1 ? 2048 / THREADS : 2, tiles, &grid));
     kern<<<(unsigned)grid, THREADS, smem, ctx->stream>>>(a, omap);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
@@ -1565,7 +1547,7 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
     const size_t qbytes = (((size_t)a.w * 4) << R_LOG) / CL;
     const size_t tw_bytes = ((size_t)1 << R_LOG) * sizeof(uint2);
     const size_t smem = STRIDED ? 4 * (qbytes + 8) + tw_bytes : SLOTS * (qbytes + tw_bytes + 8);
-    const auto kern = [] {
+    constexpr auto kern = [] {
         if constexpr (NARROW) return ntt_band_pass_narrow_kernel<F, R_LOG, CL>;
         else return ntt_band_pass_kernel<F, R_LOG, CL, STRIDED>;
     }();
@@ -1575,8 +1557,7 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
         P3_TRY(make_unit_tensor_map(a.in, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &imap));
         P3_TRY(make_unit_tensor_map(a.out, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &omap));
     }
-    // per instantiation and device: the shared memory limit and the number of clusters that fit at once, for the last size asked
-    static size_t smem_set[64] = {0};
+    // per instantiation and device: the number of clusters that fit at once, for the size set_smem_limit last saw
     static int clusters[64] = {0};
     const int dev = ctx->device & 63;
     cudaLaunchAttribute attr;
@@ -1585,14 +1566,14 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
     cudaLaunchConfig_t cfg = {};
     cfg.blockDim = dim3(NARROW ? BAND_NARROW_THREADS : BAND_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = ctx->stream;
     cfg.attrs = &attr; cfg.numAttrs = 1;
-    if (smem != smem_set[dev]) {
-        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
+    bool changed;
+    P3_TRY(set_smem_limit<kern>(ctx, smem, &changed));
+    if (changed) {
         cfg.gridDim = dim3(CL * ctx->sm_count);
         int n = 0;
         P3_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
         P3_CHECK(n > 0, P3GPU_ECUDA, "ntt: no %d-CTA cluster of the band pass fits the device", CL);
         clusters[dev] = n;
-        smem_set[dev] = smem;
     }
     const size_t bands = (size_t)a.n_cosets << (a.log_n - R_LOG);
     cfg.gridDim = dim3((unsigned)(CL * std::min<size_t>(bands, (size_t)clusters[dev])));
@@ -1653,23 +1634,12 @@ static int32_t launch_lde_mid_rcp(p3gpu_ctx *ctx, const PassArgs &a, const uint2
     const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2) + (PROD ? 5 * 8 : 0);
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: fused LDE tile does not fit shared memory");
     P3_CHECK(gs2 == (e1 + 1) * ct && gs1 == (e2 + 1) * ct, P3GPU_EINVAL, "ntt: fused LDE tile layout is no TMA box");
-    auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T, PROD>;
-    static size_t smem_set[64] = {0};   // per instantiation and device
-    if (smem > 48 * 1024 && smem > smem_set[ctx->device & 63]) {
-        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        smem_set[ctx->device & 63] = smem;
-    }
+    constexpr auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T, PROD>;
+    P3_TRY(set_smem_limit<kern>(ctx, smem));
     const size_t tiles = ((size_t)1 << (a.log_n - R_LOG)) * a.n_ctiles;
     // persistent grid: as many CTAs per SM as threads, registers and shared memory allow (one at 2^20 rows)
-    size_t per_sm = std::min<size_t>(2048 / BLOCK, (227 * 1024) / (smem + 1024));
-    static int num_regs = 0;   // per instantiation; benign race (same value)
-    if (num_regs == 0) {
-        cudaFuncAttributes fa;
-        P3_CUDA(cudaFuncGetAttributes(&fa, kern));
-        num_regs = std::max(fa.numRegs, 16);
-    }
-    per_sm = std::max<size_t>(1, std::min<size_t>(per_sm, 65536 / ((size_t)BLOCK * (size_t)num_regs)));
-    const size_t grid = std::min(tiles, per_sm * (size_t)ctx->sm_count);
+    size_t grid;
+    P3_TRY(persistent_grid<kern>(ctx, BLOCK, smem, 2048 / BLOCK, tiles, &grid));
     kern<<<(unsigned)grid, BLOCK, smem, ctx->stream>>>(a, tw_fwd, omap, imap);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
@@ -1799,12 +1769,8 @@ static int32_t launch_pipe_r(p3gpu_ctx *ctx, PassArgs a) {
     P3_CHECK(items < (1ull << 31), P3GPU_EINVAL, "ntt: too many tiles");
     P3_CHECK((size_t)a.tpi * NGROUP * GTHREADS < (1u << 20), P3GPU_EINVAL, "ntt: too many column tiles per unit for the mbarrier count");
     a.n_items = (u32)items;
-    auto kern = ntt_pass_pipe_kernel<F, R_LOG, PERM, NSTAGE, NGROUP, GTHREADS>;
-    static bool attr_set[64] = {false};
-    if (!attr_set[ctx->device & 63]) {
-        P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set[ctx->device & 63] = true;
-    }
+    constexpr auto kern = ntt_pass_pipe_kernel<F, R_LOG, PERM, NSTAGE, NGROUP, GTHREADS>;
+    P3_TRY(set_smem_limit<kern>(ctx, smem));
     const size_t grid = std::min(items, (size_t)ctx->sm_count);
     kern<<<(unsigned)grid, NGROUP * GTHREADS + 32, smem, ctx->stream>>>(tm, a);
     ctx->launches++;

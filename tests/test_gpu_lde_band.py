@@ -1,8 +1,9 @@
-"""Forward pass 2 of the three-launch coset LDE on whole-row bands (csrc/ntt.cu: ntt_band_pass_kernel, 4-CTA clusters).
+"""Forward pass 2 of the three-launch coset LDE on whole-row bands (csrc/ntt.cu: ntt_band_pass_kernel, 8-CTA clusters; up to
+48 columns ntt_band_pass_narrow_kernel, 4-CTA clusters).
 
-The band pass takes the LDE's last pass when a quarter band (2^r / 4 rows x w columns, r = log_h / 2) fits its 100 KB ring slot
-and the width is a multiple of 4: w <= 800 at 2^14 rows, <= 200 at 2^18, <= 100 at 2^20.  Every other width keeps the tile
-kernel (ntt_pass_fast_kernel), and P3GPU_NTT_BAND=0 forces it.  Each case writes into a poisoned, guarded output and must be
+The band pass takes the LDE's last pass when an eighth of a band (2^r / 8 rows x w columns, r = log_h / 2) fits its 50 KB ring
+slot (BAND_CL, BAND_SLOT_BYTES) and the width is a multiple of 4: w <= 800 at 2^14 rows, <= 200 at 2^18, <= 100 at 2^20.  Every
+other width keeps the tile kernel (ntt_pass_fast_kernel), and P3GPU_NTT_BAND=0 forces it.  Each case writes into a poisoned, guarded output and must be
 bit-identical to the same call on the tile kernel; at 2^14 rows it is also checked against the CPU oracle."""
 import numpy as np
 import pytest
@@ -90,7 +91,7 @@ def test_band_pass_small_matches_oracle(gpu, f, w, added_bits, monkeypatch):
 @pytest.mark.parametrize("f", FIELDS, ids=lambda f: f.name)
 @pytest.mark.parametrize("log_h,w", [(18, 4), (18, 8), (18, 96), (18, 100), (18, 200), (20, 4), (20, 8), (20, 96), (20, 100), (20, 104)])
 def test_band_pass_matches_tile_kernel(gpu, f, log_h, w, monkeypatch):
-    # 2^20 x 104: a quarter band of 104 KB does not fit the ring slot, so both calls run the tile kernel (the fallback)
+    # 2^20 x 104: an eighth of a band, 52 KB, does not fit the ring slot, so both calls run the tile kernel (the fallback)
     if log_h < 20:
         monkeypatch.setenv("P3GPU_NTT_PIPE", "0")
     _band_against_tile_kernel(gpu, f, log_h, w, 1, monkeypatch)
@@ -103,7 +104,7 @@ def test_band_pass_four_cosets_full_height(gpu, f, monkeypatch):
 
 @pytest.mark.parametrize("log_h,w,band", [(20, 100, True), (20, 104, False), (18, 200, True), (18, 204, False), (14, 800, True)])
 def test_band_pass_dispatch(gpu, log_h, w, band, monkeypatch):
-    # 104 columns at 2^20 rows (204 at 2^18) make a quarter band of 104 KB (102 KB), more than a ring slot: the tile kernel runs
+    # 104 columns at 2^20 rows (204 at 2^18) make an eighth of a band of 52 KB (51 KB), more than a ring slot: the tile kernel runs
     if log_h < 20:
         monkeypatch.setenv("P3GPU_NTT_PIPE", "0")
     assert _band_kernel_launched(gpu, KoalaBear, log_h, w) == band

@@ -300,6 +300,16 @@ __device__ __forceinline__ void tma_store_tile(const CUtensorMap *map, const voi
                  : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// The same store with an L2 evict-last hint: the fused LDE pass writes each output row as short segments from several tiles,
+// which should merge in L2 before they go to HBM, and the next pass reads them back.
+__device__ __forceinline__ void tma_store_tile_keep(const CUtensorMap *map, const void *smem, int c0, int c3, int c4) {
+    unsigned long long policy;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(policy));
+    asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4, %5, %6}], [%1], %7;"
+                 ::"l"(reinterpret_cast<unsigned long long>(map)), "r"((u32)__cvta_generic_to_shared(smem)), "r"(c0), "r"(0), "r"(0), "r"(c3), "r"(c4), "l"(policy)
+                 : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
@@ -966,7 +976,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
 #endif
                         // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
-                        tma_store_tile(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
+                        tma_store_tile_keep(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
                         bulk_wait_read();   // the copy has read the buffer out: the next coset (or tile) may rewrite it
 #ifdef P3GPU_NTT_PROFILE
                         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));

@@ -8,6 +8,13 @@
 //   4. the first pass's strided units (2^20 x 100: unit L = rows L + 1024 i, i < 1024), 15 clusters of 8 CTAs, a 3-slot ring, no
 //      arithmetic: CTA q moves rows i in [128q, 128q + 128) of each unit from one 419 MB buffer to another, either as ONE 3-D tensor
 //      copy in and ONE 3-D tensor store out per part, or as 128 1-D bulk copies of 400 bytes each way (4 per lane of one warp).
+//   5. the fused middle pass's traffic at 2^20 x 100, two cosets, no arithmetic: 132 persistent CTAs with one lane each load row
+//      tile T (coefficient rows T * 1024 + rho) through the inverse-layout 5-D box and store it once per coset through the
+//      forward-layout box (rows L + 1024 i, T = bitrev10(L)), 419 MB read + 839 MB written, in two shapes:
+//      (a) 20-column tiles, 2 buffers, tile k + 2 loaded once tile k's last store has been read out (ntt_lde_mid_kernel);
+//      (b) 8-column tiles (one 4-column tile per row tile), a 5-stage ring, 3 tiles held at once, each stage released once its
+//          tile's two stores have been read out; each CTA takes whole row tiles;
+//      and each shape once with its loads only and once with its stores only (each stage loaded once, then stored from repeatedly).
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 band_probe.cu -o band_probe
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -163,6 +170,93 @@ static int unit_map(EncodeFn enc, void *base, CUtensorMap *tm) {
     return 0;
 }
 
+// 5. the fused middle pass's loads and stores; BW-column tiles, NS stages, HELD tiles waiting for their stores at once
+constexpr u32 MP_LOG = 10, MP_R = 1u << MP_LOG, MP_E = 32, MP_COSETS = 2;   // r = 10: E1 = E2 = 32
+template <u32 BW> __host__ __device__ constexpr u32 mp_box_bytes() { return MP_E * (MP_E + 1) * BW * 4; }   // 32 groups of 32 rows + a zero pad row
+template <u32 BW, u32 NS> constexpr size_t mp_smem() { return NS * (size_t)mp_box_bytes<BW>() + 64; }
+
+// LOADS / STORES = false: that side's copies are left out (without loads, each stage is loaded once and stored from repeatedly)
+template <u32 BW, u32 NS, u32 HELD, bool WHOLE_ROWS, bool LOADS = true, bool STORES = true>
+__global__ void __launch_bounds__(32, 1) mid_kernel(const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    unsigned long long *full = reinterpret_cast<unsigned long long *>(smem + NS * (size_t)mp_box_bytes<BW>());
+    if (threadIdx.x != 0) return;
+    constexpr u32 NCT = (W + BW - 1) / BW;
+    const u32 n = WHOLE_ROWS ? ((MP_R - 1 - blockIdx.x) / gridDim.x + 1) * NCT : (MP_R * NCT - 1 - blockIdx.x) / gridDim.x + 1;
+    auto tile = [&](u32 k, u32 &col, u32 &L) {
+        const u32 t = WHOLE_ROWS ? (blockIdx.x + (k / NCT) * gridDim.x) * NCT + k % NCT : blockIdx.x + k * gridDim.x;
+        col = (t % NCT) * BW; L = t / NCT;
+    };
+    for (u32 s = 0; s < NS; s++) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sa(full + s)));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    auto load = [&](u32 k) {
+        u32 col, L;
+        tile(k, col, L);
+        const u32 s = k % NS, T = __brev(L) >> (32 - MP_LOG);
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sa(full + s)), "r"(mp_box_bytes<BW>()) : "memory");
+        asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
+                     ::"r"(sa(smem + s * (size_t)mp_box_bytes<BW>())), "l"(reinterpret_cast<unsigned long long>(&imap)), "r"(col), "r"(0), "r"(0),
+                       "r"(0), "r"(T), "r"(sa(full + s)) : "memory");
+    };
+    for (u32 k = 0; k < NS && k < n; k++) load(k);
+    for (u32 k = 0; k < n; k++) {
+        u32 col, L;
+        tile(k, col, L);
+        const u32 s = k % NS;
+        if (LOADS || k < NS) mbar_wait(sa(full + s), (k / NS) & 1);
+        for (u32 cs = 0; cs < MP_COSETS && STORES; cs++) {
+            asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+                         ::"l"(reinterpret_cast<unsigned long long>(&omap)), "r"(sa(smem + s * (size_t)mp_box_bytes<BW>())), "r"(col), "r"(0), "r"(0),
+                           "r"(L), "r"(cs) : "memory");
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            if (HELD == 1) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // the next coset rewrites the buffer
+        }
+        // the stores of tile k + 1 - HELD have been read out: its stage takes tile k + 1 - HELD + NS
+        asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(MP_COSETS * (HELD - 1)) : "memory");
+        if (LOADS && k + 1 >= HELD && k + 1 - HELD + NS < n) load(k + 1 - HELD + NS);
+    }
+    asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+
+// the fused pass's maps (make_pass_tensor_map at r = 10): inverse layout (column, row in group, group, 0, T) over 2^20 x W, groups of
+// 32 rows (rho = group * 32 + row); forward layout (column, row in group, group, L, coset) over MP_COSETS blocks, row L + 1024 rho
+static int mid_map(EncodeFn enc, void *base, bool fwd, u32 bw, CUtensorMap *tm) {
+    const cuuint64_t p = (cuuint64_t)W * 4;
+    cuuint64_t dims[5] = {W, MP_E, MP_E, fwd ? MP_R : 1, fwd ? MP_COSETS : MP_R};
+    cuuint64_t strides[4] = {fwd ? p << MP_LOG : p, fwd ? p << (MP_LOG + 5) : p << 5, p, fwd ? p << (2 * MP_LOG) : p << MP_LOG};
+    cuuint32_t box[5] = {bw, MP_E + 1, MP_E, 1, 1}, es[5] = {1, 1, 1, 1, 1};
+    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { printf("cuTensorMapEncodeTiled: %d\n", (int)r); return 1; }
+    return 0;
+}
+
+template <u32 BW, u32 NS, u32 HELD, bool WHOLE_ROWS, bool LOADS = true, bool STORES = true>
+static int run_mid(EncodeFn enc, u32 *coef, u32 *out, int sms, const char *what) {
+    CUtensorMap imap, omap;
+    if (mid_map(enc, coef, false, BW, &imap) || mid_map(enc, out, true, BW, &omap)) return 1;
+    constexpr size_t smem = mp_smem<BW, NS>();
+    auto kern = mid_kernel<BW, NS, HELD, WHOLE_ROWS, LOADS, STORES>;
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    std::vector<float> ts;
+    for (int rep = 0; rep < 22; rep++) {
+        CK(cudaEventRecord(e0));
+        kern<<<sms, 32, smem>>>(imap, omap);
+        CK(cudaEventRecord(e1));
+        CK(cudaEventSynchronize(e1));
+        float ms; CK(cudaEventElapsedTime(&ms, e0, e1));
+        if (rep >= 2) ts.push_back(ms);
+    }
+    std::sort(ts.begin(), ts.end());
+    const double bytes = ((LOADS ? 1.0 : 0.0) + (STORES ? MP_COSETS : 0)) * ((size_t)W * 4 << (2 * MP_LOG));
+    printf("fused middle pass traffic 2^%u x %u, %u cosets, %s: %zu B boxes, %u stages, %u held, %d CTAs: median of %zu %.3f ms (min %.3f, max %.3f) = %.0f GB/s\n",
+           2 * MP_LOG, W, MP_COSETS, what, (size_t)mp_box_bytes<BW>(), NS, HELD, sms, ts.size(), ts[ts.size() / 2], ts[0], ts.back(),
+           bytes / (ts[ts.size() / 2] * 1e-3) / 1e9);
+    return 0;
+}
+
 template <typename K, typename... A>
 static cudaError_t launch_cluster(K kern, u32 grid, u32 cl, A... args) {
     cudaLaunchConfig_t cfg = {};
@@ -279,5 +373,17 @@ int main() {
                st.back(), 2.0 * sbytes / (st[st.size() / 2] * 1e-3) / 1e9, copied ? "" : " (COPY WRONG)");
     }
     CK(cudaFree(src)); CK(cudaFree(dst));
+    // 5. the fused middle pass's traffic
+    u32 *coef, *out;
+    CK(cudaMalloc(&coef, sbytes)); CK(cudaMalloc(&out, MP_COSETS * sbytes));
+    CK(cudaMemset(coef, 1, sbytes)); CK(cudaMemset(out, 0, MP_COSETS * sbytes));
+    if (run_mid<20, 2, 1, false>(enc, coef, out, prop.multiProcessorCount, "(a) 20-column tiles, 2 buffers") ||
+        run_mid<8, 5, 3, true>(enc, coef, out, prop.multiProcessorCount, "(b) 8-column tiles, 5-stage ring, whole row tiles per CTA") ||
+        run_mid<20, 2, 1, false, true, false>(enc, coef, out, prop.multiProcessorCount, "(a) loads only") ||
+        run_mid<20, 2, 1, false, false, true>(enc, coef, out, prop.multiProcessorCount, "(a) stores only") ||
+        run_mid<8, 5, 3, true, true, false>(enc, coef, out, prop.multiProcessorCount, "(b) loads only") ||
+        run_mid<8, 5, 3, true, false, true>(enc, coef, out, prop.multiProcessorCount, "(b) stores only"))
+        return 1;
+    CK(cudaFree(coef)); CK(cudaFree(out));
     return 0;
 }

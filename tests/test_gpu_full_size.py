@@ -1,8 +1,8 @@
 """GPU parity at the BASELINE.json config 4 and config 5 SHAPES (the sizes bench.py times), through the C ABI.
 
 The CPU oracle cannot redo 10 GB of LDE + Merkle in a unit test, so each test checks, at the full shape:
-  * spot columns of the LDE against the oracle — at least one column from every column chunk the LDE driver loops over
-    (lde_tiled_impl processes wide matrices in chunks; a wrong chunk offset would only show in that chunk's columns);
+  * every word of the resident LDE against tests/ntt_reference.py on the device, and the launch count of the commit's LDE (a
+    dispatch change that moves it to another path fails here);
   * spot leaf digests against the oracle's sponge over the full-width row;
   * the left-most 2^12-row sub-tree against an oracle tree over those rows (sub-tree consistency);
   * a checksum of checksums: the cap recomputed on the CPU from a middle digest layer;
@@ -13,6 +13,8 @@ import pytest
 import torch
 
 from oracle import p3_oracle as O
+import ntt_reference as R
+from test_gpu_lde_paths import check_matrix
 
 from plonky3_b200 import _lib
 from plonky3_b200.field import BabyBear, KoalaBear
@@ -44,18 +46,27 @@ def _cap_from_layer(ohs, layer, cap_len):
     return lay
 
 
-def _check_commit(gpu, f, hash_kind, ohs, log_h, w, spot_cols, cap_height):
+def _check_commit(gpu, f, hash_kind, ohs, log_h, w, ntt_launches, cap_height):
+    """ntt_launches: the launches of the commit's LDE, which identify its path.  They are counted as the commit's launches less
+    those of merkle_commit over the resident LDE: this assumes that p3gpu_pcs_commit_dev hashes with the same call
+    (hash_merkle_commit on one matrix), so a change to either one that makes their launches differ shows as a wrong LDE count
+    here."""
     h = 1 << log_h
     g = torch.Generator(device="cuda"); g.manual_seed(1)
     x = torch.randint(0, f.P, (h, w), device="cuda", dtype=torch.int32, generator=g)
+    gpu.coset_lde_batch(f.id, x[:, :8].contiguous(), 1, f.generator)        # the twiddle heaps, so that none is built below
+    n0 = gpu.launches
     lde, layers = gpu.pcs_commit(f.id, hash_kind, x, 1)                      # TwoAdicFriPcs::commit: LDE + MMCS, resident
+    n1 = gpu.launches
+    gpu.merkle_commit(f.id, hash_kind, [lde])
+    n = (n1 - n0) - (gpu.launches - n1)
+    assert n == ntt_launches, f"the commit's LDE took {n} launches instead of {ntt_launches}: it left the path it pins"
     H = 2 * h
     assert tuple(lde.shape) == (H, w)
     assert [int(l.shape[0]) for l in layers] == [H >> k for k in range(log_h + 2)]
-    # LDE spot columns (every column chunk of the LDE driver is hit)
-    xs = host(x[:, spot_cols].contiguous())
-    exp = O.coset_lde_batch(f.id, xs, 1, f.generator, bitrev_out=True)
-    assert np.array_equal(host(lde[:, spot_cols].contiguous()), exp)
+    # the whole LDE against the reference, column chunk by column chunk on the device
+    check_matrix(f, lde, lambda c0, c1: R.coset_lde(f, x[:, c0:c1], 1, f.generator), lambda row, col: f"coset {row >> log_h}",
+                 f"{f.name} commit LDE 2^{log_h} x {w}")
     del x
     # spot leaf digests over the full-width row
     for r in (0, 1, 54321, H // 2, H - 1):
@@ -76,8 +87,8 @@ def test_config4_pcs_commit_keccak_babybear_2_22_x_300(gpu):
     """BASELINE config 4: BabyBear 2^22 x 300, blowup 2, SerializingHasher<PaddingFreeSponge<KeccakF,25,17,4>> leaves
     (9 permutations per row), CompressionFunctionFromHasher nodes, cap_height 3."""
     f = BabyBear
-    # the LDE driver works in 64-column chunks at this height: columns 0-63, 64-127, 128-191, 192-255, 256-299
-    lde, layers = _check_commit(gpu, f, _lib.HASH_KECCAK, O.keccak_hasher(), 22, 300, [0, 63, 64, 130, 200, 255, 256, 299], 3)
+    # the LDE runs on the tiled pipeline (8 + 7 + 7 layers: six launches per chunk) in 64-column chunks: columns 0-63, ..., 256-299
+    lde, layers = _check_commit(gpu, f, _lib.HASH_KECCAK, O.keccak_hasher(), 22, 300, 6 * 5, 3)
     del lde, layers
     torch.cuda.empty_cache()
 
@@ -102,14 +113,15 @@ def test_config4_fri_commit_phase_keccak_babybear_2_23(gpu):
 def test_config5_pcs_commit_poseidon2_koalabear_2_20_x_1312(gpu):
     """BASELINE config 5 trace commit: KoalaBear 2^20 x 1312, blowup 2, PaddingFreeSponge<Perm24,24,16,8> leaves (82
     permutations per row), TruncatedPermutation<Perm16> nodes, cap_height 3.  At this height the LDE runs on the cp.async
-    kernel; the tiled pipeline's driver would run 128-column chunks here (10 x 128 + 32, next test): one spot column from
-    each of the 11 chunks, plus chunk edges."""
+    kernel's three-launch path with 16-column tiles; the tiled pipeline's driver runs 128-column chunks here (10 x 128 + 32,
+    four launches each: next test)."""
+    _config5_commit(gpu, 3)
+
+
+def _config5_commit(gpu, ntt_launches):
     f = KoalaBear
     ohs = O.poseidon2_hasher(O.default_perm(f.id, 24), O.default_perm(f.id, 16))
-    cols = [128 * k + (37 * k) % 128 for k in range(10)] + [1280 + 31, 0, 127, 128, 1279, 1280]
-    lde, layers = _check_commit(gpu, f, _lib.HASH_POSEIDON2_W24, ohs, 20, 1312, cols, 3)
-    # the committed low coset (first 2^20 rows) holds the evaluations over GENERATOR * H: coset iDFT of a spot column
-    # returns the coefficients of the input column (round trip through a different transform)
+    lde, layers = _check_commit(gpu, f, _lib.HASH_POSEIDON2_W24, ohs, 20, 1312, ntt_launches, 3)
     del layers
     torch.cuda.empty_cache()
     del lde
@@ -119,7 +131,7 @@ def test_config5_pcs_commit_poseidon2_koalabear_2_20_x_1312(gpu):
 def test_config5_pcs_commit_on_the_tiled_pipeline(gpu, monkeypatch):
     """The same commit with P3GPU_NTT_PIPE=1: the LDE on the TMA pipeline with column-tile-major intermediates, in chunks."""
     monkeypatch.setenv("P3GPU_NTT_PIPE", "1")
-    test_config5_pcs_commit_poseidon2_koalabear_2_20_x_1312(gpu)
+    _config5_commit(gpu, 4 * 11)
 
 
 def test_config5_fri_commit_phase_poseidon2_koalabear_2_21(gpu):

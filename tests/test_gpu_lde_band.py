@@ -4,7 +4,8 @@
 The band pass takes the LDE's last pass when an eighth of a band (2^r / 8 rows x w columns, r = log_h / 2) fits its 50 KB ring
 slot (BAND_CL, BAND_SLOT_BYTES) and the width is a multiple of 4: w <= 800 at 2^14 rows, <= 200 at 2^18, <= 100 at 2^20.  Every
 other width keeps the tile kernel (ntt_pass_fast_kernel), and P3GPU_NTT_BAND=0 forces it.  Each case writes into a poisoned, guarded output and must be
-bit-identical to the same call on the tile kernel; at 2^14 rows it is also checked against the CPU oracle."""
+bit-identical to the same call on the tile kernel; at 2^14 rows it is also checked against the CPU oracle, and at 2^18 and 2^20 the
+tile kernel's result is checked against tests/ntt_reference.py on the device."""
 import numpy as np
 import pytest
 import torch
@@ -14,7 +15,8 @@ from oracle import p3_oracle as O
 from plonky3_b200 import _lib
 from plonky3_b200.field import BabyBear, KoalaBear
 from plonky3_b200.gpu import default_gpu
-from test_gpu_lde_paths import G, POISON, run_lde_checked
+import ntt_reference as R
+from test_gpu_lde_paths import G, POISON, check_matrix, run_lde_checked
 
 pytestmark = pytest.mark.gpu
 FIELDS = [BabyBear, KoalaBear]
@@ -58,6 +60,10 @@ def _band_against_tile_kernel(gpu, f, log_h, w, added_bits, monkeypatch):
     assert (u[:G] == POISON).all() and (u[-G:] == POISON).all(), f"{what}: band pass wrote outside its output"
     body = u[G:-G]
     assert (body < f.P).all(), f"{what}: {int((body >= f.P).sum())} words not canonical (never written?)"
+    if log_h >= 18:   # too large for the CPU oracle: the tile kernel's result against the reference transform on the device
+        H, xm = h << added_bits, x.view(h, w)
+        check_matrix(f, tile[G:G + H * w].view(H, w), lambda c0, c1: R.coset_lde(f, xm[:, c0:c1], added_bits, f.generator),
+                     lambda row, col: f"coset block {row >> log_h}", f"{what} on the tile kernel")
     bad = band != tile
     if bool(bad.any()):
         i = int(torch.nonzero(bad)[0]) - G

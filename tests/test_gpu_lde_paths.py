@@ -12,12 +12,16 @@ run_lde_checked / run_dft_checked make a missing store visible.  The context kee
 caching allocator hands a freed block back to the next allocation of that size, so a second call on the same input would find
 correct data from the first wherever it failed to write.  The helpers therefore run a dirty call on other data first, write the
 result into a buffer filled with 0xFFFFFFFF (not canonical in either field) with guard words on both sides, and check the guards,
-that every word is canonical, and the values; a failure names the coset and the row and column tiles it falls in."""
+that every word is canonical, and the values; a failure names the coset and the row and column tiles it falls in.
+
+A numpy input is checked against the CPU oracle.  Shapes too large for it take a DeviceInput (a seeded random matrix made on the
+device) and are checked on the device, column chunk by column chunk, against tests/ntt_reference.py."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import p3_oracle as O
+import ntt_reference as R
 
 from plonky3_b200 import _lib
 from plonky3_b200.dft import Radix2DitParallel
@@ -77,37 +81,62 @@ def _tiles(log_n, w, pos, col, fused):
     return s + f", first-pass row tile {pos & ((1 << r2) - 1)}, last-pass row tile {pos >> r2}"
 
 
-def _device_copy(m, off):
-    """m in a flat device buffer at word offset `off` (off = 1: contiguous, but not 16-byte aligned)."""
-    buf = torch.empty(m.size + off, dtype=torch.int32, device="cuda")
-    buf[off:] = torch.from_numpy(np.ascontiguousarray(m, dtype=np.uint32).view(np.int32).ravel()).cuda()
-    return buf
+class DeviceInput:
+    """A uniform random (h, w) matrix of Montgomery words made on the device from a seed, for shapes too large for the CPU
+    oracle: the checked calls fill their input buffer with it after the dirty call, and check the result against
+    ntt_reference on the device."""
+
+    def __init__(self, h, w, seed):
+        self.shape, self.seed = (h, w), seed
+
+
+def _fill_input(f, x, m):
+    """x (flat int32 device buffer) <- m: a numpy matrix, or the DeviceInput's matrix drawn in place."""
+    if isinstance(m, DeviceInput):
+        x.random_(0, f.P, generator=torch.Generator(device=x.device).manual_seed(m.seed))
+    else:
+        x.copy_(torch.from_numpy(np.ascontiguousarray(m, dtype=np.uint32).view(np.int32).ravel()))
 
 
 def _poisoned(words):
     return torch.full((words + 2 * G,), -1, dtype=torch.int32, device="cuda")
 
 
-def _check_output(f, buf, off, exp, where, what):
-    """buf: the whole flat output buffer (uint32), the result at word G + off; exp: the expected (rows, w) matrix."""
-    n, w = exp.size, exp.shape[1]
+def check_matrix(f, got, exp, where, what, ref="the reference"):
+    """got: an (rows, w) int32 tensor of u32 words on any device (a view is fine); exp(c0, c1): the expected columns [c0, c1) as
+    an int64 tensor of Montgomery words on got's device.  Column chunk by column chunk (bounded memory), every word must be
+    canonical and equal to exp; a failure names its row and column, the word, and where(row, col)."""
+    rows, w = got.shape
+    for c0, c1 in R.column_chunks(rows, w):
+        g = got[:, c0:c1].to(torch.int64) & 0xFFFFFFFF
+        want = exp(c0, c1)
+        for label, bad in (("not canonical", g >= f.P), (f"differ from {ref}", g != want)):
+            if bool(bad.any()):
+                i = int(torch.argmax(bad.view(-1).to(torch.uint8)))
+                row, col = divmod(i, c1 - c0)
+                val = int(g[row, col])
+                note = " (the poison: never written)" if val == POISON else ""
+                pytest.fail(f"{what}: {int(bad.sum())} of {rows * (c1 - c0)} words in columns {c0}-{c1 - 1} {label}; first at row "
+                            f"{row}, column {c0 + col}: 0x{val:08x}{note}, expected 0x{int(want[row, col]):08x}; {where(row, c0 + col)}")
+        del g, want
+
+
+def _check_output(f, buf, off, rows, w, exp, where, what):
+    """buf: the whole flat output buffer (int32 tensor), the (rows, w) result at word G + off; exp: the expected matrix, a numpy
+    array (the oracle's) or a function of a column range as check_matrix takes it (the reference's)."""
+    n = rows * w
     lo, hi = buf[:G + off], buf[G + off + n:]
-    for side, guard in (("before", lo[::-1]), ("after", hi)):
-        bad = guard != POISON
-        if bad.any():
-            k = int(np.argmax(bad))
+    for side, guard in (("before", lo.flip(0)), ("after", hi)):
+        bad = guard != -1
+        if bool(bad.any()):
+            k = int(torch.argmax(bad.to(torch.uint8)))
             pytest.fail(f"{what}: wrote outside its output, {k + 1} word(s) {side} it "
-                        f"(0x{int(guard[k]):08x}; {int(bad.sum())} guard words changed)")
-    body = buf[G + off:G + off + n]
-    for label, test in (("not canonical", lambda: body >= f.P), ("differs from the oracle", lambda: body != exp.ravel())):
-        bad = test()
-        if bad.any():
-            i = int(np.argmax(bad))
-            row, col = divmod(i, w)
-            val = int(body[i])
-            note = " (the poison: never written)" if val == POISON else ""
-            pytest.fail(f"{what}: {int(bad.sum())} of {n} words {label}; first at row {row}, column {col}: "
-                        f"0x{val:08x}{note}, expected 0x{int(exp.ravel()[i]):08x}; {where(row, col)}")
+                        f"(0x{int(guard[k]) & 0xFFFFFFFF:08x}; {int(bad.sum())} guard words changed)")
+    ref = "the reference"
+    if isinstance(exp, np.ndarray):
+        e, ref = exp, "the oracle"
+        exp = lambda c0, c1: torch.from_numpy(e[:, c0:c1].astype(np.int64)).to(buf.device)
+    check_matrix(f, buf[G + off:G + off + n].view(rows, w), exp, where, what, ref)
 
 
 def _lde_dev(gpu, f, x, in_off, out, out_off, h, w, added_bits, shift, bitrev_rows):
@@ -117,21 +146,20 @@ def _lde_dev(gpu, f, x, in_off, out, out_off, h, w, added_bits, shift, bitrev_ro
 
 
 def run_lde_checked(gpu, f, m, added_bits, shift, bitrev_rows=True, in_off=0, out_off=0, launches=None):
-    """p3gpu_coset_lde_batch_dev on m (Montgomery, (h, w)) with the input at word offset in_off and the output at word offset
-    out_off of poisoned, guarded buffers, after a dirty call on other data; checks the launch count (if given), the guards, that
-    every word is canonical and the result against the oracle.  Returns the (h << added_bits, w) output."""
+    """p3gpu_coset_lde_batch_dev on m (Montgomery, (h, w): a numpy matrix or a DeviceInput) with the input at word offset in_off
+    and the output at word offset out_off of poisoned, guarded buffers, after a dirty call on other data; checks the launch count
+    (if given), the guards, that every word is canonical and the result against the oracle (numpy input) or ntt_reference
+    (DeviceInput).  Returns the (h << added_bits, w) output as numpy for a numpy input."""
     h, w = m.shape
     log_h, H = h.bit_length() - 1, h << added_bits
-    gen = torch.Generator(device="cuda").manual_seed(h * w + added_bits)
-    xd = torch.randint(0, f.P, (h * w + in_off,), dtype=torch.int32, device="cuda", generator=gen)
-    od = torch.empty(H * w + 2 * G, dtype=torch.int32, device="cuda")
-    _lde_dev(gpu, f, xd, in_off, od, out_off, h, w, added_bits, shift, bitrev_rows)   # also builds the twiddle heaps
-    del xd, od
-    x, out = _device_copy(m, in_off), _poisoned(H * w)
+    x, out = torch.empty(h * w + in_off, dtype=torch.int32, device="cuda"), _poisoned(H * w)
+    x.random_(0, f.P, generator=torch.Generator(device="cuda").manual_seed(h * w + added_bits))
+    _lde_dev(gpu, f, x, in_off, out, out_off, h, w, added_bits, shift, bitrev_rows)   # also builds the twiddle heaps
+    _fill_input(f, x[in_off:], m)
+    out.fill_(-1)
     n0 = gpu.launches
     _lde_dev(gpu, f, x, in_off, out, out_off, h, w, added_bits, shift, bitrev_rows)
     n = gpu.launches - n0
-    got = out.cpu().numpy().view(np.uint32)
     what = f"{f.name} LDE 2^{log_h} x {w}, added_bits {added_bits}, {'bit-reversed' if bitrev_rows else 'natural'} rows"
     if launches is not None:
         assert n == launches, f"{what}: {n} launches instead of {launches}: the case left the path it pins"
@@ -143,9 +171,12 @@ def run_lde_checked(gpu, f, m, added_bits, shift, bitrev_rows=True, in_off=0, ou
             cb, pos = _brev(row & ((1 << added_bits) - 1), added_bits), _brev(row >> added_bits, log_h)
         return f"coset {_brev(cb, added_bits)} (block {cb}), " + _tiles(log_h, w, pos, col, n == 3)
 
-    exp = O.coset_lde_batch(f.id, m, added_bits, shift, bitrev_out=bitrev_rows)
-    _check_output(f, got, out_off, exp, where, what)
-    return got[G + out_off:G + out_off + H * w].reshape(H, w)
+    if isinstance(m, DeviceInput):
+        xm = x[in_off:].view(h, w)
+        _check_output(f, out, out_off, H, w, lambda c0, c1: R.coset_lde(f, xm[:, c0:c1], added_bits, shift, bitrev_rows), where, what)
+        return None
+    _check_output(f, out, out_off, H, w, O.coset_lde_batch(f.id, m, added_bits, shift, bitrev_out=bitrev_rows), where, what)
+    return out[G + out_off:G + out_off + H * w].cpu().numpy().view(np.uint32).reshape(H, w)
 
 
 _ORACLE_DFT = {_lib.DFT: lambda f, m, s: O.dft_batch(f.id, m), _lib.IDFT: lambda f, m, s: O.idft_batch(f.id, m),
@@ -159,27 +190,34 @@ def _dft_dev(gpu, f, kind, x, in_off, out, out_off, h, w, shift):
     _lib.check(gpu.L.p3gpu_dft_batch_dev(gpu.h, f.id, kind, x.data_ptr() + 4 * in_off, out.data_ptr() + 4 * (G + out_off), h, w, shift))
 
 
+_REFERENCE_DFT = {_lib.DFT: lambda f, m, s: R.dft(f, m), _lib.IDFT: lambda f, m, s: R.idft(f, m),
+                  _lib.COSET_DFT: R.coset_dft, _lib.COSET_IDFT: R.coset_idft}
+
+
 def run_dft_checked(gpu, f, kind, m, shift=0, in_off=0, out_off=0, launches=None):
-    """p3gpu_dft_batch_dev, checked the way run_lde_checked checks the LDE.  Returns the (h, w) output."""
+    """p3gpu_dft_batch_dev, checked the way run_lde_checked checks the LDE.  Returns the (h, w) output as numpy for a numpy
+    input."""
     h, w = m.shape
     log_h = h.bit_length() - 1
-    gen = torch.Generator(device="cuda").manual_seed(h * w + kind)
-    xd = torch.randint(0, f.P, (h * w + in_off,), dtype=torch.int32, device="cuda", generator=gen)
-    od = torch.empty(h * w + 2 * G, dtype=torch.int32, device="cuda")
-    _dft_dev(gpu, f, kind, xd, in_off, od, out_off, h, w, shift)
-    del xd, od
-    x, out = _device_copy(m, in_off), _poisoned(h * w)
+    x, out = torch.empty(h * w + in_off, dtype=torch.int32, device="cuda"), _poisoned(h * w)
+    x.random_(0, f.P, generator=torch.Generator(device="cuda").manual_seed(h * w + kind))
+    _dft_dev(gpu, f, kind, x, in_off, out, out_off, h, w, shift)
+    _fill_input(f, x[in_off:], m)
+    out.fill_(-1)
     n0 = gpu.launches
     _dft_dev(gpu, f, kind, x, in_off, out, out_off, h, w, shift)
     n = gpu.launches - n0
-    got = out.cpu().numpy().view(np.uint32)
     what = f"{f.name} {_KIND_NAME[kind]} 2^{log_h} x {w}"
     if launches is not None:
         assert n == launches, f"{what}: {n} launches instead of {launches}: the case left the path it pins"
     # natural-order output: row k is network position bitrev(k), written by the remapped last pass
     where = lambda row, col: _tiles(log_h, w, _brev(row, log_h), col, False)
-    _check_output(f, got, out_off, _ORACLE_DFT[kind](f, m, shift), where, what)
-    return got[G + out_off:G + out_off + h * w].reshape(h, w)
+    if isinstance(m, DeviceInput):
+        xm = x[in_off:].view(h, w)
+        _check_output(f, out, out_off, h, w, lambda c0, c1: _REFERENCE_DFT[kind](f, xm[:, c0:c1], shift), where, what)
+        return None
+    _check_output(f, out, out_off, h, w, _ORACLE_DFT[kind](f, m, shift), where, what)
+    return out[G + out_off:G + out_off + h * w].cpu().numpy().view(np.uint32).reshape(h, w)
 
 
 # ------------------------------------------------------------------------------------------ from the definition

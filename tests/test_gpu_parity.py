@@ -10,6 +10,8 @@ import torch
 
 from oracle import p3_oracle as O
 import fixture_replay as FR
+import ntt_reference as R
+from test_gpu_lde_paths import check_matrix
 
 import plonky3_b200 as P
 from plonky3_b200 import _lib
@@ -105,9 +107,8 @@ def test_large_heights_three_pass_plans(gpu, f, log_h, w):
     dft = Radix2DitParallel(f, gpu)
     m = O.random_matrix(f.id, 1 << log_h, w, seed=log_h)
     assert np.array_equal(dft.dft_batch(m), O.dft_batch(f.id, m))
-    if log_h <= 22:
-        got = dft.coset_lde_batch(dev(m), 1, f.generator).bit_reverse_rows()
-        assert np.array_equal(host(got), O.coset_lde_batch(f.id, m, 1, f.generator, bitrev_out=True))
+    got = dft.coset_lde_batch(dev(m), 1, f.generator).bit_reverse_rows()
+    assert np.array_equal(host(got), O.coset_lde_batch(f.id, m, 1, f.generator, bitrev_out=True))
 
 
 @pytest.mark.parametrize("f,log_h,w,added_bits,chunk", [(KoalaBear, 13, 52, 1, 16), (BabyBear, 12, 100, 2, 24), (KoalaBear, 21, 8, 1, 0), (BabyBear, 19, 12, 1, 8)])
@@ -124,21 +125,30 @@ def test_coset_lde_tiled_intermediates(gpu, f, log_h, w, added_bits, chunk, monk
     assert np.array_equal(host(got), O.coset_lde_batch(f.id, m, added_bits, f.generator, bitrev_out=True))
 
 
-@pytest.mark.parametrize("f,log_h,w", [(BabyBear, 21, 200), (KoalaBear, 22, 72)])
-def test_lde_many_small_tiles_pipelined_vs_cp_async_kernels(gpu, f, log_h, w, monkeypatch):
+@pytest.mark.parametrize("f,log_h,w,pipelined", [(BabyBear, 21, 200, 24), (KoalaBear, 22, 72, 12)], ids=["f0-21-200", "f1-22-72"])
+def test_lde_many_small_tiles_pipelined_vs_cp_async_kernels(gpu, f, log_h, w, pipelined, monkeypatch):
     # three-pass plans have 128/256-row tiles that are processed faster than HBM latency varies: the regime in which a consumer
-    # group of the pipelined kernel can run ahead of an in-flight load (mbarrier phase handling, csrc/ntt.cu).  Too large for the
-    # CPU oracle in a unit test, so the two independent kernel families (TMA pipeline vs cp.async tiles) must agree bit for bit.
-    # Each repeat writes into an output filled with 0xFFFFFFFF (never canonical): a tile whose store is dropped cannot pass on
-    # the previous repeat's result, which the caching allocator would otherwise hand back in the same block.
+    # group of the pipelined kernel can run ahead of an in-flight load (mbarrier phase handling, csrc/ntt.cu).  The cp.async
+    # kernel's result (six launches: the inverse and the forward network, three passes each) is checked word for word against
+    # the reference transform on the device, and the TMA pipeline's (six launches per 64-column chunk: 3 x 64 + 8 columns at
+    # 2^21 x 200, 64 + 8 at 2^22 x 72) must equal it bit for bit.  Each repeat writes into an output filled with 0xFFFFFFFF
+    # (never canonical): a tile whose store is dropped cannot pass on the previous repeat's result, which the caching allocator
+    # would otherwise hand back in the same block.
     x = torch.randint(0, f.P, (1 << log_h, w), device="cuda", dtype=torch.int32, generator=torch.Generator(device="cuda").manual_seed(log_h))
     monkeypatch.setenv("P3GPU_NTT_PIPE", "0")
+    gpu.coset_lde_batch(f.id, x, 1, f.generator)                                    # twiddle heaps
+    n0 = gpu.launches
     want = gpu.coset_lde_batch(f.id, x, 1, f.generator)
+    assert gpu.launches - n0 == 6, "cp.async kernel: the case left the path it pins"
+    check_matrix(f, want, lambda c0, c1: R.coset_lde(f, x[:, c0:c1], 1, f.generator), lambda row, col: f"coset {row >> log_h}",
+                 f"{f.name} LDE 2^{log_h} x {w} on the cp.async kernel")
     monkeypatch.setenv("P3GPU_NTT_PIPE", "1")
     for _ in range(3):
         got = torch.full_like(want, -1)
         gpu._use_torch_stream()
+        n0 = gpu.launches
         _lib.check(gpu.L.p3gpu_coset_lde_batch_dev(gpu.h, f.id, x.data_ptr(), x.shape[0], w, 1, f.generator, got.data_ptr(), 1))
+        assert gpu.launches - n0 == pipelined, "TMA pipeline: the case left the path it pins"
         assert torch.equal(got, want)
         del got
 

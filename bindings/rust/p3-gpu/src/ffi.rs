@@ -148,6 +148,12 @@ unsafe extern "C" {
                                    words: usize) -> i32;
     pub fn p3gpu_p2air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
                                             log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
+    pub fn p3gpu_blake3_air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
+                                                 log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
+    pub fn p3gpu_sha256_air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
+                                                 log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
+    pub fn p3gpu_p1air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
+                                            log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
 
     // streams, counters
     pub fn p3gpu_ctx_set_stream(ctx: *mut P3GpuCtx, cuda_stream: *mut c_void) -> i32;
@@ -183,11 +189,15 @@ unsafe extern "C" {
     pub fn p3gpu_blake3_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_blake3_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
                                          alpha: *const u32, d_quotient: *mut u32) -> i32;
+    pub fn p3gpu_blake3_air_generate_trace_cols_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, col0: usize,
+                                                    col1: usize, d_out: *mut u32) -> i32;
 
     // SHA-256 AIR (sha256-air): trace generation and quotient values, P3GPU_SHA256_AIR_COLS columns
     pub fn p3gpu_sha256_air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_sha256_air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, d_lde: *const u32, log_lde_height: c_uint, log_trace_height: c_uint,
                                          alpha: *const u32, d_quotient: *mut u32) -> i32;
+    pub fn p3gpu_sha256_air_generate_trace_cols_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_hashes: usize, col0: usize,
+                                                    col1: usize, d_out: *mut u32) -> i32;
 
     // Poseidon1 AIR (poseidon1-air, width 16): per-context constants (Poseidon1Constants::to_optimized's output, Montgomery words),
     // trace generation and quotient values
@@ -198,6 +208,8 @@ unsafe extern "C" {
     pub fn p3gpu_p1air_generate_trace_dev(ctx: *mut P3GpuCtx, field: c_int, d_inputs: *const u32, n_perms: usize, d_trace: *mut u32) -> i32;
     pub fn p3gpu_p1air_quotient_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_lde: *const u32, log_lde_height: c_uint,
                                     log_trace_height: c_uint, alpha: *const u32, d_quotient: *mut u32) -> i32;
+    pub fn p3gpu_p1air_generate_trace_cols_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, d_inputs: *const u32, n_perms: usize,
+                                               col0: usize, col1: usize, d_out: *mut u32) -> i32;
 
     // any AIR as a constraint program (symbolic expression DAG -> register program -> quotient kernel)
     pub fn p3gpu_air_program_create(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize, constraints: *const u32,

@@ -266,6 +266,11 @@ int32_t p3gpu_blake3_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uin
  * P3GPU_BLAKE3_AIR_COLS). */
 int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
                                       const uint32_t alpha[4], uint32_t *d_quotient);
+/* Columns [col0, col1) of the trace p3gpu_blake3_air_generate_trace_dev writes for the same inputs: d_out is the dense
+ * n_hashes x (col1 - col0) matrix, one rank's column block of a sharded prove, built without the full trace (d_out may be NULL iff
+ * col0 == col1).  P3GPU_EINVAL: as for the trace, or a window outside [0, P3GPU_BLAKE3_AIR_COLS]. */
+int32_t p3gpu_blake3_air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, size_t col0, size_t col1,
+                                                 uint32_t *d_out);
 
 /* ---- SHA-256 AIR (sha256-air/src), BabyBear and KoalaBear ------------------------------------------------------------------
  * One SHA-256 compression per row, rows independent (no next-row reads, no selectors, no public values), P3GPU_SHA256_AIR_COLS
@@ -280,6 +285,10 @@ int32_t p3gpu_sha256_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uin
  * P3GPU_SHA256_AIR_COLS). */
 int32_t p3gpu_sha256_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_lde, unsigned log_lde_height, unsigned log_trace_height,
                                       const uint32_t alpha[4], uint32_t *d_quotient);
+/* Columns [col0, col1) of the trace p3gpu_sha256_air_generate_trace_dev writes, with the contract of
+ * p3gpu_blake3_air_generate_trace_cols_dev (window inside [0, P3GPU_SHA256_AIR_COLS]). */
+int32_t p3gpu_sha256_air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, size_t col0, size_t col1,
+                                                 uint32_t *d_out);
 
 /* ---- Poseidon1 AIR: the AIR of prove_prime_field_31 -o poseidon-1-permutations (poseidon1-air/src), width 16 -------------------
  * VectorizedPoseidon1Air<F, 16, SBOX_DEGREE, SBOX_REGISTERS, 4, rounds_p, vector_len>: BabyBear x^7 with one S-box register,
@@ -304,6 +313,12 @@ int32_t p3gpu_p1air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t
  * BabyBear; the quotient is 2^(log_trace_height + 1) x 4).  P3GPU_ESTATE as for the trace. */
 int32_t p3gpu_p1air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_lde, unsigned log_lde_height,
                                  unsigned log_trace_height, const uint32_t alpha[4], uint32_t *d_quotient);
+/* Columns [col0, col1) of the (n_perms / vector_len) x (vector_len * columns) trace p3gpu_p1air_generate_trace_dev writes (n_perms
+ * a multiple of vector_len <= 32): d_out is the dense (n_perms / vector_len) x (col1 - col0) matrix; the window may cut a
+ * permutation (d_out may be NULL iff col0 == col1).  P3GPU_ESTATE as for the trace; P3GPU_EINVAL: as for the trace, or a window
+ * outside [0, vector_len * columns]. */
+int32_t p3gpu_p1air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms, size_t col0,
+                                            size_t col1, uint32_t *d_out);
 
 /* ---- any AIR as a constraint program (DESIGN.md section 4.7) ----------------------------------------------------------------
  * An AIR is described as the reference's symbolic expression DAG (air/src/symbolic/expression.rs): nodes in topological order
@@ -477,6 +492,24 @@ int32_t p3gpu_peer_exchange_dev(p3gpu_ctx *ctx, const p3gpu_peer_group *grp, uin
  * value at natural index bitrev(rank * R + m).  The concatenation over the ranks, un-bit-reversed, is p3gpu_p2air_quotient_dev's
  * output. */
 int32_t p3gpu_p2air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                         unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                         uint32_t *d_quotient_slice);
+
+/* The same for the Blake3, SHA-256 and Poseidon1 AIRs (either field), whose constraints read the local row only: the quotient
+ * values of MY row block after p3gpu_commit_sharded_dev with the same col_starts (log_lde_height = log_trace_height + 1, the
+ * commit's log_blowup 1, so the quotient domain is the LDE domain), read in place from grp->rows[rank] through a table of 8-column
+ * units, written to d_quotient_slice in BIT-REVERSED order as p3gpu_p2air_quotient_sharded_dev does.  col_starts[world] is the AIR's
+ * width.  P3GPU_EINVAL before any launch: a NULL argument, a bad peer group (world not a power of two <= 16), log_lde_height other
+ * than log_trace_height + 1, column blocks that do not cover the width or leave a segment bound that is neither a multiple of 8
+ * columns nor the width, alpha not canonical; P3GPU_EUNSUPPORTED: fewer than 1024 rows per rank, an unsupported field.
+ * Poseidon1: P3GPU_ESTATE as for p3gpu_p1air_quotient_dev. */
+int32_t p3gpu_blake3_air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                              unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                              uint32_t *d_quotient_slice);
+int32_t p3gpu_sha256_air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                              unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                              uint32_t *d_quotient_slice);
+int32_t p3gpu_p1air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
                                          unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
                                          uint32_t *d_quotient_slice);
 

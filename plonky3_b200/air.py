@@ -381,8 +381,23 @@ class SymbolicAir:
 class KernelAir(SymbolicAir):
     """A SymbolicAir whose prover runs the AIR's own hand-written kernels instead of a constraint program: no public values, no
     preprocessed columns, no CPU fallback.  A subclass names the AIR in `air_name` and launches its quotient kernel in
-    `_kernel_quotient`."""
+    `_kernel_quotient`; one that can be proved row-sharded (distributed.prove_sharded) also launches its sharded quotient kernel in
+    `_kernel_quotient_sharded`."""
     air_name = ""
+
+    @classmethod
+    def has_sharded_quotient(cls) -> bool:
+        """Whether the AIR has a quotient kernel for one rank's row block of the row-sharded commit."""
+        return cls._kernel_quotient_sharded is not KernelAir._kernel_quotient_sharded
+
+    def sharded_quotient_values(self, grp, log_lde_height: int, log_degree: int, alpha):
+        """The quotient values of `grp`'s row block after its sharded commit (distributed.PeerGroup.commit, log_blowup 1): (R, 4), R =
+        2^log_lde_height / world, in bit-reversed order: entry m is natural index bitrev(rank R + m) of the quotient domain."""
+        self._need_gpu("quotient evaluation")
+        return self._kernel_quotient_sharded(grp, int(log_lde_height), int(log_degree), alpha)
+
+    def _kernel_quotient_sharded(self, grp, log_lde_height: int, log_degree: int, alpha):
+        raise NotImplementedError(f"the {self.air_name} AIR has no sharded quotient kernel")
 
     def quotient_values(self, trace_lde_dev, log_degree: int, alpha, public_values=(), preprocessed_on_quotient_domain=None):
         """uni-stark/src/prover.rs:462-827 on the AIR's hand-written kernel: `trace_lde_dev` holds the trace on the quotient domain in

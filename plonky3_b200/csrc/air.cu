@@ -55,7 +55,6 @@ template <int F> __device__ __forceinline__ void air_internal_layer(u32 (&s)[AIR
 // WINDOW: only columns [col0, col1) of the vectorised trace (rows of vec_len permutations) are stored, as a dense
 // (n_perms / vec_len) x (col1 - col0) matrix — the column block one rank of the sharded prover commits.  Every permutation is
 // still evaluated (its later columns depend on all earlier rounds); only the stores are filtered.
-struct GenWindow { size_t col0, col1; unsigned vec_len; };
 
 // REG = 1 (BabyBear): a full round is written as its 16 registers, then its 16 posts; the partial rounds' (register, post_sbox)
 // pairs go through the tile 16 rounds (32 words per permutation) at a time.

@@ -190,20 +190,33 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const 
 // ---- hand-written AIR quotient kernels (keccak_air.cu, blake3_air.cu, poseidon1_air.cu) -----------------------------------
 template <int F>
 static int32_t hand_quotient_launch(p3gpu_ctx *ctx, const void *kern, u32 n_constraints, unsigned warps, size_t smem, u32 uses, const u32 *d_lde,
-                                    unsigned log_n, const u32 *alpha, u32 *d_q, const u32 *consts, unsigned lanes) {
+                                    unsigned log_n, const u32 *alpha, u32 *d_q, const u32 *consts, unsigned lanes, const AirHandShard *shard) {
     for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
     AirHandQArgs qa;
     std::vector<u32> zh, izh;
     qa.d = air_domain<F>(log_n + 1, log_n, uses, zh, izh);
     for (int j = 0; j < 2; j++) { qa.zh[j] = zh[j]; qa.izh[j] = izh[j]; }
     const std::vector<uint4> ap = air_alpha_table<F>(alpha, n_constraints);
+    std::vector<u64> units;
+    qa.units = nullptr; qa.n_units = 0; qa.row0 = 0; qa.rows = 0;
+    size_t points = (size_t)1 << qa.d.log_q;
+    if (shard) {
+        points = points / shard->world;
+        P3_TRY(air_shard_units(shard->world, shard->col_starts, points, shard->width, units));
+        qa.n_units = (u32)units.size(); qa.row0 = (u32)(shard->rank * points); qa.rows = (u32)points;
+        smem += units.size() * 8;
+    }
     void *tab = nullptr;
-    P3_TRY(ctx_scratch2(ctx, ap.size() * 16, &tab));
+    P3_TRY(ctx_scratch2(ctx, ap.size() * 16 + units.size() * 8, &tab));
     P3_CUDA(cudaMemcpyAsync(tab, ap.data(), ap.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
+    if (shard) {                                                     // the unit table behind the alpha table (16-byte entries)
+        qa.units = reinterpret_cast<const u64 *>(static_cast<uint4 *>(tab) + ap.size());
+        P3_CUDA(cudaMemcpyAsync(const_cast<u64 *>(qa.units), units.data(), units.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    }
     qa.lde = d_lde; qa.apow = static_cast<const uint4 *>(tab); qa.q = d_q;
     qa.consts = consts; qa.lanes = lanes;
     P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const size_t points = (size_t)1 << qa.d.log_q;                   // `lanes` lanes per point, persistent blocks
+    // `lanes` lanes per point, persistent blocks
     const size_t per_block = (size_t)warps * 32 / lanes;
     const unsigned grid = (unsigned)std::min<size_t>((size_t)ctx->sm_count, (points + per_block - 1) / per_block);
     void *args[] = {&qa};
@@ -214,16 +227,46 @@ static int32_t hand_quotient_launch(p3gpu_ctx *ctx, const void *kern, u32 n_cons
 
 int32_t air_hand_quotient(p3gpu_ctx *ctx, int field, const char *name, const void *kern_babybear, const void *kern_koalabear, u32 n_constraints,
                           unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q,
-                          const u32 *consts, unsigned lanes) {
+                          const u32 *consts, unsigned lanes, const AirHandShard *shard) {
     P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "%s AIR: unsupported field %d", name, field);
     const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
     P3_CHECK(log_n + 1 <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL,
              "%s AIR quotient: need log_trace_height %u + 1 <= log_lde_height %u <= %u", name, log_n, log_lde, two_adicity);
     P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % 4 == 0 && reinterpret_cast<uintptr_t>(d_q) % 4 == 0, P3GPU_EINVAL,
              "%s AIR quotient: misaligned buffer", name);
+    if (shard) {
+        // the quotient domain must be the LDE domain: then the 2N points are the 2N LDE rows, and rank g owns points bitrev(g R + m)
+        P3_CHECK(log_lde == log_n + 1, P3GPU_EINVAL, "%s AIR sharded quotient: the LDE must have 2N rows (log_blowup 1), not 2^%u over 2^%u", name,
+                 log_lde, log_n);
+        P3_CHECK(shard->world >= 1 && shard->world <= 16 && (shard->world & (shard->world - 1)) == 0 && shard->rank < shard->world, P3GPU_EINVAL,
+                 "%s AIR sharded quotient: world %u must be a power of two <= 16, rank %u below it", name, shard->world, shard->rank);
+        P3_CHECK(((size_t)2 << log_n) / shard->world >= 1024, P3GPU_EUNSUPPORTED,
+                 "%s AIR sharded quotient: %zu rows per rank (at least 1024, as the sharded commit)", name, ((size_t)2 << log_n) / shard->world);
+    }
     if (field == BABY_BEAR)
-        return hand_quotient_launch<BABY_BEAR>(ctx, kern_babybear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes);
-    return hand_quotient_launch<KOALA_BEAR>(ctx, kern_koalabear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes);
+        return hand_quotient_launch<BABY_BEAR>(ctx, kern_babybear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes, shard);
+    return hand_quotient_launch<KOALA_BEAR>(ctx, kern_koalabear, n_constraints, warps, smem, uses, d_lde, log_n, alpha, d_q, consts, lanes, shard);
+}
+
+int32_t air_shard_units(unsigned world, const size_t *col_starts, size_t rows, size_t width, std::vector<u64> &units) {
+    P3_CHECK(col_starts[world] == width, P3GPU_EINVAL, "the column blocks cover %zu columns, the trace has %zu", col_starts[world], width);
+    P3_CHECK(width < (1u << 16) && rows * width < (1ull << 48), P3GPU_EUNSUPPORTED, "row block of %zu x %zu: too large for the unit table", rows,
+             width);
+    std::vector<size_t> segs;
+    P3_TRY(shard_col_segments(world, col_starts, rows, segs));
+    units.assign((width + AIR_UNIT - 1) / AIR_UNIT, 0);
+    for (size_t s = 0; s < segs.size(); s += 3) {
+        const size_t c0 = segs[s], c1 = segs[s + 1], off = segs[s + 2];
+        P3_CHECK(c0 % AIR_UNIT == 0 && (c1 % AIR_UNIT == 0 || c1 == width), P3GPU_EINVAL,
+                 "column segment [%zu, %zu) does not start and end on a multiple of %u columns", c0, c1, AIR_UNIT);
+        for (size_t u = c0 / AIR_UNIT; u * AIR_UNIT < c1; u++) units[u] = air_unit_entry(off - c0, c1 - c0);
+    }
+    return P3GPU_OK;
+}
+
+int32_t air_check_window(const char *name, size_t col0, size_t col1, size_t width) {
+    P3_CHECK(col0 <= col1 && col1 <= width, P3GPU_EINVAL, "%s AIR: column window [%zu, %zu) outside the trace width %zu", name, col0, col1, width);
+    return P3GPU_OK;
 }
 
 }  // namespace p3

@@ -214,15 +214,54 @@ struct AirDomain {
 
 // Arguments of a hand-written AIR quotient kernel (keccak_air.cu, blake3_air.cu, poseidon1_air.cu), launched by air_hand_quotient
 // (air_program.cu): 2N points of GENERATOR * K, |K| = 2N, read from the first 2N rows of the committed bit-reversed LDE.
+// A SHARDED instance (blake3_air.cu, sha256_air.cu, poseidon1_air.cu) evaluates one rank's row block of the row-sharded commit
+// instead: block row m is memory row row0 + m of the bit-reversed LDE (natural index bitrev(row0 + m)), read in place through the
+// unit table (AirShardRow), and its quotient goes to q[m].
 struct AirHandQArgs {
-    const u32 *lde;            // bit-reversed LDE prefix, >= 2^d.log_q rows x the AIR's width
+    const u32 *lde;            // bit-reversed LDE prefix, >= 2^d.log_q rows x the AIR's width (SHARDED: the rank's row block)
     const uint4 *apow;         // alpha^(K - 1 - k), k < K
-    u32 *q;                    // 2^d.log_q x 4, natural order
+    u32 *q;                    // 2^d.log_q x 4, natural order (SHARDED: rows x 4, the block's bit-reversed slice)
     AirDomain d;
     u32 zh[2], izh[2];         // Z_H and 1 / Z_H by i mod 2
     const u32 *consts;         // the AIR's constants on the device, owned by the context (null for AIRs without any)
     u32 lanes;                 // lanes per point: 32 (one warp per point) or the AIR's vector length
+    // SHARDED only
+    const u64 *units;          // n_units entries of the unit table, one per 8 columns
+    u32 n_units, row0, rows;   // the block is memory rows [row0, row0 + rows)
 };
+
+// ---- address translation of a row block left chunk-major by p3gpu_commit_sharded_dev ------------------------------------
+// The block is a list of column segments, each a (rows x width) row-major matrix (shard_col_segments).  Every segment bound is a
+// multiple of AIR_UNIT columns or the trace's end, so each unit of AIR_UNIT columns [8u, 8u + 8) lies in one segment, and the unit
+// table holds, per unit, where that segment puts column c of block row m:  base + m * stride + c, with base = offset - first
+// column (>= 0: offset = rows * first column) in the low 48 bits and the segment's width (stride) in the high 16.  A load of 2 or 4
+// words at an even / 4-aligned column stays inside one unit, so vector loads need no splitting; they are as aligned as in the dense
+// matrix, because base and stride are multiples of 8 except in the single segment of a one-rank block (base 0, stride the width).
+// A column window of a generated trace (the trace generators' WINDOW instances): only columns [col0, col1) of the rows of vec_len
+// permutations (or of one hash per row, vec_len 1) are stored, as a dense rows x (col1 - col0) matrix.
+struct GenWindow { size_t col0, col1; unsigned vec_len; };
+
+constexpr u32 AIR_UNIT = 8;
+constexpr u64 AIR_UNIT_BASE_MASK = (1ull << 48) - 1;
+inline u64 air_unit_entry(u64 base, u64 stride) { return base | (stride << 48); }
+
+#ifdef __CUDACC__
+// the unit table into shared memory (before the block's __syncthreads)
+__device__ __forceinline__ void air_shard_table_load(const AirHandQArgs &a, u64 *tab) {
+    for (u32 t = threadIdx.x; t < a.n_units; t += blockDim.x) tab[t] = __ldg(a.units + t);
+}
+// block row m of a row block, read through the unit table in shared memory
+struct AirShardRow {
+    const u32 *blk;
+    const u64 *tab;
+    u32 m;
+    __device__ __forceinline__ const u32 *at(u32 c) const {
+        const u64 e = tab[c / AIR_UNIT];
+        return blk + (e & AIR_UNIT_BASE_MASK) + (size_t)m * (u32)(e >> 48) + c;
+    }
+    __device__ __forceinline__ u32 ld(u32 c) const { return __ldg(at(c)); }
+};
+#endif
 
 // selectors_on_coset (commit/src/domain.rs:321-361) at x_i = g * w_q^i, unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1.
 // zh = Z_H(x_i).  Shared by the constraint-program kernel and the hand-written Keccak AIR kernel (keccak_air.cu).
@@ -240,9 +279,9 @@ template <int F> __host__ __device__ __forceinline__ void air_selectors(const Ai
 template <int F> __device__ __forceinline__ u32 air_bxor(u32 x, u32 y) { return fp_sub<F>(fp_add<F>(x, y), fp_double<F>(mont_mul<F>(x, y))); }   // x + y - 2xy
 template <int F> __device__ __forceinline__ u32 air_bool(u32 x) { return mont_mul<F>(x, fp_sub<F>(x, Fp<F>::ONE)); }                         // x (x - 1)
 
-// The end of a warp's point i: reduce every lane's lazy accumulators, add them over the 32 lanes, multiply by 1 / Z_H(x_i) and let
-// lanes 0..3 store the four coefficients of q[i].
-template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQArgs &a, const u64 (&acc)[4], u32 i, unsigned lane) {
+// The end of a warp's point: reduce every lane's lazy accumulators, add them over the 32 lanes, multiply by 1 / Z_H(x_nat) and let
+// lanes 0..3 store the four coefficients of q[i].  1 / Z_H depends on the natural index nat's parity only: `odd` = nat & 1.
+template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQArgs &a, const u64 (&acc)[4], u32 i, unsigned lane, u32 odd) {
     u32 r[4];
 #pragma unroll
     for (int d = 0; d < 4; d++) r[d] = mont_redc<F>(acc[d]);
@@ -251,8 +290,14 @@ template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQAr
 #pragma unroll
         for (int d = 0; d < 4; d++) r[d] = fp_add<F>(r[d], __shfl_xor_sync(0xffffffffu, r[d], o));
     const u32 mine = lane == 0 ? r[0] : lane == 1 ? r[1] : lane == 2 ? r[2] : r[3];
-    if (lane < 4) a.q[4 * (size_t)i + lane] = mont_mul<F>(mine, (i & 1u) ? a.izh[1] : a.izh[0]);
+    if (lane < 4) a.q[4 * (size_t)i + lane] = mont_mul<F>(mine, odd ? a.izh[1] : a.izh[0]);
 }
+template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQArgs &a, const u64 (&acc)[4], u32 i, unsigned lane) {
+    air_warp_store<F>(a, acc, i, lane, i & 1u);
+}
+
+// The natural index of SHARDED block row m: bitrev(row0 + m) over the 2^log_q-point domain; its parity is the top bit of row0 + m.
+__device__ __forceinline__ u32 air_shard_odd(const AirHandQArgs &a, u32 m) { return ((a.row0 + m) >> (a.d.log_q - 1)) & 1u; }
 #endif
 
 // Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),

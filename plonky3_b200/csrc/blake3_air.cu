@@ -40,10 +40,12 @@ __device__ __forceinline__ u32 b3_rotr(u32 v, int r) { return __funnelshift_r(v,
 // 16-word state, the 16 message words and the 8 chaining-value words are all compile-time indexed); lane l owns bit l of every
 // 32-bit word.  A bit array is one 128-byte store per warp instruction (lane l writes column base + l); a state's eight limbs
 // are written by lanes 0..7.  Nothing is read but the row's 96-byte input.
+// WINDOW: only columns [win.col0, win.col1) are stored, as a dense n x (col1 - col0) matrix: the column block one rank of the sharded
+// prover commits.  The whole compression still runs; only the stores are filtered.
 constexpr int B3_GEN_WARPS = 8;
 
-template <int F>
-__global__ void __launch_bounds__(32 * B3_GEN_WARPS) blake3_air_generate_kernel(const u32 *inputs, size_t n, u32 *trace) {
+template <int F, bool WINDOW>
+__global__ void __launch_bounds__(32 * B3_GEN_WARPS) blake3_air_generate_kernel(const u32 *inputs, size_t n, u32 *trace, const GenWindow win) {
     const unsigned lane = threadIdx.x & 31u;
     const size_t row = (size_t)blockIdx.x * B3_GEN_WARPS + (threadIdx.x >> 5);
     if (row >= n) return;
@@ -60,12 +62,19 @@ __global__ void __launch_bounds__(32 * B3_GEN_WARPS) blake3_air_generate_kernel(
 #pragma unroll
     for (int j = 0; j < 4; j++) v[8 + j] = B3_IV[j];
     v[12] = (u32)row; v[13] = (u32)(row >> 32); v[14] = (u32)n; v[15] = 0u;
-    u32 *out = trace + row * B3_COLS;
-    auto bits = [&](int col, u32 w) { out[col + lane] = (w >> lane) & 1u ? ONE : 0u; };
+    u32 *out = WINDOW ? trace + row * (win.col1 - win.col0) : trace + row * B3_COLS;
+    auto put = [&](int c, u32 v) {
+        if constexpr (WINDOW) {
+            if ((size_t)c >= win.col0 && (size_t)c < win.col1) out[c - win.col0] = v;
+        } else {
+            out[c] = v;
+        }
+    };
+    auto bits = [&](int col, u32 w) { put(col + lane, (w >> lane) & 1u ? ONE : 0u); };
     auto limbs = [&](int col, u32 w0, u32 w1, u32 w2, u32 w3) {             // [4][2] limbs: lane j < 8 writes limb j
         const unsigned j = lane >> 1;
         const u32 w = j == 0 ? w0 : j == 1 ? w1 : j == 2 ? w2 : w3;
-        if (lane < 8) out[col + lane] = to_monty<F>(lane & 1u ? w >> 16 : w & 0xffffu);
+        if (lane < 8) put(col + lane, to_monty<F>(lane & 1u ? w >> 16 : w & 0xffffu));
     };
     auto save = [&](int base) {                                             // generation.rs save_state_to_trace
         limbs(base, v[0], v[1], v[2], v[3]);
@@ -129,6 +138,8 @@ __global__ void __launch_bounds__(32 * B3_GEN_WARPS) blake3_air_generate_kernel(
 //   - the 16 limb-level constraints of a quarter round (add3 / add2 / pack checks, two each) are warp-uniform values; lane j < 16
 //     keeps the j-th and folds it.
 // Each lane folds its constraints with air_qmac; the warp adds the 32 partial sums and multiplies by 1 / Z_H.
+// SHARDED: one rank's chunk-major row block (AirHandQArgs); every column address goes through the unit table behind the alpha
+// powers (air_program.cuh AirShardRow), the block's rows are the points, and the quotient lands in the block's slice.
 constexpr int BQ_WARPS = 16;
 constexpr size_t BQ_SMEM = (size_t)B3_CONSTRAINTS * 16;
 
@@ -136,13 +147,15 @@ constexpr size_t BQ_SMEM = (size_t)B3_CONSTRAINTS * 16;
 struct B3View { int r0, r1, r2, r3; };
 __device__ __forceinline__ B3View b3_state(int base) { return {base, base + B3_S_ROW1, base + B3_S_ROW2, base + B3_S_ROW3}; }
 
-template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_quotient_kernel(const AirHandQArgs a) {
+template <int F, bool SHARDED> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_quotient_kernel(const AirHandQArgs a) {
     extern __shared__ uint4 bq_sm[];
     const uint4 *ap = bq_sm;
+    u64 *units = reinterpret_cast<u64 *>(bq_sm + B3_CONSTRAINTS);
     for (int t = threadIdx.x; t < B3_CONSTRAINTS; t += blockDim.x) bq_sm[t] = __ldg(a.apow + t);
+    if constexpr (SHARDED) air_shard_table_load(a, units);
     __syncthreads();
     const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const u32 n_pts = 1u << a.d.log_q;
+    const u32 n_pts = SHARDED ? a.rows : 1u << a.d.log_q;
     const u32 T16 = to_monty<F>(1u << 16), T17 = fp_double<F>(T16), T32 = mont_mul<F>(T16, T16), T33 = fp_double<F>(T32);
     const u32 wpow = to_monty<F>(1u << (lane & 15u));                  // weight of this lane's bit in its 16-bit limb
     auto add = [](u32 x, u32 y) { return fp_add<F>(x, y); };
@@ -156,8 +169,12 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
         lo = __shfl_sync(0xffffffffu, s, 0); hi = __shfl_sync(0xffffffffu, s, 16);
     };
     for (u32 i = blockIdx.x * BQ_WARPS + warp; i < n_pts; i += gridDim.x * BQ_WARPS) {
-        const u32 *row = a.lde + (size_t)air_bitrev(i, a.d.log_q) * B3_COLS;
-        auto ld = [row](int c) { return __ldg(row + c); };
+        const u32 *row = SHARDED ? a.lde : a.lde + (size_t)air_bitrev(i, a.d.log_q) * B3_COLS;
+        const AirShardRow sr{a.lde, units, i};
+        auto ld = [row, sr](int c) {
+            if constexpr (SHARDED) return sr.ld((u32)c);
+            else return __ldg(row + c);
+        };
         u64 acc[4] = {0, 0, 0, 0};
         auto fold = [&](int k, u32 c) { air_qmac<F>(acc, c, ap[k]); };
         // the initialisation inputs are boolean (k 0..895: column k)
@@ -278,29 +295,55 @@ template <int F> __global__ void __launch_bounds__(32 * BQ_WARPS, 1) blake3_air_
             if (lane < 8) fold(k + lane, mine);
             else if (lane >= 16 && lane < 24) fold(k + 136 + 34 * ((lane - 16) >> 1) + 32 + (lane & 1u), mine);
         }
-        air_warp_store<F>(a, acc, i, lane);
+        if constexpr (SHARDED) air_warp_store<F>(a, acc, i, lane, air_shard_odd(a, i));
+        else air_warp_store<F>(a, acc, i, lane);
     }
 }
 
 // ---- host entry points ----------------------------------------------------------------------------------------------------
-template <int F> static int32_t b3_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n, u32 *d_trace) {
-    blake3_air_generate_kernel<F><<<(unsigned)((n + B3_GEN_WARPS - 1) / B3_GEN_WARPS), 32 * B3_GEN_WARPS, 0, ctx->stream>>>(d_inputs, n,
-                                                                                                                      d_trace);
+template <int F, bool WINDOW> static int32_t b3_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n, u32 *d_trace, const GenWindow &win) {
+    blake3_air_generate_kernel<F, WINDOW><<<(unsigned)((n + B3_GEN_WARPS - 1) / B3_GEN_WARPS), 32 * B3_GEN_WARPS, 0, ctx->stream>>>(d_inputs, n,
+                                                                                                                             d_trace, win);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
 
-int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace) {
+static int32_t b3_check(int field, size_t n_hashes) {
     P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "Blake3 AIR: unsupported field %d", field);
     P3_CHECK(n_hashes > 0 && (n_hashes & (n_hashes - 1)) == 0 && n_hashes <= ((size_t)1 << 32), P3GPU_EINVAL,
              "Blake3 AIR: %zu hashes (need a power of two, at most 2^32)", n_hashes);
-    return field == BABY_BEAR ? b3_generate<BABY_BEAR>(ctx, d_inputs, n_hashes, d_trace) : b3_generate<KOALA_BEAR>(ctx, d_inputs, n_hashes, d_trace);
+    return P3GPU_OK;
+}
+
+int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace) {
+    P3_TRY(b3_check(field, n_hashes));
+    const GenWindow win{};
+    return field == BABY_BEAR ? b3_generate<BABY_BEAR, false>(ctx, d_inputs, n_hashes, d_trace, win)
+                              : b3_generate<KOALA_BEAR, false>(ctx, d_inputs, n_hashes, d_trace, win);
+}
+
+int32_t blake3_air_generate_cols(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, size_t col0, size_t col1, u32 *d_out) {
+    P3_TRY(b3_check(field, n_hashes));
+    P3_TRY(air_check_window("Blake3", col0, col1, B3_COLS));
+    if (col0 == col1) return P3GPU_OK;
+    const GenWindow win{col0, col1, 1};
+    return field == BABY_BEAR ? b3_generate<BABY_BEAR, true>(ctx, d_inputs, n_hashes, d_out, win)
+                              : b3_generate<KOALA_BEAR, true>(ctx, d_inputs, n_hashes, d_out, win);
 }
 
 int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    return air_hand_quotient(ctx, field, "Blake3", (const void *)blake3_air_quotient_kernel<BABY_BEAR>, (const void *)blake3_air_quotient_kernel<KOALA_BEAR>,
-                             B3_CONSTRAINTS, BQ_WARPS, BQ_SMEM, 0, d_lde, log_lde, log_n, alpha, d_q);
+    return air_hand_quotient(ctx, field, "Blake3", (const void *)blake3_air_quotient_kernel<BABY_BEAR, false>,
+                             (const void *)blake3_air_quotient_kernel<KOALA_BEAR, false>, B3_CONSTRAINTS, BQ_WARPS, BQ_SMEM, 0, d_lde, log_lde, log_n,
+                             alpha, d_q);
+}
+
+int32_t blake3_air_quotient_sharded(p3gpu_ctx *ctx, int field, const AirHandShard &shard, const u32 *d_block, unsigned log_lde, unsigned log_n,
+                                    const u32 *alpha, u32 *d_q) {
+    const AirHandShard sh{shard.world, shard.rank, shard.col_starts, B3_COLS};
+    return air_hand_quotient(ctx, field, "Blake3", (const void *)blake3_air_quotient_kernel<BABY_BEAR, true>,
+                             (const void *)blake3_air_quotient_kernel<KOALA_BEAR, true>, B3_CONSTRAINTS, BQ_WARPS, BQ_SMEM, 0, d_block, log_lde,
+                             log_n, alpha, d_q, nullptr, 32, &sh);
 }
 
 }  // namespace p3

@@ -529,6 +529,14 @@ int32_t p3gpu_blake3_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t 
     P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
     return blake3_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
 }
+int32_t p3gpu_blake3_air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, size_t col0, size_t col1,
+                                                 uint32_t *d_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && (d_out || col0 == col1), P3GPU_EINVAL, "null argument");
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 4 == 0 && reinterpret_cast<uintptr_t>(d_out) % 4 == 0, P3GPU_EINVAL,
+             "Blake3 AIR trace: misaligned buffer");
+    return blake3_air_generate_cols(ctx, field, d_inputs, n_hashes, col0, col1, d_out);
+}
 
 // ---- SHA-256 AIR: trace generation + quotient (sha256_air.cu) -----------------------------------------
 int32_t p3gpu_sha256_air_generate_trace_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, uint32_t *d_trace) {
@@ -543,6 +551,14 @@ int32_t p3gpu_sha256_air_quotient_dev(p3gpu_ctx *ctx, int field, const uint32_t 
     P3_ENTER(ctx);
     P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
     return sha256_air_quotient(ctx, field, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+int32_t p3gpu_sha256_air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_inputs, size_t n_hashes, size_t col0, size_t col1,
+                                                 uint32_t *d_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && (d_out || col0 == col1), P3GPU_EINVAL, "null argument");
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 4 == 0 && reinterpret_cast<uintptr_t>(d_out) % 4 == 0, P3GPU_EINVAL,
+             "SHA-256 AIR trace: misaligned buffer");
+    return sha256_air_generate_cols(ctx, field, d_inputs, n_hashes, col0, col1, d_out);
 }
 
 // ---- Poseidon1 AIR: constants, trace generation + quotient (poseidon1_air.cu) -------------------------------
@@ -566,6 +582,12 @@ int32_t p3gpu_p1air_quotient_dev(p3gpu_ctx *ctx, int field, int vector_len, cons
     P3_ENTER(ctx);
     P3_CHECK(d_lde && alpha && d_quotient, P3GPU_EINVAL, "null argument");
     return p1air_quotient(ctx, field, vector_len, d_lde, log_lde_height, log_trace_height, alpha, d_quotient);
+}
+int32_t p3gpu_p1air_generate_trace_cols_dev(p3gpu_ctx *ctx, int field, int vector_len, const uint32_t *d_inputs, size_t n_perms, size_t col0,
+                                            size_t col1, uint32_t *d_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_inputs && (d_out || col0 == col1), P3GPU_EINVAL, "null argument");
+    return p1air_generate_cols(ctx, field, vector_len, d_inputs, n_perms, col0, col1, d_out);
 }
 
 // ---- any AIR as a constraint program (air_program.cu) -------------------------------------------------
@@ -775,6 +797,38 @@ int32_t p3gpu_p2air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_l
     P3_CHECK(col_starts && alpha && d_quotient_slice, P3GPU_EINVAL, "null argument");
     return air_quotient_sharded(ctx, field, vector_len, grp->world, grp->rank, grp->rows[grp->rank], col_starts, log_lde_height, log_trace_height,
                                 alpha, d_quotient_slice);
+}
+
+// the Blake3, SHA-256 and Poseidon1 AIRs' sharded quotients: air_hand_quotient's sharded mode on my row block
+static int32_t hand_shard(const p3gpu_peer_group *grp, const size_t *col_starts, const uint32_t *alpha, const uint32_t *d_q, AirHandShard &sh) {
+    P3_TRY(check_group(grp, true));
+    P3_CHECK(col_starts && alpha && d_q, P3GPU_EINVAL, "null argument");
+    sh = AirHandShard{grp->world, grp->rank, col_starts, 0};
+    return P3GPU_OK;
+}
+int32_t p3gpu_blake3_air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                              unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                              uint32_t *d_quotient_slice) {
+    P3_ENTER(ctx);
+    AirHandShard sh;
+    P3_TRY(hand_shard(grp, col_starts, alpha, d_quotient_slice, sh));
+    return blake3_air_quotient_sharded(ctx, field, sh, grp->rows[grp->rank], log_lde_height, log_trace_height, alpha, d_quotient_slice);
+}
+int32_t p3gpu_sha256_air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                              unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                              uint32_t *d_quotient_slice) {
+    P3_ENTER(ctx);
+    AirHandShard sh;
+    P3_TRY(hand_shard(grp, col_starts, alpha, d_quotient_slice, sh));
+    return sha256_air_quotient_sharded(ctx, field, sh, grp->rows[grp->rank], log_lde_height, log_trace_height, alpha, d_quotient_slice);
+}
+int32_t p3gpu_p1air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_len, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                         unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
+                                         uint32_t *d_quotient_slice) {
+    P3_ENTER(ctx);
+    AirHandShard sh;
+    P3_TRY(hand_shard(grp, col_starts, alpha, d_quotient_slice, sh));
+    return p1air_quotient_sharded(ctx, field, vector_len, sh, grp->rows[grp->rank], log_lde_height, log_trace_height, alpha, d_quotient_slice);
 }
 
 // TwoAdicFriPcs::commit of ONE trace whose columns are sharded over the ranks, bit-identical to the single-GPU commitment.

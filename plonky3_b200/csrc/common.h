@@ -173,9 +173,18 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, cons
 // the committed bit-reversed LDE: checks the field, the domain, the alignment and alpha (messages name the AIR), builds the domain
 // and the alpha^(K - 1 - k) table (scratch2), then launches `kern_<field>` on min(SMs, 2N lanes / (32 warps)) blocks of `warps`
 // warps.  `lanes`: lanes per point (32: one warp per point); `consts`: the AIR's device constants, handed to the kernel.
+// `shard` (sharded mode, the kernels' SHARDED instances): d_lde is rank `rank`'s row block of the row-sharded commit of a `width`-column
+// trace over `world` ranks with column blocks `col_starts` (log_lde = log_n + 1, R = 2N / world rows), d_q its R x 4 bit-reversed
+// quotient slice; the unit table (air_program.cuh AirShardRow) goes behind the alpha table, `smem` grows by its size.
+struct AirHandShard { unsigned world, rank; const size_t *col_starts; size_t width; };
 int32_t air_hand_quotient(p3gpu_ctx *ctx, int field, const char *name, const void *kern_babybear, const void *kern_koalabear, u32 n_constraints,
                           unsigned warps, size_t smem, u32 uses, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q,
-                          const u32 *consts = nullptr, unsigned lanes = 32);
+                          const u32 *consts = nullptr, unsigned lanes = 32, const AirHandShard *shard = nullptr);
+// The unit table of a row block (air_program.cuh AirShardRow): one entry per 8 columns of the `width`-column trace, from
+// shard_col_segments; EINVAL when a segment bound is neither a multiple of 8 columns nor the trace's end.
+int32_t air_shard_units(unsigned world, const size_t *col_starts, size_t rows, size_t width, std::vector<u64> &units);
+// A trace generator's column window [col0, col1) of a `width`-column trace: EINVAL unless col0 <= col1 <= width
+int32_t air_check_window(const char *name, size_t col0, size_t col1, size_t width);
 
 // keccak_air.cu: Keccak-f AIR trace generation / quotient
 size_t keccak_air_height(size_t n_hashes);
@@ -185,10 +194,16 @@ int32_t keccak_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigne
 // blake3_air.cu: Blake3 AIR trace generation / quotient
 int32_t blake3_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
 int32_t blake3_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+int32_t blake3_air_generate_cols(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, size_t col0, size_t col1, u32 *d_out);
+int32_t blake3_air_quotient_sharded(p3gpu_ctx *ctx, int field, const AirHandShard &shard, const u32 *d_block, unsigned log_lde, unsigned log_n,
+                                    const u32 *alpha, u32 *d_q);
 
 // sha256_air.cu: SHA-256 AIR trace generation / quotient
 int32_t sha256_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace);
 int32_t sha256_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+int32_t sha256_air_generate_cols(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, size_t col0, size_t col1, u32 *d_out);
+int32_t sha256_air_quotient_sharded(p3gpu_ctx *ctx, int field, const AirHandShard &shard, const u32 *d_block, unsigned log_lde, unsigned log_n,
+                                    const u32 *alpha, u32 *d_q);
 
 // poseidon1_air.cu: Poseidon1 AIR constants (per context), trace generation / quotient
 size_t p1air_columns(int field, int rounds_p);          // 0 for an unknown field
@@ -197,6 +212,9 @@ int32_t p1air_set_constants(p3gpu_ctx *ctx, int field, const u32 *initial_full, 
                             int rounds_p);
 int32_t p1air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_perms, u32 *d_trace);
 int32_t p1air_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q);
+int32_t p1air_generate_cols(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_inputs, size_t n_perms, size_t col0, size_t col1, u32 *d_out);
+int32_t p1air_quotient_sharded(p3gpu_ctx *ctx, int field, int vector_len, const AirHandShard &shard, const u32 *d_block, unsigned log_lde,
+                               unsigned log_n, const u32 *alpha, u32 *d_q);
 
 // challenger.cu / query.cu: transcript + query-phase gathers of the prove driver (SURVEY 8f rank 4, N1)
 int32_t challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out);

@@ -86,10 +86,14 @@ template <int F> __device__ __forceinline__ void p1_sparse(u32 (&s)[P1_W], u32 s
 // A warp's 32 permutations emit their columns in lockstep; each value goes to the warp's [32][33] tile, and every 32 columns the
 // tile is written back with consecutive lanes on consecutive words of one permutation's columns: a 128-byte row segment per store
 // instruction, instead of 32 rows 4 bytes each.
+// WINDOW: only columns [win.col0, win.col1) of the vectorised trace (rows of win.vec_len permutations) are stored, as a dense
+// (n_perms / vec_len) x (col1 - col0) matrix: the column block one rank of the sharded prover commits.  Every permutation is still
+// evaluated; only the stores are filtered.
 constexpr int P1G_WARPS = 8;
 
-template <int F>
-__global__ void __launch_bounds__(32 * P1G_WARPS, 2) p1air_generate_kernel(const u32 *inputs, size_t n_perms, u32 *trace, const u32 *kdev) {
+template <int F, bool WINDOW>
+__global__ void __launch_bounds__(32 * P1G_WARPS, 2) p1air_generate_kernel(const u32 *inputs, size_t n_perms, u32 *trace, const u32 *kdev,
+                                                                           const GenWindow win) {
     constexpr int REG = p1_reg<F>();
     extern __shared__ u32 p1g_sm[];
     const int rp = (int)__ldg(kdev);
@@ -114,7 +118,12 @@ __global__ void __launch_bounds__(32 * P1G_WARPS, 2) p1air_generate_kernel(const
             __syncwarp();
             for (unsigned idx = lane; idx < n_warp * n; idx += 32) {
                 const unsigned perm = idx / n, i = idx - perm * n;
-                trace[(p0 + perm) * cols + off + i] = tile[perm * 33 + i];
+                if constexpr (WINDOW) {
+                    const size_t pp = p0 + perm, c = (pp % win.vec_len) * cols + off + i;
+                    if (c >= win.col0 && c < win.col1) trace[(pp / win.vec_len) * (win.col1 - win.col0) + (c - win.col0)] = tile[perm * 33 + i];
+                } else {
+                    trace[(p0 + perm) * cols + off + i] = tile[perm * 33 + i];
+                }
             }
             __syncwarp();
             off += n;
@@ -173,9 +182,12 @@ __global__ void __launch_bounds__(32 * P1G_WARPS, 2) p1air_generate_kernel(const
 // on the committed values and folds its constraints with air_qmac against the alpha-power table in shared memory, laid out one
 // padded row per permutation (stride nc + 1 entries: the 8 permutations of a quarter warp hit disjoint banks).  The row's lanes add
 // their sums with a shuffle reduction; lane 0 multiplies by 1 / Z_H and stores q[i].
+// SHARDED: one rank's chunk-major row block (AirHandQArgs); every load goes through the unit table behind the constants
+// (air_program.cuh AirShardRow).  A 2- or 4-word load never leaves its 8-column unit, so a permutation that starts in the middle of
+// a unit or a chunk (BabyBear: 298 columns) needs no split loads.
 constexpr int P1Q_WARPS = 16;
 
-template <int F> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quotient_kernel(const AirHandQArgs a) {
+template <int F, bool SHARDED> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quotient_kernel(const AirHandQArgs a) {
     constexpr int REG = p1_reg<F>();
     constexpr int VEC = REG ? 2 : 4;                                    // words per load
     extern __shared__ uint4 p1q_sm[];
@@ -189,13 +201,15 @@ template <int F> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quot
         ap[v * (nc + 1) + (t - v * nc)] = __ldg(a.apow + t);
     }
     for (int t = threadIdx.x; t < p1_words(rp); t += blockDim.x) k[t] = __ldg(a.consts + P1_HDR + t);
+    u64 *units = reinterpret_cast<u64 *>(k + ((p1_words(rp) + 1) & ~1));
+    if constexpr (SHARDED) air_shard_table_load(a, units);
     __syncthreads();
     u32 c[P1_W];
 #pragma unroll
     for (int i = 0; i < P1_W; i++) c[i] = k[P1_CIRC + i];
     const unsigned lane = threadIdx.x & 31u;
     const unsigned lshift = __ffs(lanes) - 1;
-    const size_t total = (size_t)1 << (a.d.log_q + lshift);
+    const size_t total = SHARDED ? (size_t)a.rows << lshift : (size_t)1 << (a.d.log_q + lshift);
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     // whole warps iterate together (the shuffles need every lane); lanes past the end only take part in them
     for (size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x; t - lane < total; t += stride) {
@@ -204,11 +218,26 @@ template <int F> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quot
         const int v = (int)(t & (lanes - 1));
         u64 acc[4] = {0, 0, 0, 0};
         if (live) {
-            const u32 *row = a.lde + ((size_t)air_bitrev(i, a.d.log_q) * lanes + v) * cols;
+            const u32 *row = SHARDED ? a.lde : a.lde + ((size_t)air_bitrev(i, a.d.log_q) * lanes + v) * cols;
+            const AirShardRow sr{a.lde, units, i};
+            const u32 pc = (u32)(v * cols);                         // SHARDED: the permutation's first column
             const uint4 *apv = ap + v * (nc + 1);
             auto fold = [&](u32 x) { air_qmac<F>(acc, x, *apv++); };
+            auto ld1 = [&](int off) {
+                if constexpr (SHARDED) return sr.ld(pc + off);
+                else return __ldg(row + off);
+            };
             auto ld16 = [&](u32 (&dst)[P1_W], int off) {
-                if constexpr (VEC == 4) {
+                if constexpr (SHARDED && VEC == 4) {
+#pragma unroll
+                    for (int x = 0; x < 4; x++) {
+                        const uint4 w = __ldg(reinterpret_cast<const uint4 *>(sr.at(pc + off + 4 * x)));
+                        dst[4 * x] = w.x; dst[4 * x + 1] = w.y; dst[4 * x + 2] = w.z; dst[4 * x + 3] = w.w;
+                    }
+                } else if constexpr (SHARDED) {
+#pragma unroll
+                    for (int x = 0; x < 8; x++) { const uint2 w = __ldg(reinterpret_cast<const uint2 *>(sr.at(pc + off + 2 * x))); dst[2 * x] = w.x; dst[2 * x + 1] = w.y; }
+                } else if constexpr (VEC == 4) {
                     const uint4 *p4 = reinterpret_cast<const uint4 *>(row + off);
 #pragma unroll
                     for (int x = 0; x < 4; x++) { const uint4 w = __ldg(p4 + x); dst[4 * x] = w.x; dst[4 * x + 1] = w.y; dst[4 * x + 2] = w.z; dst[4 * x + 3] = w.w; }
@@ -245,11 +274,11 @@ template <int F> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quot
                 const u32 tt = s[0], t3 = p1_cube<F>(tt);
                 u32 o = t3;
                 if constexpr (REG) {
-                    const u32 x3 = __ldg(row + off);
+                    const u32 x3 = ld1(off);
                     fold(fp_sub<F>(x3, t3));
                     o = mont_mul<F>(mont_mul<F>(x3, x3), tt);
                 }
-                const u32 post = __ldg(row + off + REG);
+                const u32 post = ld1(off + REG);
                 fold(fp_sub<F>(o, post));
                 const u32 s0 = r < rp - 1 ? fp_add<F>(post, k[p1_prc(rp) + r]) : post;
                 p1_sparse<F>(s, s0, k + P1_SFR + P1_W * r, k + p1_v(rp) + P1_W * r);
@@ -264,7 +293,7 @@ template <int F> __global__ void __launch_bounds__(32 * P1Q_WARPS, 1) p1air_quot
 #pragma unroll
             for (int d = 0; d < 4; d++) rr[d] = fp_add<F>(rr[d], __shfl_xor_sync(0xffffffffu, rr[d], o));
         if (live && v == 0) {
-            const u32 z = (i & 1u) ? a.izh[1] : a.izh[0];
+            const u32 z = (SHARDED ? air_shard_odd(a, i) : i & 1u) ? a.izh[1] : a.izh[0];
 #pragma unroll
             for (int d = 0; d < 4; d++) a.q[4 * (size_t)i + d] = mont_mul<F>(rr[d], z);
         }
@@ -328,16 +357,16 @@ static int32_t p1_state(p3gpu_ctx *ctx, int field) {
     return P3GPU_OK;
 }
 
-template <int F> static int32_t p1_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n_perms, u32 *d_trace) {
+template <int F, bool WINDOW> static int32_t p1_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n_perms, u32 *d_trace, const GenWindow &win) {
     const int nk = p1_words(ctx->p1_rounds_p);
     const size_t smem = (size_t)((nk + 3) & ~3) * 4 + (size_t)P1G_WARPS * 32 * 33 * 4;
-    auto kern = p1air_generate_kernel<F>;
+    auto kern = p1air_generate_kernel<F, WINDOW>;
     P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
     P3_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32 * P1G_WARPS, smem));
     const size_t blocks = (n_perms + 32 * P1G_WARPS - 1) / (32 * P1G_WARPS);
     const unsigned grid = (unsigned)std::min<size_t>(blocks, (size_t)std::max(per_sm, 1) * ctx->sm_count);
-    kern<<<grid, 32 * P1G_WARPS, smem, ctx->stream>>>(d_inputs, n_perms, d_trace, ctx->p1_consts);
+    kern<<<grid, 32 * P1G_WARPS, smem, ctx->stream>>>(d_inputs, n_perms, d_trace, ctx->p1_consts, win);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
@@ -348,10 +377,26 @@ int32_t p1air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_
     P3_CHECK(n_perms > 0, P3GPU_EINVAL, "Poseidon1 AIR: no permutations");
     P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 16 == 0 && reinterpret_cast<uintptr_t>(d_trace) % 4 == 0, P3GPU_EINVAL,
              "Poseidon1 AIR trace: inputs must be 16-byte aligned, the trace 4-byte aligned");
-    return field == BABY_BEAR ? p1_generate<BABY_BEAR>(ctx, d_inputs, n_perms, d_trace) : p1_generate<KOALA_BEAR>(ctx, d_inputs, n_perms, d_trace);
+    const GenWindow win{};
+    return field == BABY_BEAR ? p1_generate<BABY_BEAR, false>(ctx, d_inputs, n_perms, d_trace, win)
+                              : p1_generate<KOALA_BEAR, false>(ctx, d_inputs, n_perms, d_trace, win);
 }
 
-int32_t p1air_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
+int32_t p1air_generate_cols(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_inputs, size_t n_perms, size_t col0, size_t col1, u32 *d_out) {
+    P3_TRY(p1_state(ctx, field));
+    P3_CHECK(vector_len >= 1 && vector_len <= 32 && n_perms > 0 && n_perms % (size_t)vector_len == 0, P3GPU_EINVAL,
+             "Poseidon1 AIR: %zu permutations do not fill rows of %d", n_perms, vector_len);
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_inputs) % 16 == 0 && reinterpret_cast<uintptr_t>(d_out) % 4 == 0, P3GPU_EINVAL,
+             "Poseidon1 AIR trace: inputs must be 16-byte aligned, the trace 4-byte aligned");
+    P3_TRY(air_check_window("Poseidon1", col0, col1, (size_t)vector_len * p1air_columns(field, ctx->p1_rounds_p)));
+    if (col0 == col1) return P3GPU_OK;
+    const GenWindow win{col0, col1, (unsigned)vector_len};
+    return field == BABY_BEAR ? p1_generate<BABY_BEAR, true>(ctx, d_inputs, n_perms, d_out, win)
+                              : p1_generate<KOALA_BEAR, true>(ctx, d_inputs, n_perms, d_out, win);
+}
+
+static int32_t p1_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q,
+                           const AirHandShard *shard) {
     P3_TRY(p1_state(ctx, field));
     P3_CHECK(vector_len >= 1 && vector_len <= 32 && (vector_len & (vector_len - 1)) == 0, P3GPU_EINVAL,
              "Poseidon1 AIR quotient: vector length %d must be a power of two <= 32", vector_len);
@@ -359,9 +404,26 @@ int32_t p1air_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_l
     const unsigned lde_align = reg ? 8 : 16;                          // the kernel's load width
     P3_CHECK(reinterpret_cast<uintptr_t>(d_lde) % lde_align == 0, P3GPU_EINVAL, "Poseidon1 AIR quotient: the LDE must be %u-byte aligned", lde_align);
     const int nc = p1_constraints(reg, rp);
-    const size_t smem = (size_t)vector_len * (nc + 1) * 16 + (size_t)p1_words(rp) * 4;
-    return air_hand_quotient(ctx, field, "Poseidon1", (const void *)p1air_quotient_kernel<BABY_BEAR>, (const void *)p1air_quotient_kernel<KOALA_BEAR>,
-                             (u32)(nc * vector_len), P1Q_WARPS, smem, 0, d_lde, log_lde, log_n, alpha, d_q, ctx->p1_consts, (unsigned)vector_len);
+    if (!shard) {
+        const size_t smem = (size_t)vector_len * (nc + 1) * 16 + (size_t)p1_words(rp) * 4;
+        return air_hand_quotient(ctx, field, "Poseidon1", (const void *)p1air_quotient_kernel<BABY_BEAR, false>,
+                                 (const void *)p1air_quotient_kernel<KOALA_BEAR, false>, (u32)(nc * vector_len), P1Q_WARPS, smem, 0, d_lde, log_lde,
+                                 log_n, alpha, d_q, ctx->p1_consts, (unsigned)vector_len);
+    }
+    const size_t smem = (size_t)vector_len * (nc + 1) * 16 + (size_t)((p1_words(rp) + 1) & ~1) * 4;   // the unit table 8-byte aligned behind
+    const AirHandShard sh{shard->world, shard->rank, shard->col_starts, (size_t)vector_len * p1_cols(reg, rp)};
+    return air_hand_quotient(ctx, field, "Poseidon1", (const void *)p1air_quotient_kernel<BABY_BEAR, true>,
+                             (const void *)p1air_quotient_kernel<KOALA_BEAR, true>, (u32)(nc * vector_len), P1Q_WARPS, smem, 0, d_lde, log_lde, log_n,
+                             alpha, d_q, ctx->p1_consts, (unsigned)vector_len, &sh);
+}
+
+int32_t p1air_quotient(p3gpu_ctx *ctx, int field, int vector_len, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
+    return p1_quotient(ctx, field, vector_len, d_lde, log_lde, log_n, alpha, d_q, nullptr);
+}
+
+int32_t p1air_quotient_sharded(p3gpu_ctx *ctx, int field, int vector_len, const AirHandShard &shard, const u32 *d_block, unsigned log_lde,
+                               unsigned log_n, const u32 *alpha, u32 *d_q) {
+    return p1_quotient(ctx, field, vector_len, d_block, log_lde, log_n, alpha, d_q, &shard);
 }
 
 }  // namespace p3

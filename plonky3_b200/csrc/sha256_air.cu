@@ -41,24 +41,33 @@ __device__ __forceinline__ u32 sh_rotr(u32 v, int r) { return __funnelshift_r(v,
 // schedule is lane-distributed (lane l holds W[l] and W[32 + l]; W[j] is one shuffle away).  Lane l owns bit l of every word, so
 // a bit array is one 128-byte store per warp instruction; the packed limbs of a schedule step (6) or a round (12) are one store by
 // the low lanes.  Nothing is read but the row's 96-byte input.
+// WINDOW: only columns [win.col0, win.col1) are stored, as a dense n x (col1 - col0) matrix: the column block one rank of the sharded
+// prover commits.  The whole compression still runs; only the stores are filtered.
 constexpr int SG_WARPS = 8;
 
-template <int F>
-__global__ void __launch_bounds__(32 * SG_WARPS) sha256_air_generate_kernel(const u32 *inputs, size_t n, u32 *trace) {
+template <int F, bool WINDOW>
+__global__ void __launch_bounds__(32 * SG_WARPS) sha256_air_generate_kernel(const u32 *inputs, size_t n, u32 *trace, const GenWindow win) {
     const unsigned lane = threadIdx.x & 31u;
     const size_t row = (size_t)blockIdx.x * SG_WARPS + (threadIdx.x >> 5);
     if (row >= n) return;
     const u32 ONE = Fp<F>::ONE;
     const u32 word = lane < 24 ? __ldg(inputs + row * 24 + lane) : 0u;
-    u32 *out = trace + row * SH_COLS;
-    auto bits = [&](int col, u32 w) { out[col + lane] = (w >> lane) & 1u ? ONE : 0u; };
+    u32 *out = WINDOW ? trace + row * (win.col1 - win.col0) : trace + row * SH_COLS;
+    auto put = [&](int c, u32 v) {
+        if constexpr (WINDOW) {
+            if ((size_t)c >= win.col0 && (size_t)c < win.col1) out[c - win.col0] = v;
+        } else {
+            out[c] = v;
+        }
+    };
+    auto bits = [&](int col, u32 w) { put(col + lane, (w >> lane) & 1u ? ONE : 0u); };
     auto limb = [](u32 w, unsigned hi) { return to_monty<F>(hi ? w >> 16 : w & 0xffffu); };
     u32 h[8];
 #pragma unroll
     for (int j = 0; j < 8; j++) h[j] = __shfl_sync(0xffffffffu, word, 16 + j);
     {
         const u32 hw = __shfl_sync(0xffffffffu, word, 16 + ((lane >> 1) & 7u));   // lane l < 16: limb l & 1 of H[l >> 1]
-        if (lane < 16) out[SH_H_IN + lane] = limb(hw, lane & 1u);
+        if (lane < 16) put(SH_H_IN + lane, limb(hw, lane & 1u));
     }
     // message schedule (generation.rs step 2)
     u32 w0 = lane < 16 ? word : 0u, w1 = 0u;
@@ -79,7 +88,7 @@ __global__ void __launch_bounds__(32 * SG_WARPS) sha256_air_generate_kernel(cons
         if (lane < 6) {                                                 // sched_sigma0[i], sched_sigma1[i], sched_tmp[i], i = t - 16
             const unsigned j = lane >> 1;
             const u32 v = j == 0 ? s0 : j == 1 ? s1 : tmp;
-            out[(j == 0 ? SH_SIG0 : j == 1 ? SH_SIG1 : SH_TMP) + 2 * (t - 16) + (lane & 1u)] = limb(v, lane & 1u);
+            put((j == 0 ? SH_SIG0 : j == 1 ? SH_SIG1 : SH_TMP) + 2 * (t - 16) + (lane & 1u), limb(v, lane & 1u));
         }
     }
     // compression (generation.rs step 3): the chains' first four slots are (d, c, b, a) = H3..H0 and (h, g, f, e) = H7..H4
@@ -101,7 +110,7 @@ __global__ void __launch_bounds__(32 * SG_WARPS) sha256_air_generate_kernel(cons
         if (lane < 12) {                                                // rounds[t]: sigma1_e, ch, tmp1, t1, sigma0_a, maj
             const unsigned j = lane >> 1;
             const u32 v = j == 0 ? s1e : j == 1 ? ch : j == 2 ? tmp1 : j == 3 ? t1 : j == 4 ? s0a : maj;
-            out[SH_ROUNDS + 12 * t + lane] = limb(v, lane & 1u);
+            put(SH_ROUNDS + 12 * t + lane, limb(v, lane & 1u));
         }
         bits(SH_A + 32 * (t + 4), na);
         bits(SH_E + 32 * (t + 4), ne);
@@ -126,16 +135,20 @@ __global__ void __launch_bounds__(32 * SG_WARPS) sha256_air_generate_kernel(cons
 //   - every a / e chain word is loaded and packed once: a 4-deep window of bits and limbs covers its uses as a, b, c and d (e, f,
 //     g and h); the 64 schedule words are packed once up front, lane-distributed over four registers.
 // Each lane folds its constraints with air_qmac; air_warp_store adds the 32 partial sums and multiplies by 1 / Z_H.
+// SHARDED: one rank's chunk-major row block (AirHandQArgs); every column address goes through the unit table behind the alpha
+// powers (air_program.cuh AirShardRow), the block's rows are the points, and the quotient lands in the block's slice.
 constexpr int SQ_WARPS = 24;
 constexpr size_t SQ_SMEM = (size_t)SH_CONSTRAINTS * 16;
 
-template <int F> __global__ void __launch_bounds__(32 * SQ_WARPS, 1) sha256_air_quotient_kernel(const AirHandQArgs a) {
+template <int F, bool SHARDED> __global__ void __launch_bounds__(32 * SQ_WARPS, 1) sha256_air_quotient_kernel(const AirHandQArgs a) {
     extern __shared__ uint4 sq_sm[];
     const uint4 *ap = sq_sm;
+    u64 *units = reinterpret_cast<u64 *>(sq_sm + SH_CONSTRAINTS);
     for (int t = threadIdx.x; t < SH_CONSTRAINTS; t += blockDim.x) sq_sm[t] = __ldg(a.apow + t);
+    if constexpr (SHARDED) air_shard_table_load(a, units);
     __syncthreads();
     const unsigned lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const u32 n_pts = 1u << a.d.log_q;
+    const u32 n_pts = SHARDED ? a.rows : 1u << a.d.log_q;
     const u32 ONE = Fp<F>::ONE;
     const u32 T16 = to_monty<F>(1u << 16), T17 = fp_double<F>(T16), T32 = mont_mul<F>(T16, T16), T33 = fp_double<F>(T32);
     const u32 wpow = to_monty<F>(1u << (lane & 15u));                  // weight of this lane's bit in its 16-bit limb
@@ -156,8 +169,12 @@ template <int F> __global__ void __launch_bounds__(32 * SQ_WARPS, 1) sha256_air_
         return air_bxor<F>(air_bxor<F>(b1, b2), shr && lane + r3 >= 32 ? 0u : b3);
     };
     for (u32 i = blockIdx.x * SQ_WARPS + warp; i < n_pts; i += gridDim.x * SQ_WARPS) {
-        const u32 *row = a.lde + (size_t)air_bitrev(i, a.d.log_q) * SH_COLS;
-        auto ld = [row](int c) { return __ldg(row + c); };
+        const u32 *row = SHARDED ? a.lde : a.lde + (size_t)air_bitrev(i, a.d.log_q) * SH_COLS;
+        const AirShardRow sr{a.lde, units, i};
+        auto ld = [row, sr](int c) {
+            if constexpr (SHARDED) return sr.ld((u32)c);
+            else return __ldg(row + c);
+        };
         u64 acc[4] = {0, 0, 0, 0};
         auto fold = [&](int k, u32 c) { air_qmac<F>(acc, c, ap[k]); };
         u32 mine = 0;
@@ -277,29 +294,54 @@ template <int F> __global__ void __launch_bounds__(32 * SQ_WARPS, 1) sha256_air_
             add2(lo, hi, bc(hin, 2 * j), bc(hin, 2 * j + 1), j < 4 ? al[w] : el[w], j < 4 ? ah[w] : eh[w], 2 * j);
         }
         if (lane < 16) fold(SH_K_FINAL + lane, mine);
-        air_warp_store<F>(a, acc, i, lane);
+        if constexpr (SHARDED) air_warp_store<F>(a, acc, i, lane, air_shard_odd(a, i));
+        else air_warp_store<F>(a, acc, i, lane);
     }
 }
 
 // ---- host entry points ----------------------------------------------------------------------------------------------------
-template <int F> static int32_t sh_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n, u32 *d_trace) {
-    sha256_air_generate_kernel<F><<<(unsigned)((n + SG_WARPS - 1) / SG_WARPS), 32 * SG_WARPS, 0, ctx->stream>>>(d_inputs, n, d_trace);
+template <int F, bool WINDOW> static int32_t sh_generate(p3gpu_ctx *ctx, const u32 *d_inputs, size_t n, u32 *d_trace, const GenWindow &win) {
+    sha256_air_generate_kernel<F, WINDOW><<<(unsigned)((n + SG_WARPS - 1) / SG_WARPS), 32 * SG_WARPS, 0, ctx->stream>>>(d_inputs, n, d_trace, win);
     ctx->launches++;
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
 
-int32_t sha256_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace) {
+static int32_t sh_check(int field, size_t n_hashes) {
     P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "SHA-256 AIR: unsupported field %d", field);
     P3_CHECK(n_hashes > 0 && (n_hashes & (n_hashes - 1)) == 0 && n_hashes <= ((size_t)1 << 32), P3GPU_EINVAL,
              "SHA-256 AIR: %zu hashes (need a power of two, at most 2^32)", n_hashes);
-    return field == BABY_BEAR ? sh_generate<BABY_BEAR>(ctx, d_inputs, n_hashes, d_trace) : sh_generate<KOALA_BEAR>(ctx, d_inputs, n_hashes, d_trace);
+    return P3GPU_OK;
+}
+
+int32_t sha256_air_generate(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, u32 *d_trace) {
+    P3_TRY(sh_check(field, n_hashes));
+    const GenWindow win{};
+    return field == BABY_BEAR ? sh_generate<BABY_BEAR, false>(ctx, d_inputs, n_hashes, d_trace, win)
+                              : sh_generate<KOALA_BEAR, false>(ctx, d_inputs, n_hashes, d_trace, win);
+}
+
+int32_t sha256_air_generate_cols(p3gpu_ctx *ctx, int field, const u32 *d_inputs, size_t n_hashes, size_t col0, size_t col1, u32 *d_out) {
+    P3_TRY(sh_check(field, n_hashes));
+    P3_TRY(air_check_window("SHA-256", col0, col1, SH_COLS));
+    if (col0 == col1) return P3GPU_OK;
+    const GenWindow win{col0, col1, 1};
+    return field == BABY_BEAR ? sh_generate<BABY_BEAR, true>(ctx, d_inputs, n_hashes, d_out, win)
+                              : sh_generate<KOALA_BEAR, true>(ctx, d_inputs, n_hashes, d_out, win);
 }
 
 int32_t sha256_air_quotient(p3gpu_ctx *ctx, int field, const u32 *d_lde, unsigned log_lde, unsigned log_n, const u32 *alpha, u32 *d_q) {
-    return air_hand_quotient(ctx, field, "SHA-256", (const void *)sha256_air_quotient_kernel<BABY_BEAR>,
-                             (const void *)sha256_air_quotient_kernel<KOALA_BEAR>, SH_CONSTRAINTS, SQ_WARPS, SQ_SMEM, 0, d_lde, log_lde, log_n,
+    return air_hand_quotient(ctx, field, "SHA-256", (const void *)sha256_air_quotient_kernel<BABY_BEAR, false>,
+                             (const void *)sha256_air_quotient_kernel<KOALA_BEAR, false>, SH_CONSTRAINTS, SQ_WARPS, SQ_SMEM, 0, d_lde, log_lde, log_n,
                              alpha, d_q);
+}
+
+int32_t sha256_air_quotient_sharded(p3gpu_ctx *ctx, int field, const AirHandShard &shard, const u32 *d_block, unsigned log_lde, unsigned log_n,
+                                    const u32 *alpha, u32 *d_q) {
+    const AirHandShard sh{shard.world, shard.rank, shard.col_starts, SH_COLS};
+    return air_hand_quotient(ctx, field, "SHA-256", (const void *)sha256_air_quotient_kernel<BABY_BEAR, true>,
+                             (const void *)sha256_air_quotient_kernel<KOALA_BEAR, true>, SH_CONSTRAINTS, SQ_WARPS, SQ_SMEM, 0, d_block, log_lde,
+                             log_n, alpha, d_q, nullptr, 32, &sh);
 }
 
 }  // namespace p3

@@ -359,6 +359,27 @@ def column_segments(world: int, col_starts, rows: int):
     return [(int(buf[3 * k]), int(buf[3 * k + 1]), int(buf[3 * k + 2])) for k in range(n.value)]
 
 
+def chunk_major_block(rows_dense, world: int, col_starts):
+    """Rows of the bit-reversed LDE laid out as p3gpu_commit_sharded_dev leaves a row block (`column_segments`): a flat CUDA int32
+    tensor, the inverse of PeerGroup.row_block_dense.  Lets one GPU build the block any rank of a `world`-rank commit would hash."""
+    R = int(rows_dense.shape[0])
+    out = torch.empty(R * int(rows_dense.shape[1]), dtype=rows_dense.dtype, device=rows_dense.device)
+    for c0, c1, off in column_segments(world, col_starts, R):
+        out[off:off + R * (c1 - c0)] = rows_dense[:, c0:c1].reshape(-1)
+    return out
+
+
+def block_view(world: int, rank: int, block):
+    """A _lib.PeerGroupStruct that names only my row block `block` (a CUDA tensor in the layout of `chunk_major_block`), for the
+    sharded quotient entry points, which read nothing but grp->rows[rank].  The other ranks' row and control pointers are set to the
+    same block to pass the group's null checks; nothing that exchanges, synchronises or hashes may be given this view."""
+    st = _lib.PeerGroupStruct()
+    st.world, st.rank, st.timeout_s = world, rank, 1.0
+    for q in range(world):
+        st.ctrl[q] = st.rows[q] = block.data_ptr()
+    return st
+
+
 def query_owner(index: int, rows_per_rank: int):
     """(rank, local row) holding row `index` of the bit-reversed LDE after the row-sharded commit."""
     return index // rows_per_rank, index % rows_per_rank
@@ -381,7 +402,10 @@ def _bitrev(x, bits: int):
 class ShardedTrace:
     """The trace's prover data and its opener when the trace's columns are split over the ranks of a PeerGroup: rank g holds
     columns [col_starts[g], col_starts[g+1]), and after the sharded commit LDE rows [g R, (g+1) R), R = LDE height / world, with
-    its sub-tree.  `uni_stark.prove(config, air, block, shard=ShardedTrace(grp, col_starts))` proves the Poseidon2 AIR with it.
+    its sub-tree.  `uni_stark.prove(config, air, block, shard=ShardedTrace(grp, col_starts))` proves with it any air.KernelAir that
+    has a sharded quotient kernel (the Poseidon2 AIR over KoalaBear, the Blake3, SHA-256 and Poseidon1 AIRs), under either
+    configuration: the commit, the exchanges and the openings carry 8-word digests, which is what both the Poseidon2 and the Keccak
+    MMCS write ([F; 8] and [u64; 4]).
 
     It carries out the steps that read the trace's rows.  Ranks exchange data over peer memory only where a value depends on rows
     they do not own, and after every exchange all ranks hold identical bytes, so their transcripts stay identical:
@@ -420,11 +444,11 @@ class ShardedTrace:
         return cap, self
 
     def quotient_values(self, air, quotient_domain, alpha):
-        """The Poseidon2 AIR's quotient values in natural order over the quotient domain, which must be the LDE domain: the sharded
+        """The AIR's quotient values in natural order over the quotient domain, which must be the LDE domain: the AIR's sharded
         kernel on my rows in place, the bit-reversed slices all-gathered and put back in natural order by one gather."""
         assert quotient_domain[1] == self.log_height, "the sharded quotient covers the LDE domain: log_num_quotient_chunks == log_blowup"
         H = self.shape[0]
-        q_slice = self.grp.p2air_quotient(self.field, air.vector_len, self.log_height, self.log_degree, alpha)
+        q_slice = air.sharded_quotient_values(self.grp, self.log_height, self.log_degree, alpha)
         q_bitrev = self.grp.exchange(q_slice).reshape(H, 4)
         return q_bitrev[_bitrev(torch.arange(H, device=self.device, dtype=torch.int64), self.log_height)].contiguous()
 
@@ -504,19 +528,42 @@ class ShardedTrace:
         return [np.ascontiguousarray(ans[:, :W])], np.ascontiguousarray(ans[:, W:]).reshape(n, plen, 8)
 
 
-def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
-    """uni_stark.prove of the Poseidon2 AIR with the trace sharded by column block over the ranks of `grp` (rank g holds columns
-    [col_starts[g], col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  Every rank returns the same Proof, byte for
-    byte the one `uni_stark.prove` writes for the whole trace on one GPU; its timings_ms are each span's maximum over the ranks."""
+def sharded_air_error(config, air):
+    """None, or why prove_sharded cannot prove `air` under `config`: it needs a StarkConfig or KeccakStarkConfig and an air.KernelAir
+    with a sharded quotient kernel whose constraints read the local row only (a row's next row lies on another rank)."""
+    from .air import KernelAir
     from .field import KoalaBear
-    from .uni_stark import VectorizedPoseidon2Air, get_log_num_quotient_chunks, prove
+    from .poseidon2_air import VectorizedPoseidon2Air
+    from .uni_stark import KeccakStarkConfig, StarkConfig
+    if not isinstance(air, KernelAir):
+        return (f"prove_sharded: {type(air).__name__} is a constraint-program AIR; only AIRs with hand-written kernels have a sharded "
+                "quotient")
+    name = air.air_name or type(air).__name__
+    if air.main_next_row_columns():
+        return f"prove_sharded: the {name} AIR reads the next row, which lies on another rank"
+    if not air.has_sharded_quotient():
+        return f"prove_sharded: the {name} AIR has no sharded quotient kernel"
+    if isinstance(air, VectorizedPoseidon2Air) and air.field.id != KoalaBear.id:
+        # its sharded quotient kernel reads 16-byte units of 4-column segments; BabyBear's 298-column permutations start mid-unit
+        return f"prove_sharded: the Poseidon2 AIR over {air.field.name} has no sharded prove (KoalaBear only)"
+    if not isinstance(config, (StarkConfig, KeccakStarkConfig)):
+        return f"prove_sharded: {type(config).__name__} is not a StarkConfig or KeccakStarkConfig"
+    return None
+
+
+def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
+    """uni_stark.prove with the trace sharded by column block over the ranks of `grp` (rank g holds columns [col_starts[g],
+    col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  `config`: StarkConfig or KeccakStarkConfig; `air`: the Poseidon2
+    AIR over KoalaBear, or the Blake3, SHA-256 or Poseidon1 AIR over either field (sharded_air_error says why another is refused,
+    before any device work).  Every rank returns the same Proof, byte for byte the one `uni_stark.prove` writes for the whole trace on
+    one GPU; its timings_ms are each span's maximum over the ranks."""
+    from .uni_stark import get_log_num_quotient_chunks, prove
+    err = sharded_air_error(config, air)
+    if err:
+        raise ValueError(err)
     pcs = config.pcs
     assert grp.gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
-    assert isinstance(air, VectorizedPoseidon2Air), "the sharded quotient kernel evaluates the Poseidon2 AIR only"
-    if air.field.id != KoalaBear.id:
-        # the sharded quotient kernel reads 16-byte units of 4-column segments; BabyBear's 298-column permutations start mid-unit
-        raise ValueError(f"prove_sharded: the Poseidon2 AIR over {air.field.name} has no sharded prove (KoalaBear only)")
-    assert len(public_values) == 0, "the Poseidon2 AIR has no public values"
+    assert len(public_values) == 0, f"the {air.air_name} AIR has no public values"
     assert get_log_num_quotient_chunks(air) == pcs.fri.log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
     proof = prove(config, air, trace_block, shard=ShardedTrace(grp, col_starts))
     if grp.world > 1 and dist.is_initialized():

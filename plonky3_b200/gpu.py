@@ -329,6 +329,18 @@ class Gpu:
         """`_air_quotient_2n` of the Blake3 AIR (9168 columns)."""
         return self._air_quotient_2n(self.L.p3gpu_blake3_air_quotient_dev, _lib.BLAKE3_AIR_COLS, field, lde_dev, log_trace_height, alpha)
 
+    def blake3_air_generate_trace_cols(self, field, inputs_dev, col0, col1):
+        """Columns [col0, col1) of `blake3_air_generate_trace`'s output: (n, col1 - col0)."""
+        import torch
+        x = self._air_inputs(inputs_dev, torch.int32, 24)
+        return self._air_trace_cols(lambda out: self.L.p3gpu_blake3_air_generate_trace_cols_dev(self.h, field, x.data_ptr(), int(x.shape[0]),
+                                                                                               col0, col1, out), int(x.shape[0]), col0, col1)
+
+    def blake3_air_quotient_sharded(self, field, group, col_starts, log_lde_height, log_trace_height, alpha):
+        """`_air_quotient_sharded` of the Blake3 AIR."""
+        return self._air_quotient_sharded(self.L.p3gpu_blake3_air_quotient_sharded_dev, field, group, col_starts, log_lde_height,
+                                          log_trace_height, alpha)
+
     # ------------------------------------------------------------------ SHA-256 AIR
     def sha256_air_generate_trace(self, field, inputs_dev):
         """(n, 24) contiguous CUDA int32 tensor of u32 words (the 16-word block, the 8-word chaining state), n a power of two -> the
@@ -343,6 +355,18 @@ class Gpu:
     def sha256_air_quotient(self, field, lde_dev, log_trace_height, alpha):
         """`_air_quotient_2n` of the SHA-256 AIR (7728 columns)."""
         return self._air_quotient_2n(self.L.p3gpu_sha256_air_quotient_dev, _lib.SHA256_AIR_COLS, field, lde_dev, log_trace_height, alpha)
+
+    def sha256_air_generate_trace_cols(self, field, inputs_dev, col0, col1):
+        """Columns [col0, col1) of `sha256_air_generate_trace`'s output: (n, col1 - col0)."""
+        import torch
+        x = self._air_inputs(inputs_dev, torch.int32, 24)
+        return self._air_trace_cols(lambda out: self.L.p3gpu_sha256_air_generate_trace_cols_dev(self.h, field, x.data_ptr(), int(x.shape[0]),
+                                                                                               col0, col1, out), int(x.shape[0]), col0, col1)
+
+    def sha256_air_quotient_sharded(self, field, group, col_starts, log_lde_height, log_trace_height, alpha):
+        """`_air_quotient_sharded` of the SHA-256 AIR."""
+        return self._air_quotient_sharded(self.L.p3gpu_sha256_air_quotient_sharded_dev, field, group, col_starts, log_lde_height,
+                                          log_trace_height, alpha)
 
     # ------------------------------------------------------------------ Poseidon1 AIR
     def p1air_set_constants(self, field, initial_full, terminal_full, mds_circ_col, first_round_constants, m_i, partial_rc,
@@ -375,6 +399,19 @@ class Gpu:
         entry = lambda h, f, *rest: self.L.p3gpu_p1air_quotient_dev(h, f, vector_len, *rest)
         return self._air_quotient_2n(entry, vector_len * self._p1air_cols, field, lde_dev, log_trace_height, alpha)
 
+    def p1air_generate_trace_cols(self, field, inputs_dev, col0, col1, vector_len=8):
+        """Columns [col0, col1) of `p1air_generate_trace`'s output: (n_perms / vector_len, col1 - col0)."""
+        import torch
+        x = self._air_inputs(inputs_dev, torch.int32, 16)
+        n = int(x.shape[0])
+        return self._air_trace_cols(lambda out: self.L.p3gpu_p1air_generate_trace_cols_dev(self.h, field, vector_len, x.data_ptr(), n, col0, col1,
+                                                                                          out), n // vector_len, col0, col1)
+
+    def p1air_quotient_sharded(self, field, group, col_starts, log_lde_height, log_trace_height, alpha, vector_len=8):
+        """`_air_quotient_sharded` of the Poseidon1 AIR with vector_len permutations per row."""
+        entry = lambda h, f, *rest: self.L.p3gpu_p1air_quotient_sharded_dev(h, f, vector_len, *rest)
+        return self._air_quotient_sharded(entry, field, group, col_starts, log_lde_height, log_trace_height, alpha)
+
     # ------------------------------------------------------------------ shared by the hand-written Keccak, Blake3 and Poseidon1 AIRs
     @staticmethod
     def _air_inputs(t, dtype, width):
@@ -382,6 +419,26 @@ class Gpu:
         assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"inputs: contiguous CUDA {str(dtype).removeprefix('torch.')} (n, {width})"
         assert t.dim() == 2 and int(t.shape[1]) == width
         return t
+
+    def _air_trace_cols(self, launch, rows, col0, col1):
+        """A trace generator's column window: a (rows, col1 - col0) device matrix filled by `launch(out pointer)`."""
+        col0, col1 = int(col0), int(col1)
+        if not 0 <= col0 <= col1:
+            raise _lib.P3GpuError(f"column window [{col0}, {col1})", _lib.EINVAL)
+        self._use_torch_stream()
+        out = self._empty((rows, col1 - col0))
+        check(launch(out.data_ptr() if col1 > col0 else None))
+        return out
+
+    def _air_quotient_sharded(self, entry, field, group, col_starts, log_lde_height, log_trace_height, alpha):
+        """My row block's quotient values after the row-sharded commit: (R, 4), R = 2^log_lde_height / world, the bit-reversed slice
+        `rank` (entry m is natural index bitrev(rank R + m)).  `group`: the _lib.PeerGroupStruct of the commit (its row block is
+        read in place), `col_starts`: the commit's world + 1 column offsets; `entry`: the AIR's p3gpu_*_quotient_sharded_dev."""
+        self._use_torch_stream()
+        cs = (C.c_size_t * len(col_starts))(*[int(x) for x in col_starts])
+        q = self._empty(((1 << log_lde_height) // int(group.world), 4))
+        check(entry(self.h, field, C.byref(group), cs, log_lde_height, log_trace_height, self._ef(alpha).ctypes.data, q.data_ptr()))
+        return q
 
     def _air_quotient_2n(self, entry, width, field, lde_dev, log_trace_height, alpha):
         """Quotient values (2^(log_trace_height + 1), 4) in natural order over GENERATOR * K from the first 2^(log_trace_height + 1)

@@ -279,7 +279,18 @@ class VectorizedPoseidon1Air(KernelAir):
         self._upload()
         return self.gpu.p1air_generate_trace(self.field.id, inputs_dev, self.vector_len)
 
+    def generate_trace_cols(self, inputs_dev, col0: int, col1: int):
+        """Columns [col0, col1) of `generate_trace_rows(inputs_dev)` without building the full trace: one rank's column block for
+        `distributed.prove_sharded`.  The window may cut a permutation."""
+        self._need_gpu("trace generation")
+        self._upload()
+        return self.gpu.p1air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1), self.vector_len)
+
     def _kernel_quotient(self, trace_lde_dev, log_degree: int, alpha):
         """`trace_lde_dev`: the trace on GENERATOR * K, |K| = 2N (the committed LDE's prefix).  Returns (2N, 4)."""
         self._upload()
         return self.gpu.p1air_quotient(self.field.id, trace_lde_dev, int(log_degree), alpha, self.vector_len)
+
+    def _kernel_quotient_sharded(self, grp, log_lde_height: int, log_degree: int, alpha):
+        self._upload()
+        return self.gpu.p1air_quotient_sharded(self.field.id, grp.struct, grp.col_starts, log_lde_height, log_degree, alpha, self.vector_len)

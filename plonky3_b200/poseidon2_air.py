@@ -15,7 +15,7 @@ row-sharded p3gpu_p2air_quotient_sharded_dev that distributed.py runs), with no 
 
 Column layout of one permutation (columns.rs): inputs [0,16) | 4 beginning full rounds {sbox registers [16 REG], post [16]} |
 rounds_p partial rounds {sbox register [REG], post_sbox} | 4 ending full rounds {sbox registers, post}, REG = sbox_registers(field);
-a row holds vector_len permutations side by side.  The row-sharded prove (distributed.prove_sharded) is KoalaBear-only.  uni_stark re-exports RoundConstants, VectorizedPoseidon2Air and VECTOR_LEN.
+a row holds vector_len permutations side by side.  The row-sharded prove (distributed.prove_sharded) is KoalaBear-only for this AIR.  uni_stark re-exports RoundConstants, VectorizedPoseidon2Air and VECTOR_LEN.
 """
 from __future__ import annotations
 
@@ -171,3 +171,7 @@ class VectorizedPoseidon2Air(KernelAir):
         """`trace_lde_dev`: the whole committed LDE.  Returns (its height, 4)."""
         self._upload()
         return self.gpu.p2air_quotient(self.field.id, trace_lde_dev, log_degree, alpha, self.vector_len)
+
+    def _kernel_quotient_sharded(self, grp, log_lde_height: int, log_degree: int, alpha):
+        """PeerGroup.p2air_quotient (KoalaBear only; the device refuses BabyBear)."""
+        return grp.p2air_quotient(self.field, self.vector_len, log_lde_height, log_degree, alpha)

@@ -158,6 +158,15 @@ class Sha256Air(KernelAir):
         x = self._to_device(torch.from_numpy(random_inputs(n).view(np.int32)))
         return self.generate_trace_rows(x)
 
+    def generate_trace_cols(self, inputs_dev, col0: int, col1: int):
+        """Columns [col0, col1) of `generate_trace_rows(inputs_dev)` without building the full trace: one rank's column block for
+        `distributed.prove_sharded`."""
+        self._need_gpu("trace generation")
+        return self.gpu.sha256_air_generate_trace_cols(self.field.id, inputs_dev, int(col0), int(col1))
+
     def _kernel_quotient(self, trace_lde_dev, log_degree: int, alpha):
         """`trace_lde_dev`: the trace on GENERATOR * K, |K| = 2N (the committed LDE's prefix).  Returns (2N, 4)."""
         return self.gpu.sha256_air_quotient(self.field.id, trace_lde_dev, int(log_degree), alpha)
+
+    def _kernel_quotient_sharded(self, grp, log_lde_height: int, log_degree: int, alpha):
+        return self.gpu.sha256_air_quotient_sharded(self.field.id, grp.struct, grp.col_starts, log_lde_height, log_degree, alpha)

@@ -9,8 +9,9 @@ p3gpu_air_quotient_layout_dev); poseidon2_air.VectorizedPoseidon2Air, the config
 koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`),
 keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air and poseidon1_air.VectorizedPoseidon1Air through their
 hand-written kernels.  With
-`shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 AIR with the trace's columns split over several GPUs, the
-shard standing in for the trace commit, the quotient values and the trace's row reads of the opening.
+`shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 (KoalaBear), Blake3, SHA-256 and Poseidon1 AIRs with the
+trace's columns split over several GPUs, the shard standing in for the trace commit, the quotient values and the trace's row reads of
+the opening.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
     alpha <- transcript;  quotient values on GENERATOR * K ................... air.quotient_values (p3gpu_p2air_quotient_dev, ...)

@@ -63,6 +63,8 @@ pub const P3GPU_COSET_IDFT: i32 = 3;
 pub const P3GPU_HASH_POSEIDON2_W16: i32 = 0;
 pub const P3GPU_HASH_POSEIDON2_W24: i32 = 1;
 pub const P3GPU_HASH_KECCAK: i32 = 2;
+pub const P3GPU_HASH_SHA256: i32 = 3;
+pub const P3GPU_HASH_SHA256_COMPRESS: i32 = 4;
 
 #[repr(C)]
 pub struct P3GpuPeerGroup {
@@ -236,6 +238,7 @@ unsafe extern "C" {
     pub fn p3gpu_challenger_sample(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, h_out: *mut u32, n: usize) -> i32;
     pub fn p3gpu_challenger_grind(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, bits: c_uint, witness: *mut u32) -> i32;
     pub fn p3gpu_challenger_new_keccak256(ctx: *mut P3GpuCtx, field: c_int, out: *mut *mut P3GpuChallenger) -> i32;
+    pub fn p3gpu_challenger_new_sha256(ctx: *mut P3GpuCtx, field: c_int, out: *mut *mut P3GpuChallenger) -> i32;
     pub fn p3gpu_challenger_observe_digest(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, h_words: *const u32, n: usize) -> i32;
     pub fn p3gpu_challenger_sample_bits(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger, bits: c_uint, n: usize, h_out: *mut u32) -> i32;
 }

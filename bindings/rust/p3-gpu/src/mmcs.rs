@@ -11,15 +11,20 @@ use p3_symmetric::MerkleCap;
 use crate::ffi::*;
 use crate::{GpuCtx, GpuField};
 
-/// Which of the reference's hash configurations the GPU runs (`examples/src/types.rs:19-53`).
+/// Which of the reference's hash configurations the GPU runs (`examples/src/types.rs:19-53`,
+/// `keccak-air/examples/prove_baby_bear_sha256*.rs`); the discriminants are the ABI's `P3GPU_HASH_*`.
 #[derive(Clone, Copy)]
 pub enum GpuHash {
     /// `PaddingFreeSponge<Perm16,16,8,8>` + `TruncatedPermutation<Perm16,2,8,16>`
-    Poseidon2W16,
+    Poseidon2W16 = P3GPU_HASH_POSEIDON2_W16 as isize,
     /// `PaddingFreeSponge<Perm24,24,16,8>` + `TruncatedPermutation<Perm16,2,8,16>`
-    Poseidon2W24,
+    Poseidon2W24 = P3GPU_HASH_POSEIDON2_W24 as isize,
     /// `SerializingHasher<PaddingFreeSponge<KeccakF,25,17,4>>` + `CompressionFunctionFromHasher<_,2,4>`
-    Keccak,
+    Keccak = P3GPU_HASH_KECCAK as isize,
+    /// `SerializingHasher<Sha256>` + `CompressionFunctionFromHasher<Sha256,2,32>` (`[u8; 32]` digests)
+    Sha256 = P3GPU_HASH_SHA256 as isize,
+    /// `SerializingHasher<Sha256>` + `Sha256Compress` (`[u8; 32]` digests)
+    Sha256Compress = P3GPU_HASH_SHA256_COMPRESS as isize,
 }
 
 /// Wraps the reference MMCS (`inner`, used for `open_batch` / `verify_batch` and for its hash parameters) and replaces `commit`.

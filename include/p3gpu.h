@@ -63,8 +63,11 @@ enum {
 enum {
     P3GPU_HASH_POSEIDON2_W16 = 0, /* leaf PaddingFreeSponge<Perm16,16,8,8>,  node TruncatedPermutation<Perm16,2,8,16> */
     P3GPU_HASH_POSEIDON2_W24 = 1, /* leaf PaddingFreeSponge<Perm24,24,16,8>, node TruncatedPermutation<Perm16,2,8,16> */
-    P3GPU_HASH_KECCAK = 2         /* leaf SerializingHasher<PaddingFreeSponge<KeccakF,25,17,4>>, node CompressionFunctionFromHasher<_,2,4> */
+    P3GPU_HASH_KECCAK = 2,        /* leaf SerializingHasher<PaddingFreeSponge<KeccakF,25,17,4>>, node CompressionFunctionFromHasher<_,2,4> */
+    P3GPU_HASH_SHA256 = 3,        /* leaf SerializingHasher<Sha256>, node CompressionFunctionFromHasher<Sha256,2,32> */
+    P3GPU_HASH_SHA256_COMPRESS = 4 /* leaf SerializingHasher<Sha256>, node Sha256Compress (one compress256 from H256_256) */
 };
+/* The SHA-256 kinds' digests are [u8; 32], held as 8 words whose own (little-endian) bytes are the digest's bytes in order. */
 
 /* ---- context ---------------------------------------------------------------------------------- */
 int32_t p3gpu_ctx_create(int device, p3gpu_ctx **out);
@@ -405,6 +408,11 @@ int32_t p3gpu_challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bi
  * the END of the 32-byte digest (masked to 31 bits, resampled while >= p) and returns Montgomery words; `grind` returns the smallest
  * witness (Montgomery word), observes it and consumes the checked sample. */
 int32_t p3gpu_challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out);
+/* SerializingChallenger32<F, HashChallenger<u8, Sha256, 32>> (the transcript of the SHA-256 configurations,
+ * keccak-air/examples/prove_baby_bear_sha256*.rs), created empty as by from_hasher(vec![], Sha256).  Same semantics as the
+ * Keccak-256 handle with SHA-256 as the hash; its digests are [u8; 32], observed through p3gpu_challenger_observe_digest as the
+ * 8 words' own bytes. */
+int32_t p3gpu_challenger_new_sha256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out);
 /* Observe n digest words as the MMCS commits them (a cap, or any digest): on the duplex handle they are field elements (Montgomery
  * words, as p3gpu_challenger_observe); on the Keccak-256 handle a [u64; 4] digest held as 8 words is observed as its 32
  * little-endian bytes, i.e. the words' own bytes in order. */

@@ -107,6 +107,8 @@ struct MerkleTree {                     // merkle-tree/src/merkle_tree.rs:33-69 
     }
 };
 
+// `hash`: one of the P3GPU_HASH_* kinds.  Every kind's digest is 8 words; for P3GPU_HASH_SHA256 and P3GPU_HASH_SHA256_COMPRESS
+// they hold a [u8; 32] digest, the words' little-endian bytes being the digest's bytes in order.
 class MerkleTreeMmcs {
   public:
     MerkleTreeMmcs(Context &c, int field, int hash, size_t cap_height) : c_(c), field_(field), hash_(hash), cap_height_(cap_height) {}

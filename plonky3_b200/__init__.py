@@ -4,8 +4,8 @@ The compute lives in libp3gpu.so (plonky3_b200/csrc, C ABI in include/p3gpu.h); 
 of the reference's trait surfaces (TwoAdicSubgroupDft, Mmcs, FriParameters/FriFoldingStrategy, Pcs::commit).
 There is no CPU fallback: without the built library and a CUDA device every entry point raises."""
 from . import _lib
-from ._lib import P3GpuError, HASH_KECCAK, HASH_POSEIDON2_W16, HASH_POSEIDON2_W24
+from ._lib import P3GpuError, HASH_KECCAK, HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_SHA256, HASH_SHA256_COMPRESS
 from .field import BabyBear, KoalaBear, Field, FIELDS
 
 __all__ = ["_lib", "P3GpuError", "BabyBear", "KoalaBear", "Field", "FIELDS", "HASH_KECCAK", "HASH_POSEIDON2_W16",
-           "HASH_POSEIDON2_W24"]
+           "HASH_POSEIDON2_W24", "HASH_SHA256", "HASH_SHA256_COMPRESS"]

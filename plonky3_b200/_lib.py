@@ -13,7 +13,7 @@ LIB_PATH = pathlib.Path(os.environ["P3GPU_LIB"]) if os.environ.get("P3GPU_LIB") 
 BABY_BEAR, KOALA_BEAR = 0, 1
 EOK, EINVAL, EUNSUPPORTED, ECUDA, ENOMEM, ESTATE = 0, -1, -2, -3, -4, -5
 DFT, IDFT, COSET_DFT, COSET_IDFT = 0, 1, 2, 3
-HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_KECCAK = 0, 1, 2
+HASH_POSEIDON2_W16, HASH_POSEIDON2_W24, HASH_KECCAK, HASH_SHA256, HASH_SHA256_COMPRESS = 0, 1, 2, 3, 4
 KECCAK_AIR_COLS = 2633                       # P3GPU_KECCAK_AIR_COLS
 BLAKE3_AIR_COLS = 9168                       # P3GPU_BLAKE3_AIR_COLS
 SHA256_AIR_COLS = 7728                       # P3GPU_SHA256_AIR_COLS
@@ -36,6 +36,7 @@ EXPORTS = [
     "p3gpu_air_program_create", "p3gpu_air_program_destroy", "p3gpu_air_program_info", "p3gpu_air_quotient_dev",
     "p3gpu_air_program_create_layout", "p3gpu_air_quotient_layout_dev",
     "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
+    "p3gpu_challenger_new_sha256",
     "p3gpu_keccak_air_generate_trace_dev", "p3gpu_keccak_air_quotient_dev",
     "p3gpu_blake3_air_generate_trace_dev", "p3gpu_blake3_air_quotient_dev",
     "p3gpu_sha256_air_generate_trace_dev", "p3gpu_sha256_air_quotient_dev",
@@ -142,6 +143,7 @@ def load():
         "p3gpu_air_program_create_layout": (i32, [vp, ci, vp, sz, vp, sz, vp, C.POINTER(vp)]),
         "p3gpu_air_quotient_layout_dev": (i32, [vp, vp, vp, cu, vp, cu, vp, cu, cu, cu, vp, vp, vp]),
         "p3gpu_challenger_new_keccak256": (i32, [vp, ci, C.POINTER(vp)]),
+        "p3gpu_challenger_new_sha256": (i32, [vp, ci, C.POINTER(vp)]),
         "p3gpu_challenger_observe_digest": (i32, [vp, vp, vp, sz]),
         "p3gpu_challenger_sample_bits": (i32, [vp, vp, cu, sz, vp]),
         "p3gpu_keccak_air_generate_trace_dev": (i32, [vp, ci, vp, sz, vp]),

@@ -1,7 +1,7 @@
 """DuplexChallenger (challenger/src/duplex_challenger.rs:60-300) + GrindingChallenger::grind (grinding_challenger.rs:100-232) with the
 sponge resident on the GPU (csrc/challenger.cu): caps and opened values produced on the device are absorbed there; only sampled
-challenges come back.  SerializingChallenger32 over a Keccak-256 HashChallenger is the same on the device for the Keccak
-configuration.  Protocol plumbing of the prove driver (uni_stark.py), mirroring the reference's method names."""
+challenges come back.  SerializingChallenger32 over a Keccak-256 or SHA-256 HashChallenger is the same on the device for the Keccak
+and SHA-256 configurations.  Protocol plumbing of the prove driver (uni_stark.py), mirroring the reference's method names."""
 from __future__ import annotations
 
 import ctypes as C
@@ -84,28 +84,34 @@ class DuplexChallenger:
 
 
 class SerializingChallenger32:
-    """SerializingChallenger32<F, HashChallenger<u8, Keccak256Hash, 32>> (challenger/src/serializing_challenger.rs,
-    hash_challenger.rs): the transcript of the Keccak configuration (examples/src/types.rs:19-35), resident on the GPU like
-    DuplexChallenger and with the same method surface.  Field elements are observed as the 4 little-endian bytes of their canonical
-    values; a [u64; 4] digest (8 words) as its 32 bytes; samples are rejection-sampled from 4 bytes popped off the end of the
-    Keccak-256 digest; `sample_bits` masks the raw u32; `grind` returns the smallest witness.  Values in and out are Montgomery
-    words, as everywhere else in the prover."""
+    """SerializingChallenger32<F, HashChallenger<u8, H, 32>> (challenger/src/serializing_challenger.rs, hash_challenger.rs) with
+    H = Keccak256Hash, the transcript of the Keccak configuration (examples/src/types.rs:19-35), or H = Sha256, the transcript of
+    the SHA-256 configurations (keccak-air/examples/prove_baby_bear_sha256*.rs); `hasher` is "keccak256" (the default) or
+    "sha256".  Resident on the GPU like DuplexChallenger and with the same method surface.  Field elements are observed as the 4
+    little-endian bytes of their canonical values; a digest (8 words: [u64; 4] or [u8; 32]) as its 32 bytes; samples are
+    rejection-sampled from 4 bytes popped off the end of the hash's digest; `sample_bits` masks the raw u32; `grind` returns the
+    smallest witness.  Values in and out are Montgomery words, as everywhere else in the prover."""
 
-    def __init__(self, field: Field, gpu):
-        self.field, self.gpu = field, gpu
+    HASHERS = ("keccak256", "sha256")
+
+    def __init__(self, field: Field, gpu, hasher: str = "keccak256"):
+        if hasher not in self.HASHERS:
+            raise ValueError(f"unknown transcript hash {hasher!r} (one of {', '.join(self.HASHERS)})")
+        self.field, self.gpu, self.hasher = field, gpu, hasher
         h = C.c_void_p()
         gpu._use_torch_stream()
-        check(gpu.L.p3gpu_challenger_new_keccak256(gpu.h, field.id, C.byref(h)))
+        new = gpu.L.p3gpu_challenger_new_sha256 if hasher == "sha256" else gpu.L.p3gpu_challenger_new_keccak256
+        check(new(gpu.h, field.id, C.byref(h)))
         self.h = h
 
     @classmethod
-    def from_hasher(cls, initial_state, field: Field, gpu):
-        """from_hasher(initial_state, Keccak256Hash): `initial_state` bytes become the start of the input buffer.  The transcript
-        takes whole 32-bit words, so their number must be a multiple of 4."""
+    def from_hasher(cls, initial_state, field: Field, gpu, hasher: str = "keccak256"):
+        """from_hasher(initial_state, H): `initial_state` bytes become the start of the input buffer.  The transcript takes whole
+        32-bit words, so their number must be a multiple of 4."""
         init = bytes(initial_state)
         if len(init) % 4:
             raise ValueError("the initial state must be a whole number of 32-bit words")
-        c = cls(field, gpu)
+        c = cls(field, gpu, hasher)
         if init:
             c._observe_digest(np.frombuffer(init, dtype="<u4").astype(np.uint32))
         return c
@@ -120,7 +126,7 @@ class SerializingChallenger32:
 
     def clone(self):
         c = object.__new__(SerializingChallenger32)
-        c.field, c.gpu = self.field, self.gpu
+        c.field, c.gpu, c.hasher = self.field, self.gpu, self.hasher
         h = C.c_void_p()
         self.gpu._use_torch_stream()
         check(self.gpu.L.p3gpu_challenger_clone(self.gpu.h, self.h, C.byref(h)))
@@ -146,7 +152,7 @@ class SerializingChallenger32:
 
     def observe(self, value: int): self.observe_slice(np.array([value], dtype=np.uint32))
     def observe_canonical(self, x: int): self.observe(self.field.to_monty(x))
-    def observe_cap(self, cap): self._observe_digest(cap)                             # CanObserve<MerkleCap<F, [u64; 4]>>: the bytes
+    def observe_cap(self, cap): self._observe_digest(cap)                             # CanObserve<MerkleCap<F, [u64; 4] | [u8; 32]>>: the bytes
     def observe_algebra_slice(self, ys): self.observe_slice(ys)
 
     # ---- CanSample

@@ -670,6 +670,11 @@ int32_t p3gpu_challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challeng
     P3_CHECK(out, P3GPU_EINVAL, "null argument");
     return challenger_new_keccak256(ctx, field, out);
 }
+int32_t p3gpu_challenger_new_sha256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out) {
+    P3_ENTER(ctx);
+    P3_CHECK(out, P3GPU_EINVAL, "null argument");
+    return challenger_new_sha256(ctx, field, out);
+}
 int32_t p3gpu_challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const uint32_t *h_words, size_t n) {
     P3_ENTER(ctx);
     P3_CHECK(ch && (h_words || n == 0), P3GPU_EINVAL, "null argument");

@@ -18,19 +18,24 @@
 // digest then becomes both the new input buffer and the output buffer, whose bytes are popped from the end.  Absorbing the input
 // block by block as it fills gives the same digest, so the device keeps a running Keccak state plus the pending partial block (at
 // most 33 words: every input is a whole number of 32-bit words) instead of a buffer that grows with the opened values.
+//
+// The third kind is the same HashChallenger over Sha256 (sha256/src/lib.rs), the transcript of the SHA-256 configurations
+// (keccak-air/examples/prove_baby_bear_sha256*.rs): the SHA-256 midstate over the full 64-byte blocks, the pending big-endian message
+// words of the partial block (at most 15), the number of full blocks (for the length in the padding) and the output buffer.
 struct p3gpu_challenger {
-    int kind;           // CH_DUPLEX or CH_KECCAK256
+    int kind;           // CH_DUPLEX, CH_KECCAK256 or CH_SHA256
     int field, width, rate;
     p3::u32 *state;     // device, duplex: [0, width) sponge state | [32, 32+rate) input buffer | [64, 64+rate) output buffer | [96] n_in | [97] n_out
                         //         keccak: [0, 50) Keccak state (lo[25], hi[25]) | [64, 98) pending words | [98] n_pending | [100, 108) output words | [108] n_out words
+                        //         sha256: [0, 8) midstate | [8] full blocks | [64, 80) pending words | [98] n_pending | [100, 108) output = H[0..8) | [108] n_out words
     p3::u32 *stage;     // device staging for host observes / samples (4096 words)
 };
 
 namespace p3 {
 
-constexpr int CH_DUPLEX = 0, CH_KECCAK256 = 1;
+constexpr int CH_DUPLEX = 0, CH_KECCAK256 = 1, CH_SHA256 = 2;
 constexpr int CH_IN = 32, CH_OUT = 64, CH_NIN = 96, CH_NOUT = 97, CH_WORDS = 128, CH_STAGE = 4096;
-constexpr int KCH_PEND = 64, KCH_NPEND = 98, KCH_OUT = 100, KCH_NOUT = 108;
+constexpr int KCH_PEND = 64, KCH_NPEND = 98, KCH_OUT = 100, KCH_NOUT = 108, SCH_BLOCKS = 8;
 
 template <int F, int W>
 __device__ void ch_duplexing(u32 *st, int rate, const Poseidon2Consts &k) {
@@ -195,6 +200,99 @@ __global__ void __launch_bounds__(128) kch_grind_kernel(const u32 *st, u32 base,
     if ((sample & mask) == 0) atomicMin(best, cand);
 }
 
+// ---- SerializingChallenger32<F, HashChallenger<u8, Sha256, 32>> ------------------------------------------------------------
+// The tail of the message after the full blocks: `n` pending words, then `extra` (if has_extra), then the padding for a message of
+// `blocks` full blocks plus the tail.  One or two compressions from the midstate `h`; one inlined copy of the compression.
+__device__ __forceinline__ void sch_finish(u32 (&h)[8], const u32 *pend, u32 n, bool has_extra, u32 extra, u32 blocks) {
+    const u32 tail = n + (has_extra ? 1u : 0u);
+    const u64 nb = sha256_blocks(tail), bits = ((u64)blocks * 16 + tail) * 32;
+#pragma unroll 1
+    for (u64 b = 0; b < nb; b++) {
+        u32 w[16];
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            const u64 j = 16 * b + i;
+            w[i] = j < n ? pend[i] : (j < tail ? extra : sha256_pad_word(j, tail, nb, bits));
+        }
+        sha256_compress(h, w);
+    }
+}
+
+// HashChallenger::flush: the digest's bytes are H big-endian; they become the new input buffer (8 message words = H, the midstate
+// back at the IV) and the output buffer
+__device__ void sch_flush(u32 *st) {
+    u32 h[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) h[i] = st[i];
+    sch_finish(h, st + KCH_PEND, st[KCH_NPEND], false, 0, st[SCH_BLOCKS]);
+#pragma unroll
+    for (int k = 0; k < 8; k++) { st[KCH_PEND + k] = h[k]; st[KCH_OUT + k] = h[k]; st[k] = SHA256_IV[k]; }
+    st[SCH_BLOCKS] = 0;
+    st[KCH_NPEND] = 8;
+    st[KCH_NOUT] = 8;
+}
+
+// four bytes popped from the END of the output buffer: bytes 4m+3, 4m+2, 4m+1, 4m as a little-endian u32, which is H[m]
+__device__ __forceinline__ u32 sch_pop_u32(u32 *st) {
+    if (st[KCH_NOUT] == 0) sch_flush(st);
+    const u32 m = st[KCH_NOUT] - 1;
+    st[KCH_NOUT] = m;
+    return st[KCH_OUT + m];
+}
+
+// MONTY: field elements as the 4 little-endian bytes of their canonical values; otherwise the words' own bytes (a [u8; 32] digest
+// held as 8 words).  Either way the big-endian message word is the byte-swapped value.
+template <int F, bool MONTY>
+__global__ void sch_observe_kernel(u32 *st, const u32 *vals, size_t n) {
+    if (threadIdx.x | blockIdx.x) return;
+    if (n == 0) return;
+    u32 h[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) h[i] = st[i];
+    st[KCH_NOUT] = 0;                                                          // any buffered output is now invalid
+    u32 m = st[KCH_NPEND];
+    for (size_t j = 0; j < n; j++) {
+        st[KCH_PEND + m] = bswap32(MONTY ? from_monty<F>(vals[j]) : vals[j]);
+        if (++m == 16) {
+            u32 w[16];
+#pragma unroll
+            for (int i = 0; i < 16; i++) w[i] = st[KCH_PEND + i];
+            sha256_compress(h, w);
+            st[SCH_BLOCKS]++;
+            m = 0;
+        }
+    }
+    st[KCH_NPEND] = m;
+#pragma unroll
+    for (int i = 0; i < 8; i++) st[i] = h[i];
+}
+
+template <int F>
+__global__ void sch_sample_kernel(u32 *st, u32 *out, size_t n, bool raw, u32 mask) {
+    if (threadIdx.x | blockIdx.x) return;
+    for (size_t j = 0; j < n; j++) {
+        if (raw) { out[j] = sch_pop_u32(st) & mask; continue; }
+        u32 v;
+        do { v = sch_pop_u32(st) & 0x7fffffffu; } while (v >= Fp<F>::P);
+        out[j] = to_monty<F>(v);
+    }
+}
+
+// Candidate c is valid iff observe(c); sample_bits(bits) == 0.  Each thread finishes the hash from the midstate: the pending words,
+// its candidate and the padding, one or two compressions.  The first sampled u32 is H[7].  best = smallest valid c.
+template <int F>
+__global__ void __launch_bounds__(128) sch_grind_kernel(const u32 *st, u32 base, u32 count, u32 mask, u32 *best) {
+    const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= count) return;
+    const u32 cand = base + t;
+    if (cand >= Fp<F>::P) return;
+    u32 h[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) h[i] = st[i];
+    sch_finish(h, st + KCH_PEND, st[KCH_NPEND], true, bswap32(cand), st[SCH_BLOCKS]);
+    if ((h[7] & mask) == 0) atomicMin(best, cand);
+}
+
 template <typename Fn> static int32_t field_dispatch(int field, Fn &&fn) {
     if (field == BABY_BEAR) return fn(std::integral_constant<int, BABY_BEAR>());
     return fn(std::integral_constant<int, KOALA_BEAR>());
@@ -233,6 +331,14 @@ int32_t challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **o
     P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "unknown field %d", field);
     return challenger_alloc(ctx, CH_KECCAK256, field, 0, 0, out);
 }
+// SerializingChallenger32::from_hasher(vec![], Sha256): empty buffers, the midstate at the IV
+int32_t challenger_new_sha256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out) {
+    P3_CHECK(field == BABY_BEAR || field == KOALA_BEAR, P3GPU_EUNSUPPORTED, "unknown field %d", field);
+    static const u32 iv[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+    P3_TRY(challenger_alloc(ctx, CH_SHA256, field, 0, 0, out));
+    P3_CUDA(cudaMemcpyAsync((*out)->state, iv, sizeof iv, cudaMemcpyHostToDevice, ctx->stream));   // pageable source: staged before return
+    return P3GPU_OK;
+}
 void challenger_free(p3gpu_ctx *ctx, p3gpu_challenger *ch) {
     if (!ch) return;
     cudaStreamSynchronize(ctx->stream);
@@ -248,8 +354,15 @@ int32_t challenger_clone(p3gpu_ctx *ctx, const p3gpu_challenger *src, p3gpu_chal
 static int32_t kch_observe_dev(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *d_vals, size_t n, bool monty) {
     if (n == 0) return P3GPU_OK;
     P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
-        if (monty) kch_observe_kernel<decltype(f)::value, true><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
-        else kch_observe_kernel<decltype(f)::value, false><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        constexpr int F = decltype(f)::value;
+        if (ch->kind == CH_SHA256) {
+            if (monty) sch_observe_kernel<F, true><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+            else sch_observe_kernel<F, false><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        } else if (monty) {
+            kch_observe_kernel<F, true><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        } else {
+            kch_observe_kernel<F, false><<<1, 1, 0, ctx->stream>>>(ch->state, d_vals, n);
+        }
         return P3GPU_OK;
     }));
     ctx->launches++;
@@ -257,7 +370,7 @@ static int32_t kch_observe_dev(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *
     return P3GPU_OK;
 }
 int32_t challenger_observe_dev(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *d_vals, size_t n) {
-    if (ch->kind == CH_KECCAK256) return kch_observe_dev(ctx, ch, d_vals, n, true);
+    if (ch->kind != CH_DUPLEX) return kch_observe_dev(ctx, ch, d_vals, n, true);
     if (n == 0) return P3GPU_OK;
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
@@ -292,7 +405,8 @@ int32_t challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u3
 }
 static int32_t kch_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size_t n, bool raw, u32 mask) {
     P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
-        kch_sample_kernel<decltype(f)::value><<<1, 1, 0, ctx->stream>>>(ch->state, ch->stage, n, raw, mask);
+        if (ch->kind == CH_SHA256) sch_sample_kernel<decltype(f)::value><<<1, 1, 0, ctx->stream>>>(ch->state, ch->stage, n, raw, mask);
+        else kch_sample_kernel<decltype(f)::value><<<1, 1, 0, ctx->stream>>>(ch->state, ch->stage, n, raw, mask);
         return P3GPU_OK;
     }));
     ctx->launches++;
@@ -304,7 +418,7 @@ static int32_t kch_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size
 int32_t challenger_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size_t n) {
     P3_CHECK(n <= (size_t)CH_STAGE, P3GPU_EINVAL, "too many samples in one call");
     if (n == 0) return P3GPU_OK;
-    if (ch->kind == CH_KECCAK256) return kch_sample(ctx, ch, h_out, n, false, 0);
+    if (ch->kind != CH_DUPLEX) return kch_sample(ctx, ch, h_out, n, false, 0);
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
     P3_TRY(ch_dispatch(ch->field, ch->width, [&](auto f, auto w) -> int32_t {
@@ -324,7 +438,7 @@ int32_t challenger_sample_bits(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bi
     P3_CHECK(bits < 32 && (1ull << bits) < p, P3GPU_EINVAL, "sample_bits(%u): 2^bits must be below the field order", bits);
     P3_CHECK(n <= (size_t)CH_STAGE, P3GPU_EINVAL, "too many samples in one call");
     if (n == 0) return P3GPU_OK;
-    if (ch->kind == CH_KECCAK256) return kch_sample(ctx, ch, h_out, n, true, (1u << bits) - 1u);
+    if (ch->kind != CH_DUPLEX) return kch_sample(ctx, ch, h_out, n, true, (1u << bits) - 1u);
     P3_TRY(challenger_sample(ctx, ch, h_out, n));
     for (size_t i = 0; i < n; i++)
         h_out[i] = (ch->field == BABY_BEAR ? from_monty<BABY_BEAR>(h_out[i]) : from_monty<KOALA_BEAR>(h_out[i])) & (u32)((1ull << bits) - 1);
@@ -338,7 +452,8 @@ static int32_t kch_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, u3
     for (u64 base = 0; base < p && found == 0xffffffffu; base += batch) {
         P3_CUDA(cudaMemsetAsync(best, 0xff, 4, ctx->stream));
         P3_TRY(field_dispatch(ch->field, [&](auto f) -> int32_t {
-            kch_grind_kernel<decltype(f)::value><<<(batch + 127) / 128, 128, 0, ctx->stream>>>(ch->state, (u32)base, batch, mask, best);
+            if (ch->kind == CH_SHA256) sch_grind_kernel<decltype(f)::value><<<(batch + 127) / 128, 128, 0, ctx->stream>>>(ch->state, (u32)base, batch, mask, best);
+            else kch_grind_kernel<decltype(f)::value><<<(batch + 127) / 128, 128, 0, ctx->stream>>>(ch->state, (u32)base, batch, mask, best);
             return P3GPU_OK;
         }));
         ctx->launches++;
@@ -361,7 +476,7 @@ int32_t challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, u3
     P3_CHECK(bits < 31, P3GPU_EINVAL, "proof-of-work bits %u too large", bits);
     const u32 p = ch->field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
     if (bits == 0) { *witness_monty = 0; return P3GPU_OK; }
-    if (ch->kind == CH_KECCAK256) return kch_grind(ctx, ch, bits, witness_monty);
+    if (ch->kind != CH_DUPLEX) return kch_grind(ctx, ch, bits, witness_monty);
     const Poseidon2Consts *k;
     P3_TRY(ch_consts(ctx, ch, &k));
     u32 *best = ch->stage + CH_STAGE - 1;

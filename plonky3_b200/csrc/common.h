@@ -225,6 +225,7 @@ int32_t challenger_observe_host(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 
 int32_t challenger_sample(p3gpu_ctx *ctx, p3gpu_challenger *ch, u32 *h_out, size_t n);
 int32_t challenger_grind(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, u32 *witness_monty);
 int32_t challenger_new_keccak256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out);
+int32_t challenger_new_sha256(p3gpu_ctx *ctx, int field, p3gpu_challenger **out);
 int32_t challenger_observe_digest(p3gpu_ctx *ctx, p3gpu_challenger *ch, const u32 *h_words, size_t n);
 int32_t challenger_sample_bits(p3gpu_ctx *ctx, p3gpu_challenger *ch, unsigned bits, size_t n, u32 *h_out);
 int32_t query_gather_rows(p3gpu_ctx *ctx, const u32 *d_mat, size_t h, size_t w, const u32 *h_idx, size_t n, unsigned shift, u32 *d_out);

@@ -1,11 +1,12 @@
-// Poseidon2 / Keccak-f sponges and the Merkle-tree builder for sm_90a.
+// Poseidon2 / Keccak-f sponges, SHA-256 and the Merkle-tree builder for sm_90a.
 //
 // Replaces MerkleTree::new (merkle-tree/src/merkle_tree.rs:95-178: first_digest_layer :268-338, compress :490-538,
 // compress_and_inject :348-460) with the hash constructions the reference's MerkleTreeMmcs is instantiated with:
 //   Poseidon2 (poseidon2/src/lib.rs:131-147, external.rs:60-159,288-336, monty-31/src/poseidon2.rs:76-85),
 //   PaddingFreeSponge (symmetric/src/sponge.rs:182-216), TruncatedPermutation (symmetric/src/compression.rs:34-49),
 //   KeccakF + SerializingHasher u64 packing (keccak/src/lib.rs:70-76, field/src/integers.rs:494-509),
-//   CompressionFunctionFromHasher (symmetric/src/compression.rs:60-70).
+//   CompressionFunctionFromHasher (symmetric/src/compression.rs:60-70),
+//   SerializingHasher<Sha256> and Sha256Compress (symmetric/src/serializing_hasher.rs, sha256/src/lib.rs).
 //
 // Mapping: one sponge per thread (state in registers, rounds as loops so that a kernel stays inside the instruction cache, round
 // constants passed as a __grid_constant__ kernel parameter = constant-bank operands).  The permutations themselves live in
@@ -185,6 +186,73 @@ __global__ void __launch_bounds__(128) keccak_compress_kernel(const u32 *in, con
 }
 
 // =================================================================================================
+// SHA-256
+// =================================================================================================
+// leaf = SerializingHasher<Sha256> (symmetric/src/serializing_hasher.rs): the byte stream of the concatenated row is every element's
+// to_unique_u32() — the Montgomery word — as 4 little-endian bytes (monty-31/src/monty_31.rs), so message word j is element j
+// byte-swapped; 16 elements a block, then the padding of a message of `total` words.  One loop over the blocks, so the kernel holds
+// one inlined copy of the compression.  The digest's bytes are the state words big-endian: word k = bswap(H[k]).
+__global__ void __launch_bounds__(128) sha256_leaf_kernel(const __grid_constant__ LeafArgs a) {
+    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= a.height) return;
+    const bool single = (a.n_mats == 1);
+    const u32 w0 = a.width[0];
+    const u32 *row0 = a.ptr[0] + r * w0;
+    u64 total = 0;
+    for (int m = 0; m < a.n_mats; m++) total += a.wid(m);
+    const u64 nb = sha256_blocks(total);
+    RowCursor cur(a, r);
+    u32 st[8];
+    sha256_iv(st);
+    for (u64 b = 0; b < nb; b++) {
+        u32 w[16];
+        const u64 j0 = 16 * b;
+        if (single && j0 + 16 <= total) {                     // a whole block of one row: no per-word tests
+#pragma unroll
+            for (int i = 0; i < 16; i++) w[i] = bswap32(__ldg(row0 + j0 + i));
+        } else {
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                const u64 j = j0 + i;
+                if (j < total) w[i] = bswap32(single ? __ldg(row0 + j) : cur.next());
+                else w[i] = sha256_pad_word(j, total, nb, total * 32);
+            }
+        }
+        sha256_compress(st, w);
+    }
+    uint4 *o = reinterpret_cast<uint4 *>(a.out + r * 8);
+    o[0] = make_uint4(bswap32(st[0]), bswap32(st[1]), bswap32(st[2]), bswap32(st[3]));
+    o[1] = make_uint4(bswap32(st[4]), bswap32(st[5]), bswap32(st[6]), bswap32(st[7]));
+}
+
+// node, same rmode convention as the other compress kernels.  The 64-byte block is left || right (each digest's bytes, i.e. its
+// words byte-swapped).  HASHER: CompressionFunctionFromHasher<Sha256, 2, 32> (symmetric/src/compression.rs) = SHA-256 of the 64
+// bytes: the block, then the constant padding block (0x80, zeros, bit length 512), whose message schedule folds to constants.
+// Otherwise Sha256Compress (sha256/src/lib.rs): one compress256 of the block from H256_256, no padding.
+template <bool HASHER>
+__global__ void __launch_bounds__(128) sha256_compress_kernel(const u32 *in, const u32 *inj, size_t inj_h, u32 *out, size_t n, int rmode) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint4 *l = reinterpret_cast<const uint4 *>(rmode == 0 ? in + 16 * i : out + 8 * i);
+    const uint4 a0 = l[0], a1 = l[1];
+    uint4 b0 = make_uint4(0, 0, 0, 0), b1 = b0;
+    if (rmode == 0) { b0 = l[2]; b1 = l[3]; }
+    else if (i < inj_h) { const uint4 *rp = reinterpret_cast<const uint4 *>(inj + 8 * i); b0 = rp[0]; b1 = rp[1]; }
+    const u32 w[16] = {bswap32(a0.x), bswap32(a0.y), bswap32(a0.z), bswap32(a0.w), bswap32(a1.x), bswap32(a1.y), bswap32(a1.z), bswap32(a1.w),
+                       bswap32(b0.x), bswap32(b0.y), bswap32(b0.z), bswap32(b0.w), bswap32(b1.x), bswap32(b1.y), bswap32(b1.z), bswap32(b1.w)};
+    u32 st[8];
+    sha256_iv(st);
+    sha256_compress(st, w);
+    if (HASHER) {
+        const u32 pad[16] = {0x80000000u, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 512u};
+        sha256_compress(st, pad);
+    }
+    uint4 *o = reinterpret_cast<uint4 *>(out + 8 * i);
+    o[0] = make_uint4(bswap32(st[0]), bswap32(st[1]), bswap32(st[2]), bswap32(st[3]));
+    o[1] = make_uint4(bswap32(st[4]), bswap32(st[5]), bswap32(st[6]), bswap32(st[7]));
+}
+
+// =================================================================================================
 // host side
 // =================================================================================================
 static inline unsigned nblocks(size_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
@@ -225,6 +293,8 @@ static int32_t launch_leaf(p3gpu_ctx *ctx, int field, int hash, const LeafArgs &
     const unsigned g = nblocks(a.height, 128);
     if (hash == P3GPU_HASH_KECCAK) {
         keccak_leaf_kernel<<<g, 128, 0, ctx->stream>>>(a);
+    } else if (hash == P3GPU_HASH_SHA256 || hash == P3GPU_HASH_SHA256_COMPRESS) {
+        sha256_leaf_kernel<<<g, 128, 0, ctx->stream>>>(a);
     } else {
         const Poseidon2Consts *k;
         P3_TRY(get_consts(ctx, field, hash == P3GPU_HASH_POSEIDON2_W24 ? 24 : 16, &k));
@@ -243,6 +313,10 @@ static int32_t launch_compress(p3gpu_ctx *ctx, int field, int hash, const u32 *i
     const unsigned g = nblocks(n, 128);
     if (hash == P3GPU_HASH_KECCAK) {
         keccak_compress_kernel<<<g, 128, 0, ctx->stream>>>(in, inj, inj_h, out, n, rmode);
+    } else if (hash == P3GPU_HASH_SHA256) {
+        sha256_compress_kernel<true><<<g, 128, 0, ctx->stream>>>(in, inj, inj_h, out, n, rmode);
+    } else if (hash == P3GPU_HASH_SHA256_COMPRESS) {
+        sha256_compress_kernel<false><<<g, 128, 0, ctx->stream>>>(in, inj, inj_h, out, n, rmode);
     } else {
         const Poseidon2Consts *k;
         P3_TRY(get_consts(ctx, field, 16, &k));
@@ -275,7 +349,7 @@ static int32_t validate_heights(const size_t *hs, size_t n) {
 
 int32_t hash_merkle_commit(p3gpu_ctx *ctx, int field, int hash, size_t n_mats, const u32 *const *d_mats, const size_t *heights,
                            const size_t *widths, u32 *d_layers, size_t *layer_lens, size_t *n_layers_out) {
-    P3_CHECK(hash >= P3GPU_HASH_POSEIDON2_W16 && hash <= P3GPU_HASH_KECCAK, P3GPU_EUNSUPPORTED, "unknown hash %d", hash);
+    P3_CHECK(hash >= P3GPU_HASH_POSEIDON2_W16 && hash <= P3GPU_HASH_SHA256_COMPRESS, P3GPU_EUNSUPPORTED, "unknown hash %d", hash);
     P3_CHECK(n_mats >= 1, P3GPU_EINVAL, "No matrices given?");
     P3_TRY(validate_heights(heights, n_mats));
     for (size_t i = 0; i < n_mats; i++) P3_CHECK(widths[i] < (1ull << 31), P3GPU_EINVAL, "matrix width too large");
@@ -357,7 +431,7 @@ int32_t hash_merkle_commit(p3gpu_ctx *ctx, int field, int hash, size_t n_mats, c
 // elsewhere (multi-GPU row sharding: every rank compresses the gathered sub-tree roots redundantly).
 int32_t hash_merkle_from_digests(p3gpu_ctx *ctx, int field, int hash, const u32 *d_digests, size_t n, u32 *d_layers,
                                  size_t *layer_lens, size_t *n_layers_out) {
-    P3_CHECK(hash >= P3GPU_HASH_POSEIDON2_W16 && hash <= P3GPU_HASH_KECCAK, P3GPU_EUNSUPPORTED, "unknown hash %d", hash);
+    P3_CHECK(hash >= P3GPU_HASH_POSEIDON2_W16 && hash <= P3GPU_HASH_SHA256_COMPRESS, P3GPU_EUNSUPPORTED, "unknown hash %d", hash);
     P3_CHECK(n >= 1, P3GPU_EINVAL, "no digests");
     size_t n_layers = 0;
     size_t cur_len = padded_len2(n);

@@ -1,7 +1,7 @@
-// The two permutations of the hot path as device functions: Poseidon2 over the 31-bit Montgomery fields (width 16 / 24) and
-// Keccak-f[1600].  Kept apart from the kernels (hash.cu) so that the same source can also be compiled as plain C++ and executed
-// on the host against the CPU oracle (tests/cpp/hash_core_host.cpp): g++ ignores the CUDA attributes, and the one intrinsic used
-// here gets a host body there.
+// The hash primitives of the hot path as device functions: Poseidon2 over the 31-bit Montgomery fields (width 16 / 24),
+// Keccak-f[1600] and the SHA-256 compression.  Kept apart from the kernels (hash.cu) so that the same source can also be compiled
+// as plain C++ and executed on the host against the CPU oracle (tests/cpp/hash_core_host.cpp, keccak256_host.cpp,
+// sha256_host.cpp): g++ ignores the CUDA attributes, and the intrinsics used here get host bodies there.
 #pragma once
 #include "field.cuh"
 #include "poseidon2_consts.h"
@@ -242,6 +242,95 @@ __device__ inline void keccak256(const unsigned char *msg, size_t len, unsigned 
         const u32 v = keccak256_digest_word(s, k);
         for (int j = 0; j < 4; j++) out[4 * k + j] = (unsigned char)(v >> (8 * j));
     }
+}
+
+// =================================================================================================
+// SHA-256 (FIPS 180-4; sha256/src/lib.rs Sha256 = sha2::Sha256, Sha256Compress = one compress256 from H256_256)
+// =================================================================================================
+// The 64 rounds and the 48 schedule words are fully unrolled: the round constants become constant-bank operands and the 16-word
+// schedule window stays in registers under static indices.  A round is 3 funnel-shift rotations + 1 LOP3 for each of Sigma0 and
+// Sigma1, one LOP3 each for Ch and Maj and three IADD3s; a schedule word 2 rotations + 1 shift + 1 LOP3 for each of sigma0 and
+// sigma1 and two IADD3s.  All of it is integer-ALU work.  Message words are big-endian: a 32-bit word holding 4 stream bytes in
+// little-endian order (a field element's bytes, a digest word) enters the block byte-swapped.
+static __constant__ u32 SHA256_K[64] = {
+    0x428a2f98u, 0x71374491u, 0xb5c0fbcfu, 0xe9b5dba5u, 0x3956c25bu, 0x59f111f1u, 0x923f82a4u, 0xab1c5ed5u, 0xd807aa98u, 0x12835b01u,
+    0x243185beu, 0x550c7dc3u, 0x72be5d74u, 0x80deb1feu, 0x9bdc06a7u, 0xc19bf174u, 0xe49b69c1u, 0xefbe4786u, 0x0fc19dc6u, 0x240ca1ccu,
+    0x2de92c6fu, 0x4a7484aau, 0x5cb0a9dcu, 0x76f988dau, 0x983e5152u, 0xa831c66du, 0xb00327c8u, 0xbf597fc7u, 0xc6e00bf3u, 0xd5a79147u,
+    0x06ca6351u, 0x14292967u, 0x27b70a85u, 0x2e1b2138u, 0x4d2c6dfcu, 0x53380d13u, 0x650a7354u, 0x766a0abbu, 0x81c2c92eu, 0x92722c85u,
+    0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u, 0x19a4c116u, 0x1e376c08u,
+    0x2748774cu, 0x34b0bcb5u, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u, 0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u,
+    0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u};
+static __constant__ u32 SHA256_IV[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+
+__device__ __forceinline__ u32 rotr32(u32 x, int r) { return __funnelshift_l(x, x, 32 - r); }
+__device__ __forceinline__ u32 bswap32(u32 x) {
+#ifdef __CUDA_ARCH__
+    return __byte_perm(x, 0, 0x0123);
+#else
+    return __builtin_bswap32(x);
+#endif
+}
+__device__ __forceinline__ void sha256_iv(u32 (&st)[8]) {
+#pragma unroll
+    for (int i = 0; i < 8; i++) st[i] = SHA256_IV[i];
+}
+
+// compress256: st = st + rounds(st, block w) for one 16-word big-endian block
+__device__ __forceinline__ void sha256_compress(u32 (&st)[8], const u32 (&win)[16]) {
+    u32 w[16];
+#pragma unroll
+    for (int i = 0; i < 16; i++) w[i] = win[i];
+    u32 a = st[0], b = st[1], c = st[2], d = st[3], e = st[4], f = st[5], g = st[6], h = st[7];
+#pragma unroll
+    for (int r = 0; r < 64; r++) {
+        const int i = r & 15;
+        if (r >= 16) {
+            const u32 w15 = w[(i + 1) & 15], w2 = w[(i + 14) & 15];
+            const u32 s0 = rotr32(w15, 7) ^ rotr32(w15, 18) ^ (w15 >> 3);
+            const u32 s1 = rotr32(w2, 17) ^ rotr32(w2, 19) ^ (w2 >> 10);
+            w[i] = w[i] + s0 + w[(i + 9) & 15] + s1;
+        }
+        const u32 S1 = rotr32(e, 6) ^ rotr32(e, 11) ^ rotr32(e, 25);
+        const u32 ch = (e & f) ^ (~e & g);
+        const u32 t1 = h + S1 + ch + SHA256_K[r] + w[i];
+        const u32 S0 = rotr32(a, 2) ^ rotr32(a, 13) ^ rotr32(a, 22);
+        const u32 maj = (a & b) ^ (a & c) ^ (b & c);
+        h = g; g = f; f = e; e = d + t1;
+        d = c; c = b; b = a; a = t1 + S0 + maj;
+    }
+    st[0] += a; st[1] += b; st[2] += c; st[3] += d; st[4] += e; st[5] += f; st[6] += g; st[7] += h;
+}
+
+// Word j (j >= n) of the padding after the last n message words, which fill nb blocks with it: 0x80 right after the message (a whole
+// word: every input is a whole number of words), zeros, then the whole message's bit length `bits` as a big-endian u64 in the last
+// two words of block nb - 1.
+__device__ __forceinline__ u32 sha256_pad_word(u64 j, u64 n, u64 nb, u64 bits) {
+    if (j == n) return 0x80000000u;
+    if (j == 16 * nb - 2) return (u32)(bits >> 32);
+    if (j == 16 * nb - 1) return (u32)bits;
+    return 0u;
+}
+// blocks of a padded message of n words: room for the 0x80 word and the two length words
+__device__ __forceinline__ u64 sha256_blocks(u64 n) { return (n + 2) / 16 + 1; }
+
+// SHA-256 of any byte string (the host tests' entry point)
+__device__ inline void sha256(const unsigned char *msg, size_t len, unsigned char out[32]) {
+    u32 st[8];
+    sha256_iv(st);
+    const size_t nb = (len + 9 + 63) / 64;
+    for (size_t blk = 0; blk < nb; blk++) {
+        unsigned char b[64];
+        for (int i = 0; i < 64; i++) {
+            const size_t j = blk * 64 + i;
+            b[i] = j < len ? msg[j] : (j == len ? 0x80 : 0);
+        }
+        if (blk == nb - 1) for (int i = 0; i < 8; i++) b[56 + i] = (unsigned char)(((u64)len * 8) >> (56 - 8 * i));
+        u32 w[16];
+        for (int i = 0; i < 16; i++) w[i] = (u32)b[4 * i] << 24 | (u32)b[4 * i + 1] << 16 | (u32)b[4 * i + 2] << 8 | b[4 * i + 3];
+        sha256_compress(st, w);
+    }
+    for (int k = 0; k < 8; k++)
+        for (int j = 0; j < 4; j++) out[4 * k + j] = (unsigned char)(st[k] >> (24 - 8 * j));
 }
 
 }  // namespace p3

@@ -404,8 +404,8 @@ class ShardedTrace:
     columns [col_starts[g], col_starts[g+1]), and after the sharded commit LDE rows [g R, (g+1) R), R = LDE height / world, with
     its sub-tree.  `uni_stark.prove(config, air, block, shard=ShardedTrace(grp, col_starts))` proves with it any air.KernelAir that
     has a sharded quotient kernel (the Poseidon2 AIR over KoalaBear, the Blake3, SHA-256 and Poseidon1 AIRs), under either
-    configuration: the commit, the exchanges and the openings carry 8-word digests, which is what both the Poseidon2 and the Keccak
-    MMCS write ([F; 8] and [u64; 4]).
+    configuration: the commit, the exchanges and the openings carry 8-word digests, which is what the Poseidon2, the Keccak and the
+    SHA-256 MMCS write ([F; 8], [u64; 4] and [u8; 32]).
 
     It carries out the steps that read the trace's rows.  Ranks exchange data over peer memory only where a value depends on rows
     they do not own, and after every exchange all ranks hold identical bytes, so their transcripts stay identical:
@@ -529,12 +529,13 @@ class ShardedTrace:
 
 
 def sharded_air_error(config, air):
-    """None, or why prove_sharded cannot prove `air` under `config`: it needs a StarkConfig or KeccakStarkConfig and an air.KernelAir
+    """None, or why prove_sharded cannot prove `air` under `config`: it needs a StarkConfig, KeccakStarkConfig or Sha256StarkConfig
+    and an air.KernelAir
     with a sharded quotient kernel whose constraints read the local row only (a row's next row lies on another rank)."""
     from .air import KernelAir
     from .field import KoalaBear
     from .poseidon2_air import VectorizedPoseidon2Air
-    from .uni_stark import KeccakStarkConfig, StarkConfig
+    from .uni_stark import KeccakStarkConfig, Sha256StarkConfig, StarkConfig
     if not isinstance(air, KernelAir):
         return (f"prove_sharded: {type(air).__name__} is a constraint-program AIR; only AIRs with hand-written kernels have a sharded "
                 "quotient")
@@ -546,14 +547,14 @@ def sharded_air_error(config, air):
     if isinstance(air, VectorizedPoseidon2Air) and air.field.id != KoalaBear.id:
         # its sharded quotient kernel reads 16-byte units of 4-column segments; BabyBear's 298-column permutations start mid-unit
         return f"prove_sharded: the Poseidon2 AIR over {air.field.name} has no sharded prove (KoalaBear only)"
-    if not isinstance(config, (StarkConfig, KeccakStarkConfig)):
-        return f"prove_sharded: {type(config).__name__} is not a StarkConfig or KeccakStarkConfig"
+    if not isinstance(config, (StarkConfig, KeccakStarkConfig, Sha256StarkConfig)):
+        return f"prove_sharded: {type(config).__name__} is not a StarkConfig or KeccakStarkConfig, nor a Sha256StarkConfig"
     return None
 
 
 def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
     """uni_stark.prove with the trace sharded by column block over the ranks of `grp` (rank g holds columns [col_starts[g],
-    col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  `config`: StarkConfig or KeccakStarkConfig; `air`: the Poseidon2
+    col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  `config`: StarkConfig, KeccakStarkConfig or Sha256StarkConfig; `air`: the Poseidon2
     AIR over KoalaBear, or the Blake3, SHA-256 or Poseidon1 AIR over either field (sharded_air_error says why another is refused,
     before any device work).  Every rank returns the same Proof, byte for byte the one `uni_stark.prove` writes for the whole trace on
     one GPU; its timings_ms are each span's maximum over the ranks."""

@@ -168,6 +168,8 @@ class MerkleTreeMmcs:
       MerkleTreeMmcs.poseidon2(perm16)            leaf PaddingFreeSponge<Perm16,16,8,8>,  node TruncatedPermutation<Perm16,2,8,16>
       MerkleTreeMmcs.poseidon2(perm16, perm24)    leaf PaddingFreeSponge<Perm24,24,16,8>, node TruncatedPermutation<Perm16,2,8,16>
       MerkleTreeMmcs.keccak(field)                leaf SerializingHasher<PaddingFreeSponge<KeccakF,25,17,4>>, node CompressionFunctionFromHasher
+      MerkleTreeMmcs.sha256(field)                leaf SerializingHasher<Sha256>, node CompressionFunctionFromHasher<Sha256, 2, 32>
+      MerkleTreeMmcs.sha256(field, node="compress")  leaf SerializingHasher<Sha256>, node Sha256Compress
     """
 
     def __init__(self, field: Field, hash_kind: int, cap_height: int = 0, gpu: Optional[Gpu] = None, perms=()):
@@ -184,6 +186,16 @@ class MerkleTreeMmcs:
     @classmethod
     def keccak(cls, field: Field, cap_height: int = 0, gpu=None):
         return cls(field, _lib.HASH_KECCAK, cap_height, gpu)
+
+    @classmethod
+    def sha256(cls, field: Field, cap_height: int = 0, gpu=None, node: str = "hasher"):
+        """MerkleTreeMmcs<F, u8, SerializingHasher<Sha256>, C, 2, 32> (keccak-air/examples/prove_baby_bear_sha256*.rs): `node`
+        "hasher" is C = CompressionFunctionFromHasher<Sha256, 2, 32>, "compress" is C = Sha256Compress.  Digests are [u8; 32], held
+        as 8 words whose little-endian bytes are the digest's bytes."""
+        kinds = {"hasher": _lib.HASH_SHA256, "compress": _lib.HASH_SHA256_COMPRESS}
+        if node not in kinds:
+            raise ValueError(f"unknown SHA-256 node compression {node!r} (\"hasher\" or \"compress\")")
+        return cls(field, kinds[node], cap_height, gpu)
 
     # commit/src/mmcs.rs:42, merkle-tree/src/mmcs/batch.rs:42-64
     def commit(self, inputs: list):

@@ -17,7 +17,9 @@ Layout = serde declaration order, postcard rules:
   F = the 4 little-endian bytes of the Montgomery word (monty-31/src/monty_31.rs:167-179);  EF = 4 F.
 Digests (caps, FRI commit-phase caps, pruned-path sibling hashes) take one of two codecs.  DIGEST_F8, the default: [F; 8] (the
 Poseidon2 MMCS), 8 Montgomery words.  DIGEST_U64X4: [u64; 4] (the Keccak MMCS, examples/src/types.rs:19-35), held as 8 words
-(lo, hi of each u64) and written as 4 postcard varints of at most 10 bytes each.
+(lo, hi of each u64) and written as 4 postcard varints of at most 10 bytes each.  DIGEST_U8X32: [u8; 32] (the SHA-256 MMCS,
+keccak-air/examples/prove_baby_bear_sha256*.rs), held as 8 words whose little-endian bytes are the digest's bytes and written as
+those 32 raw bytes (a postcard array carries no length; the Vec around it keeps its varint length).
 Pinned byte for byte against the reference's committed proof fixture (tests/golden/uni_stark_two_adic_v1.json `postcard_hex`)."""
 from __future__ import annotations
 
@@ -25,7 +27,8 @@ import numpy as np
 
 from .merkle_tree import prune_paths
 
-DIGEST_F8, DIGEST_U64X4 = "f8", "u64x4"
+DIGEST_F8, DIGEST_U64X4, DIGEST_U8X32 = "f8", "u64x4", "u8x32"
+DIGEST_CODECS = (DIGEST_F8, DIGEST_U64X4, DIGEST_U8X32)
 
 
 def _varint(n: int) -> bytes:
@@ -52,7 +55,7 @@ def _vec_of(a, width: int) -> bytes:
 
 def _vec_of_digests(a, digest: str) -> bytes:
     """Vec<digest>: a cap or a pruned path's sibling hashes, (n, 8) words."""
-    if digest == DIGEST_F8:
+    if digest in (DIGEST_F8, DIGEST_U8X32):                        # [u8; 32]: the words' own bytes, no range to respect
         return _vec_of(a, 8)
     if digest != DIGEST_U64X4:
         raise ValueError(f"unknown digest codec {digest!r}")
@@ -66,7 +69,8 @@ def _option_vec_ef(a) -> bytes:
 
 
 def proof_to_postcard(proof, digest: str = DIGEST_F8) -> bytes:
-    """`proof`: plonky3_b200.uni_stark.Proof (non-ZK).  `digest`: DIGEST_F8 or DIGEST_U64X4, the configuration's digest type."""
+    """`proof`: plonky3_b200.uni_stark.Proof (non-ZK).  `digest`: DIGEST_F8, DIGEST_U64X4 or DIGEST_U8X32, the configuration's
+    digest type."""
     vd = lambda a: _vec_of_digests(a, digest)
     out = bytearray()
     out += vd(proof.trace_commit) + vd(proof.quotient_commit) + b"\x00"
@@ -102,7 +106,7 @@ def proof_to_postcard(proof, digest: str = DIGEST_F8) -> bytes:
 
 class _Reader:
     def __init__(self, data: bytes, prime=None, digest: str = DIGEST_F8):
-        if digest not in (DIGEST_F8, DIGEST_U64X4):
+        if digest not in DIGEST_CODECS:
             raise ValueError(f"unknown digest codec {digest!r}")
         self.b, self.pos, self.prime, self.digest = data, 0, prime, digest
 
@@ -134,6 +138,13 @@ class _Reader:
         """Vec<digest> as (n, 8) words."""
         if self.digest == DIGEST_F8:
             return self.vec_of(8)
+        if self.digest == DIGEST_U8X32:                             # 32 raw bytes each, any values
+            n = self.varint()
+            if 32 * n > len(self.b) - self.pos:
+                raise ValueError("truncated proof")
+            a = np.frombuffer(self.b, dtype="<u4", count=8 * n, offset=self.pos).astype(np.uint32).reshape(n, 8)
+            self.pos += 32 * n
+            return a
         n = self.varint()
         if n > len(self.b) - self.pos:                              # every u64 takes at least one byte
             raise ValueError("truncated proof")
@@ -173,8 +184,8 @@ class _Reader:
 def proof_from_postcard(data: bytes, prime=None, digest: str = DIGEST_F8) -> dict:
     """The inverse: every field of the wire proof as arrays of Montgomery words (pruned multiproofs are left pruned — the
     verifier consumes them against its own query indices).  With `prime` given, words >= prime are rejected as the reference's
-    deserialiser rejects them (one field element has one encoding).  Digests (DIGEST_U64X4: 4 u64 varints) come back as (n, 8)
-    words either way.  Raises ValueError on malformed input."""
+    deserialiser rejects them (one field element has one encoding).  Digests (DIGEST_U64X4: 4 u64 varints, DIGEST_U8X32: 32 bytes)
+    come back as (n, 8) words either way.  Raises ValueError on malformed input."""
     r = _Reader(data, prime, digest)
     p = {"trace_commit": r.digests(), "quotient_commit": r.digests()}
     if r.byte() != 0:

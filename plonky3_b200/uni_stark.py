@@ -64,6 +64,18 @@ class KeccakStarkConfig:
 
 
 @dataclass
+class Sha256StarkConfig:
+    """The SHA-256 configurations (keccak-air/examples/prove_baby_bear_sha256.rs, prove_baby_bear_sha256_compress.rs): a SHA-256
+    MMCS (MerkleTreeMmcs.sha256, either node compression) and the transcript SerializingChallenger32<F, HashChallenger<u8, Sha256,
+    32>>.  Its digests are [u8; 32], which the wire form writes as 32 raw bytes (proof_io.DIGEST_U8X32)."""
+    pcs: TwoAdicFriPcs
+    digest_codec: str = "u8x32"
+
+    def initialise_challenger(self) -> SerializingChallenger32:
+        return SerializingChallenger32.from_hasher([], self.pcs.dft.field, self.pcs.dft.gpu, hasher="sha256")
+
+
+@dataclass
 class Proof:
     """uni-stark/src/proof.rs:19-62 + fri/src/proof.rs:12-24 as plain arrays (Montgomery words)."""
     trace_commit: np.ndarray
@@ -84,7 +96,7 @@ class Proof:
     preprocessed_next: Optional[np.ndarray] = None    # ... and its preprocessed_next_row_columns() is not empty
     input_opening_indices: list = dc_field(default_factory=list)     # per input batch: the height-reduced query indices
     commit_phase_indices: list = dc_field(default_factory=list)      # per FRI round: the opened group index of every query
-    digest_codec: str = "f8"                      # how the configuration's digests serialise (proof_io: "f8" [F; 8], "u64x4" [u64; 4])
+    digest_codec: str = "f8"                      # how the configuration's digests serialise (proof_io: "f8" [F; 8], "u64x4" [u64; 4], "u8x32" [u8; 32])
 
     def to_postcard(self) -> bytes:
         """The reference's wire form (`postcard::to_allocvec(&proof)`, uni-stark/tests/fib_air.rs:401-412)."""
@@ -145,7 +157,7 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
 
 
 def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
-    """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig or KeccakStarkConfig — every transcript
+    """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig, KeccakStarkConfig or Sha256StarkConfig — every transcript
     call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air,
     keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air or poseidon1_air.VectorizedPoseidon1Air.  `trace`: device
     (CUDA int32) matrix of height 2^n.  `public_values`: canonical integers.

@@ -108,8 +108,8 @@ def fold_row(e: Ext, index: int, log_height: int, log_arity: int, beta, evals):
 
 
 def _observe_cap(challenger, cap):
-    """Observe a commitment as digests, not as field elements: a byte transcript (SerializingChallenger32 over a Keccak MMCS) absorbs a
-    [u64; 4] digest as its 32 bytes, which the words' canonical values are not.  A transcript without observe_cap only ever sees
+    """Observe a commitment as digests, not as field elements: a byte transcript (SerializingChallenger32 over a Keccak or SHA-256
+    MMCS) absorbs a [u64; 4] or [u8; 32] digest as its 32 bytes, which the words' canonical values are not.  A transcript without observe_cap only ever sees
     [F; 8] digests, which are field elements."""
     getattr(challenger, "observe_cap", challenger.observe_slice)(np.asarray(cap, dtype=np.uint32))
 
@@ -253,7 +253,7 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk=None):
     preprocessed_width(), preprocessed_next_row_columns(), periodic_columns() and takes the keywords preprocessed_local,
     preprocessed_next and periodic_values in its folder.  `preprocessed_vk`: uni_stark.PreprocessedVerifierKey, required iff the AIR
     has preprocessed columns.  `config.digest_codec` (default "f8") selects the wire form of digests: "u64x4" for the Keccak
-    configuration (uni_stark.KeccakStarkConfig).  Returns None; raises VerificationError."""
+    configuration (uni_stark.KeccakStarkConfig), "u8x32" for the SHA-256 configurations (uni_stark.Sha256StarkConfig).  Returns None; raises VerificationError."""
     from .uni_stark import get_log_num_quotient_chunks
     digest = getattr(config, "digest_codec", "f8")                # [F; 8] digests unless the configuration says otherwise
     if hasattr(proof, "to_postcard"):

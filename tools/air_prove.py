@@ -6,6 +6,12 @@ cap height 3.  One configuration per process:
     python tools/air_prove.py --air sha256 --field koala-bear --config keccak [--log-rows 18] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air poseidon1 --field koala-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
     python tools/air_prove.py --air poseidon2 --field baby-bear --config keccak [--log-rows 20] [--reps 3] [--kernel-reps 10]
+    python tools/air_prove.py --air keccak --field baby-bear --config sha256 --fri benchmark --log-rows 15
+
+  --config   keccak (Keccak MMCS, Keccak-256 transcript), poseidon2 (Poseidon2 MMCS, duplex transcript), sha256 / sha256-compress
+             (SHA-256 MMCS with CompressionFunctionFromHasher<Sha256> or Sha256Compress nodes, SHA-256 transcript: the reference's
+             prove_baby_bear_sha256 / _sha256_compress, whose KeccakAir statement is `--air keccak --fri benchmark --log-rows 15`)
+  --fri      high-arity (new_benchmark_high_arity, the default) or benchmark (new_benchmark: arity 2)
 
   keccak   `-o keccak-f-permutations -l 20`: 43,690 hashes, a 2^20 x 2633 trace (the trace and its LDE take 33 GB together)
   blake3   `-o blake-3-permutations` at 2^18 compressions, a 2^18 x 9168 trace (29 GB with its LDE; the reference's `-l 20`
@@ -42,7 +48,7 @@ from plonky3_b200.fri import FriParameters, TwoAdicFriPcs
 from plonky3_b200.gpu import default_gpu
 from plonky3_b200.merkle_tree import MerkleTreeMmcs
 from plonky3_b200.poseidon2 import default_poseidon2
-from plonky3_b200.uni_stark import KeccakStarkConfig, StarkConfig, prove, verify
+from plonky3_b200.uni_stark import KeccakStarkConfig, Sha256StarkConfig, StarkConfig, prove, verify
 
 DATASHEET_HBM_BYTES_PER_S = 3.35e12          # NVIDIA H100 SXM data sheet, HBM3
 
@@ -103,7 +109,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--air", choices=sorted(AIRS), required=True)
     ap.add_argument("--field", choices=["koala-bear", "baby-bear"], default="koala-bear")
-    ap.add_argument("--config", choices=["keccak", "poseidon2"], default="keccak")
+    ap.add_argument("--config", choices=["keccak", "poseidon2", "sha256", "sha256-compress"], default="keccak")
+    ap.add_argument("--fri", choices=["high-arity", "benchmark"], default="high-arity")
     ap.add_argument("--log-rows", type=int, default=None, help="trace height (default: 20 for keccak and poseidon1/2, 18 for blake3 and sha256)")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--kernel-reps", type=int, default=10)
@@ -112,13 +119,17 @@ def main():
     log_rows = default_log_rows if a.log_rows is None else a.log_rows
     f = KoalaBear if a.field == "koala-bear" else BabyBear
     gpu = default_gpu(0)
+    fri = FriParameters.new_benchmark if a.fri == "benchmark" else FriParameters.new_benchmark_high_arity
     if a.config == "keccak":
         m = MerkleTreeMmcs.keccak(f, cap_height=3, gpu=gpu)
-        config = KeccakStarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, FriParameters.new_benchmark_high_arity(m)))
+        config = KeccakStarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, fri(m)))
+    elif a.config in ("sha256", "sha256-compress"):
+        m = MerkleTreeMmcs.sha256(f, cap_height=3, gpu=gpu, node="compress" if a.config == "sha256-compress" else "hasher")
+        config = Sha256StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, fri(m)))
     else:
         p16, p24 = default_poseidon2(f, 16), default_poseidon2(f, 24)
         m = MerkleTreeMmcs.poseidon2(p16, p24, cap_height=3, gpu=gpu)
-        config = StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, FriParameters.new_benchmark_high_arity(m)), p24, 16)
+        config = StarkConfig(TwoAdicFriPcs(Radix2DitParallel(f, gpu), m, fri(m)), p24, 16)
     air = Air(f, gpu)
     n = hashes(log_rows)
     inputs = torch.from_numpy(random_inputs(f, n).view(dtype)).cuda()
@@ -152,7 +163,7 @@ def main():
     verify(config, Air(f), raw)
     verify_ms = (time.perf_counter() - t0) * 1e3
     print(json.dumps({
-        "card_and_power_limit": _card(), "air": a.air, "field": a.field, "config": a.config, "hashes": n, "trace_rows": 1 << log_rows,
+        "card_and_power_limit": _card(), "air": a.air, "field": a.field, "config": a.config, "fri": a.fri, "hashes": n, "trace_rows": 1 << log_rows,
         "width": air.width(), "trace_generation_ms": round(gen_ms, 3), "trace_bytes_written": trace_bytes,
         "trace_generation_bytes_per_s": float("%.3g" % (trace_bytes / gen_ms * 1e3)),
         "quotient_kernel_ms": round(q_ms, 3), "quotient_lde_bytes_read": lde_bytes,

@@ -229,6 +229,16 @@ unsafe extern "C" {
                                          log_periodic_rows: c_uint, log_quotient_size: c_uint, log_trace_height: c_uint,
                                          public_values: *const u32, alpha: *const u32, d_quotient: *mut u32) -> i32;
 
+    // the debug constraint check of any AIR over the trace domain (pass 1: per-row failure counts; pass 2: the listed rows' failures)
+    pub fn p3gpu_air_check_program_create(ctx: *mut P3GpuCtx, field: c_int, nodes: *const P3GpuAirNode, n_nodes: usize,
+                                          constraints: *const u32, n_constraints: usize, layout: *const P3GpuAirLayout,
+                                          out: *mut *mut P3GpuAirProgram) -> i32;
+    pub fn p3gpu_air_check_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, d_trace: *const u32, height: usize, d_preprocessed: *const u32,
+                               d_periodic: *const u32, periodic_rows: usize, public_values: *const u32, d_counts: *mut u32) -> i32;
+    pub fn p3gpu_air_check_rows_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, d_trace: *const u32, height: usize,
+                                    d_preprocessed: *const u32, d_periodic: *const u32, periodic_rows: usize, public_values: *const u32,
+                                    d_rows: *const u32, n_rows: usize, d_offsets: *const u64, d_failed: *mut u32) -> i32;
+
     // DuplexChallenger with device-resident state
     pub fn p3gpu_challenger_new(ctx: *mut P3GpuCtx, field: c_int, width: c_int, rate: c_int, out: *mut *mut P3GpuChallenger) -> i32;
     pub fn p3gpu_challenger_free(ctx: *mut P3GpuCtx, ch: *mut P3GpuChallenger);

@@ -387,6 +387,38 @@ int32_t p3gpu_air_quotient_layout_dev(p3gpu_ctx *ctx, const p3gpu_air_program *p
                                       unsigned log_periodic_rows, unsigned log_quotient_size, unsigned log_trace_height,
                                       const uint32_t *public_values, const uint32_t alpha[4], uint32_t *d_quotient);
 
+/* ---- the debug constraint check of any AIR (DESIGN.md section 4.14) ---------------------------------------------------------
+ * p3_air::check_constraints / check_all_constraints (air/src/check_constraints.rs:429-627) on the device: every constraint of the
+ * program evaluated on every row of the trace, with the reference's debug semantics over the trace domain.  Row i is read in natural
+ * order, its next row is (i + 1) mod height for any height >= 1 (main and preprocessed trace alike); the selectors are
+ * is_first_row = [i = 0], is_last_row = [i = height - 1], is_transition = [i != height - 1] as Montgomery 0 / 1; periodic column k
+ * at row i is row i mod periodic_rows of the periodic table; public values as for the quotient.  A constraint fails on a row when
+ * its value there is non-zero. */
+/* As p3gpu_air_program_create_layout (the same P3GPU_EINVAL cases), for a check program.  A check program has no alpha table and
+ * keeps its slots in global memory, so it has no constraint limit of its own (beyond the 28-bit field of its instructions) and its
+ * only slot limit is the 16-bit operand field: P3GPU_EUNSUPPORTED beyond 65,535 simultaneously live values.  Only the check entry
+ * points run it: p3gpu_air_quotient_dev / _layout_dev refuse it with P3GPU_EINVAL.  p3gpu_air_program_info and
+ * p3gpu_air_program_destroy take both kinds of program. */
+int32_t p3gpu_air_check_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                       size_t n_constraints, const p3gpu_air_layout *layout, p3gpu_air_program **out);
+/* Pass 1: d_counts[i] = the number of constraints failing on row i, for every row i < height.
+ *   d_trace          height x width Montgomery words, row-major (natural order)
+ *   d_preprocessed   height x preprocessed_width, row-major; NULL iff the layout has no preprocessed columns
+ *   d_periodic       periodic_rows x n_periodic, row-major: every periodic column repeated to periodic_rows rows (the largest
+ *                    period); NULL iff the layout has no periodic columns, else periodic_rows >= 1
+ *   public_values    n_public canonical Montgomery words (host)
+ * P3GPU_EINVAL before anything launches: a quotient program, height 0 or > 2^31, inputs given / missing against the layout,
+ * a non-canonical public value, a misaligned buffer. */
+int32_t p3gpu_air_check_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_trace, size_t height, const uint32_t *d_preprocessed,
+                            const uint32_t *d_periodic, size_t periodic_rows, const uint32_t *public_values, uint32_t *d_counts);
+/* Pass 2: for each listed row j < n_rows, the indices of the constraints failing on row d_rows[j], in ascending order, at
+ * d_failed[d_offsets[j]] onward (one thread walks one row); nothing else of d_failed is written.  The caller sizes the ranges from
+ * pass 1's counts.  Inputs and P3GPU_EINVAL as for pass 1, and a listed row >= height, before anything launches; n_rows = 0 launches
+ * nothing. */
+int32_t p3gpu_air_check_rows_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_trace, size_t height,
+                                 const uint32_t *d_preprocessed, const uint32_t *d_periodic, size_t periodic_rows, const uint32_t *public_values,
+                                 const uint32_t *d_rows, size_t n_rows, const uint64_t *d_offsets, uint32_t *d_failed);
+
 /* ---- transcript and query phase of the prove driver (SURVEY.md 8f rank 4 / N1) ----------------------------------------
  * DuplexChallenger<F, Poseidon2<width>, width, rate> (challenger/src/duplex_challenger.rs:60-300) with its state resident on the
  * device, so that caps and opened values produced on the GPU are absorbed without a PCIe round trip per duplexing.  The

@@ -35,6 +35,7 @@ EXPORTS = [
     "p3gpu_p2air_generate_trace_cols_dev", "p3gpu_shard_col_segments", "p3gpu_peer_exchange_dev", "p3gpu_p2air_quotient_sharded_dev",
     "p3gpu_air_program_create", "p3gpu_air_program_destroy", "p3gpu_air_program_info", "p3gpu_air_quotient_dev",
     "p3gpu_air_program_create_layout", "p3gpu_air_quotient_layout_dev",
+    "p3gpu_air_check_program_create", "p3gpu_air_check_dev", "p3gpu_air_check_rows_dev",
     "p3gpu_challenger_new_keccak256", "p3gpu_challenger_observe_digest", "p3gpu_challenger_sample_bits",
     "p3gpu_challenger_new_sha256",
     "p3gpu_keccak_air_generate_trace_dev", "p3gpu_keccak_air_quotient_dev",
@@ -142,6 +143,9 @@ def load():
         "p3gpu_air_quotient_dev": (i32, [vp, vp, vp, cu, cu, cu, vp, vp, vp]),
         "p3gpu_air_program_create_layout": (i32, [vp, ci, vp, sz, vp, sz, vp, C.POINTER(vp)]),
         "p3gpu_air_quotient_layout_dev": (i32, [vp, vp, vp, cu, vp, cu, vp, cu, cu, cu, vp, vp, vp]),
+        "p3gpu_air_check_program_create": (i32, [vp, ci, vp, sz, vp, sz, vp, C.POINTER(vp)]),
+        "p3gpu_air_check_dev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp]),
+        "p3gpu_air_check_rows_dev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, sz, vp, vp]),
         "p3gpu_challenger_new_keccak256": (i32, [vp, ci, C.POINTER(vp)]),
         "p3gpu_challenger_new_sha256": (i32, [vp, ci, C.POINTER(vp)]),
         "p3gpu_challenger_observe_digest": (i32, [vp, vp, vp, sz]),

@@ -20,11 +20,17 @@ Preprocessed columns (`preprocessed_trace=`, read as `b.preprocessed().local[c]`
 each period a power of two) are evaluated on the quotient domain from a small table the AIR builds on the device
 (`periodic_table`, fri/src/periodic.rs).
 
+`check_constraints` / `check_all_constraints` (air/src/check_constraints.rs:429-627) evaluate every constraint on every row of a
+trace on the device, with the reference's debug semantics over the trace domain, and name the failing rows and constraints;
+`uni_stark.prove(..., check_constraints=True)` runs the first before committing.  Assertions may carry labels
+(`assert_zero_named`, air/src/named.rs), which the reports show.
+
 Not offered: extension-field constraints (assert_zero_ext), ZK.
 """
 from __future__ import annotations
 
-from typing import Callable, Optional, Sequence
+from dataclasses import dataclass
+from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 
@@ -114,6 +120,19 @@ class _Ops:
         x = self._root._e(x)
         self.assert_zero(x * (x - 1))
 
+    # NamedAirBuilder (air/src/named.rs:127-190): the same constraint, with a label kept as host metadata for the check's reports
+    def assert_zero_named(self, x, name):
+        k = len(self._root.constraints)
+        self.assert_zero(x)
+        self._root.labels[k] = str(name)
+
+    def assert_eq_named(self, x, y, name): self.assert_zero_named(self._root._e(x) - y, name)
+    def assert_one_named(self, x, name): self.assert_zero_named(self._root._e(x) - 1, name)
+
+    def assert_bool_named(self, x, name):
+        x = self._root._e(x)
+        self.assert_zero_named(x * (x - 1), name)
+
     def when(self, cond): return _Filtered(self, self._root._e(cond))
     def when_first_row(self): return self.when(self._root.is_first_row())
     def when_last_row(self): return self.when(self._root.is_last_row())
@@ -147,6 +166,7 @@ class SymbolicAirBuilder(_Ops):
         self.nodes: list = []          # (op, a, b, imm)
         self.degrees: list = []
         self.constraints: list = []    # node indices in assertion order
+        self.labels: dict = {}         # constraint index -> label of a named assertion
         self._memo: dict = {}
 
     def _e(self, x) -> Expr:
@@ -249,6 +269,7 @@ class SymbolicAir:
             raise ValueError("the constraints read the preprocessed next row but preprocessed_next_row_columns() is empty")
         self._degree_hint = max_constraint_degree
         self._program = None
+        self._check_program = None
         self._periodic_tables = {}
 
     # ---- BaseAir / the degree the quotient is split by
@@ -293,6 +314,18 @@ class SymbolicAir:
             else:
                 self._program = self.gpu.air_program_create(self.field.id, self.nodes, self.constraints, self.width(), self.num_public_values())
         return self._program
+
+    def check_program(self):
+        """The AIR's constraints compiled for the debug check (p3gpu_air_check_program_create): no constraint limit, up to 65,535
+        slots, so every hand-written AIR's DAG compiles too."""
+        self._need_gpu("the constraint check")
+        if self._check_program is None:
+            layout = (self.width(), self.num_public_values(), self.preprocessed_width(), self.num_periodic_columns())
+            self._check_program = self.gpu.air_check_program_create(self.field.id, self.nodes, self.constraints, layout)
+        return self._check_program
+
+    def constraint_label(self, k: int) -> Optional[str]:
+        return self.builder.labels.get(int(k))
 
     def periodic_table(self, log_degree: int, log_quotient_size: int):
         """build_periodic_lde_table_two_adic (fri/src/periodic.rs:43-160) on the device: every column padded to the largest period
@@ -376,6 +409,121 @@ class SymbolicAir:
         for c in self.builder.constraints:
             acc = e.add(e.mul(acc, alpha), vals[c])
         return acc
+
+
+@dataclass(frozen=True)
+class ConstraintFailure:
+    """One violated constraint (air/src/check_constraints.rs ConstraintFailure): the row, the constraint's index in assertion order
+    and the label of a named assertion."""
+    row: int
+    constraint: int
+    label: Optional[str] = None
+
+    def __str__(self):
+        if self.label is None:
+            return f"#{self.constraint}"
+        return f"#{self.constraint} " + '"' + self.label.replace("\\", "\\\\").replace('"', '\\"') + '"'
+
+
+@dataclass
+class ConstraintReport:
+    """check_all_constraints' result (ConstraintReport): the failures in row order, each row's in constraint order."""
+    failures: List[ConstraintFailure]
+    total_rows: int
+    total_constraints_per_row: int
+
+    def is_ok(self) -> bool:
+        return not self.failures
+
+
+class ConstraintViolation(ValueError):
+    """check_constraints' failure: the first failing row and every constraint that failed on it."""
+
+    def __init__(self, row: int, failures: List[ConstraintFailure]):
+        self.row, self.failures = int(row), list(failures)
+        super().__init__(f"constraints not satisfied on row {self.row}: failed constraints = [{', '.join(map(str, self.failures))}]")
+
+
+def _device_matrix(air, m, what):
+    """`m` (host numpy or device matrix of Montgomery words) as a contiguous int32 tensor on the AIR's device."""
+    import torch
+    if not isinstance(m, torch.Tensor):
+        m = torch.from_numpy(np.ascontiguousarray(m, dtype=np.uint32).view(np.int32))
+    if m.dim() != 2:
+        raise ValueError(f"{what}: a matrix, got shape {tuple(m.shape)}")
+    return air._to_device(m.to(torch.int32).contiguous())
+
+
+def _check_inputs(air, trace, public_values):
+    """What both passes read: the trace, the preprocessed trace (height checked as the reference asserts), the periodic table
+    (each column repeated to the largest period) and the public values (Montgomery)."""
+    air._need_gpu("the constraint check")
+    if int(trace.dim()) != 2 or int(trace.shape[1]) != air.width():
+        raise ValueError(f"trace of shape {tuple(trace.shape)}: the AIR has {air.width()} columns")
+    height = int(trace.shape[0])
+    if height < 1:
+        raise ValueError("the trace has no rows")
+    if len(public_values) != air.num_public_values():
+        raise ValueError(f"{len(public_values)} public values given, the AIR has {air.num_public_values()}")
+    pre = None
+    if air.preprocessed_width() > 0:
+        pre = _device_matrix(air, air.preprocessed_trace(), "preprocessed trace")
+        if int(pre.shape[0]) != height:
+            raise ValueError(f"the constraint check needs the preprocessed trace height ({int(pre.shape[0])}) to match the trace "
+                             f"height ({height})")
+    per = None
+    cols = air.periodic_columns()
+    if cols:
+        p_max = max(len(c) for c in cols)
+        padded = np.array([[c[i % len(c)] for c in cols] for i in range(p_max)], dtype=np.uint64)
+        per = _device_matrix(air, air.field.to_monty_array(padded).astype(np.uint32), "periodic table")
+    pv = [air.field.to_monty(int(v) % air.field.P) for v in public_values]
+    return height, pre, per, pv
+
+
+def _failures(air, trace, public_values, max_failures):
+    """Both passes: the per-row counts on the device, then the failing constraints of the rows check_all_constraints would visit
+    with this cap (the cap is tested before each row), selected on the device."""
+    import torch
+    height, pre, per, pv = _check_inputs(air, trace, public_values)
+    prog, gpu = air.check_program(), air.gpu
+    counts = gpu.air_check_counts(prog, trace, pre, per, pv).to(torch.int64)
+    ends = torch.cumsum(counts, 0)
+    before = ends - counts                                         # failures in the rows above each row
+    keep = counts > 0
+    if max_failures is not None:
+        keep &= before < int(max_failures)
+    rows = torch.nonzero(keep).flatten()
+    n_rows = int(rows.numel())
+    if n_rows == 0:
+        return height, []
+    offsets = (before[rows] - before[rows[0]]).contiguous()
+    per_row = counts[rows]
+    total = int(offsets[-1] + per_row[-1])
+    failed = gpu.air_check_rows(prog, trace, pre, per, pv, rows.to(torch.int32).contiguous(), offsets, total)
+    rows_h, per_row_h, failed_h = rows.cpu().numpy(), per_row.cpu().numpy(), failed.cpu().numpy()
+    out, at = [], 0
+    for r, c in zip(rows_h.tolist(), per_row_h.tolist()):
+        out.extend(ConstraintFailure(r, k, air.constraint_label(k)) for k in failed_h[at:at + c].tolist())
+        at += c
+    return height, out
+
+
+def check_all_constraints(air: "SymbolicAir", trace, public_values=(), max_failures: Optional[int] = None) -> ConstraintReport:
+    """p3_air::check_all_constraints (air/src/check_constraints.rs:528-627) on the device: every constraint on every row of `trace`
+    (a device int32 matrix of Montgomery words, any height >= 1, as for `prove`).  `public_values`: canonical integers.  With
+    `max_failures`, rows stop being visited once that many failures are collected; the cap is tested between rows, so the last
+    row's failures may overshoot it."""
+    height, failures = _failures(air, trace, public_values, max_failures)
+    return ConstraintReport(failures, height, len(air.constraints))
+
+
+def check_constraints(air: "SymbolicAir", trace, public_values=()) -> None:
+    """p3_air::check_constraints (air/src/check_constraints.rs:429-505) on the device: raises ConstraintViolation naming the first
+    row with a failing constraint and every constraint that fails there."""
+    _, failures = _failures(air, trace, public_values, 1)
+    if failures:
+        raise ConstraintViolation(failures[0].row, failures)
 
 
 class KernelAir(SymbolicAir):

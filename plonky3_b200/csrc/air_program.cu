@@ -12,12 +12,6 @@
 #include "common.h"
 #include "air_program.cuh"
 
-struct p3gpu_air_program {
-    int device = 0;
-    p3::AirProgram prog;
-    p3::AirInsn *d_insns = nullptr;
-};
-
 namespace p3 {
 
 struct AirQArgs {
@@ -75,14 +69,15 @@ template <int F, bool EXT> __global__ void __launch_bounds__(AIR_BLOCK) air_prog
 }
 
 int32_t air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const u32 *constraints, size_t n_constraints,
-                           const p3gpu_air_layout &layout, p3gpu_air_program **out) {
+                           const p3gpu_air_layout &layout, p3gpu_air_program **out, bool check) {
     std::string err;
     AirProgram prog;
     const int32_t rc = air_compile(field, nodes, n_nodes, constraints, n_constraints, layout.width, layout.n_public, layout.preprocessed_width,
-                                   layout.n_periodic, prog, err);
+                                   layout.n_periodic, prog, err, check ? AIR_CHECK_LIMITS : AIR_QUOTIENT_LIMITS);
     P3_CHECK(rc == P3GPU_OK, rc, "%s", err.c_str());
     std::unique_ptr<p3gpu_air_program> p(new p3gpu_air_program);
     p->device = ctx->device;
+    p->check = check;
     P3_CUDA(cudaMalloc(&p->d_insns, std::max<size_t>(prog.insns.size(), 1) * sizeof(AirInsn)));
     if (!prog.insns.empty())
         P3_CUDA(cudaMemcpy(p->d_insns, prog.insns.data(), prog.insns.size() * sizeof(AirInsn), cudaMemcpyHostToDevice));
@@ -153,6 +148,8 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const 
                              const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs,
                              const u32 *alpha, u32 *d_q, bool layout_entry) {
     P3_CHECK(pg->device == ctx->device, P3GPU_EINVAL, "AIR program was created on device %d, the context is on device %d", pg->device, ctx->device);
+    P3_CHECK(!pg->check, P3GPU_EINVAL,
+             "the AIR program was created with p3gpu_air_check_program_create: evaluate the quotient of a p3gpu_air_program_create program");
     const AirProgram &p = pg->prog;
     const int field = p.field;
     P3_CHECK(layout_entry || (p.pre_width == 0 && p.n_periodic == 0), P3GPU_EINVAL,

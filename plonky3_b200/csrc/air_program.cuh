@@ -1,9 +1,11 @@
 // Constraint programs: an AIR given as a symbolic expression DAG (the reference's SymbolicExpression, air/src/symbolic/expression.rs),
-// compiled once into a register program that air_program.cu's quotient kernel interprets over the quotient domain.
+// compiled once into a register program that air_program.cu's quotient kernel interprets over the quotient domain and
+// air_check.cu's check kernel interprets over the trace domain.
 //
-// This header holds everything that is not a CUDA launch — the node validation, the compiler, the per-instruction semantics and
-// the per-row quotient evaluation — so host C++ can include it (tests/cpp/air_program_check.cpp and, for the EXT instance,
-// tests/cpp/air_layout_check.cpp run it against the oracle on the CPU) exactly as the kernel does.
+// This header holds everything that is not a CUDA launch — the node validation, the compiler, the per-instruction semantics, the
+// per-row quotient evaluation and the per-row constraint check — so host C++ can include it (tests/cpp/air_program_check.cpp and,
+// for the EXT instance, tests/cpp/air_layout_check.cpp run the quotient against the oracle on the CPU, tests/cpp/air_check_host.cpp
+// the check) exactly as the kernels do.
 //
 //   nodes        p3gpu_air_node {op, a, b, imm} in topological order (operands refer only to earlier nodes)
 //   compile      drop dead nodes; per constraint in assertion order emit its not yet emitted cone (post-order), then FOLD it;
@@ -28,6 +30,11 @@ constexpr u32 AIR_OP_FOLD = 11;                 // instruction-only op, after th
 constexpr u32 AIR_OP_PRE_LOCAL = 12, AIR_OP_PRE_NEXT = 13, AIR_OP_PERIODIC = 14;     // P3GPU_AIR_PREPROCESSED_LOCAL / _NEXT, PERIODIC
 constexpr u32 AIR_MAX_SLOTS = 384;              // 384 slots x 128 threads x 4 B = 192 KiB of shared memory per block
 constexpr u32 AIR_MAX_CONSTRAINTS = 2048;       // alpha-power table: 32 KiB of shared memory
+// A check program (air_check.cu) has no alpha table and keeps its slots in global memory: its limits are the instruction fields'
+// (16-bit slot operands, 28-bit FOLD constraint index).
+constexpr u32 AIR_CHECK_MAX_SLOTS = 65535, AIR_CHECK_MAX_CONSTRAINTS = (1u << 28) - 1;
+struct AirLimits { u32 max_slots, max_constraints; };
+constexpr AirLimits AIR_QUOTIENT_LIMITS = {AIR_MAX_SLOTS, AIR_MAX_CONSTRAINTS}, AIR_CHECK_LIMITS = {AIR_CHECK_MAX_SLOTS, AIR_CHECK_MAX_CONSTRAINTS};
 constexpr u32 AIR_BLOCK = 128;
 constexpr unsigned AIR_MAX_RATE_BITS = 8;       // q = log_quotient_size - log_trace_height <= 8: Z_H tables of <= 256 entries
 
@@ -45,13 +52,27 @@ struct AirProgram {
     std::vector<AirInsn> insns;
 };
 
+}  // namespace p3
+
+// A compiled program on the device: a quotient program (p3gpu_air_program_create*) or a check program
+// (p3gpu_air_check_program_create), which only the check entry points run.
+struct p3gpu_air_program {
+    int device = 0;
+    bool check = false;
+    p3::AirProgram prog;
+    p3::AirInsn *d_insns = nullptr;
+};
+
+namespace p3 {
+
 inline size_t air_smem_bytes(u32 n_slots, u32 n_constraints) { return (size_t)n_constraints * 16 + (size_t)n_slots * AIR_BLOCK * 4; }
 
 // Validates the node list and compiles it.  Returns P3GPU_OK, P3GPU_EINVAL (malformed nodes / constraints) or P3GPU_EUNSUPPORTED
-// (beyond the slot or constraint limit); `err` says why.
+// (beyond the slot or constraint limit of `lim`); `err` says why.
 // pre_width / n_periodic: the preprocessed columns and periodic columns the leaves may read (0: none).
 inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints, size_t n_constraints,
-                           u32 width, u32 n_public, u32 pre_width, u32 n_periodic, AirProgram &out, std::string &err) {
+                           u32 width, u32 n_public, u32 pre_width, u32 n_periodic, AirProgram &out, std::string &err,
+                           const AirLimits &lim = AIR_QUOTIENT_LIMITS) {
     auto fail = [&](int32_t code, const std::string &m) { err = m; return code; };
     if (field != BABY_BEAR && field != KOALA_BEAR) return fail(P3GPU_EUNSUPPORTED, "AIR program: unsupported field " + std::to_string(field));
     const u32 P = field == BABY_BEAR ? Fp<BABY_BEAR>::P : Fp<KOALA_BEAR>::P;
@@ -94,8 +115,8 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
     for (size_t k = 0; k < n_constraints; k++)
         if (constraints[k] >= n_nodes) return fail(P3GPU_EINVAL, "AIR program: constraint " + std::to_string(k) + " names node " +
                                                                std::to_string(constraints[k]) + " of " + std::to_string(n_nodes));
-    if (n_constraints > AIR_MAX_CONSTRAINTS)
-        return fail(P3GPU_EUNSUPPORTED, "AIR program: " + std::to_string(n_constraints) + " constraints (at most " + std::to_string(AIR_MAX_CONSTRAINTS) + ")");
+    if (n_constraints > lim.max_constraints)
+        return fail(P3GPU_EUNSUPPORTED, "AIR program: " + std::to_string(n_constraints) + " constraints (at most " + std::to_string(lim.max_constraints) + ")");
 
     auto is_binary = [](u32 op) { return op == P3GPU_AIR_ADD || op == P3GPU_AIR_SUB || op == P3GPU_AIR_MUL; };
     // schedule: events are node indices (compute) or ~k (fold constraint k)
@@ -164,8 +185,8 @@ inline int32_t air_compile(int field, const p3gpu_air_node *nodes, size_t n_node
         if (free_slots.empty()) free_slots.push_back(prog.n_slots++);
         slot[i] = free_slots.back();
         free_slots.pop_back();
-        if (prog.n_slots > AIR_MAX_SLOTS)
-            return fail(P3GPU_EUNSUPPORTED, "AIR program: more than " + std::to_string(AIR_MAX_SLOTS) + " simultaneously live values (slots)");
+        if (prog.n_slots > lim.max_slots)
+            return fail(P3GPU_EUNSUPPORTED, "AIR program: more than " + std::to_string(lim.max_slots) + " simultaneously live values (slots)");
         prog.insns.push_back({op | (slot[i] << 4), arg});
     }
     out = std::move(prog);
@@ -300,6 +321,40 @@ template <int F> __device__ __forceinline__ void air_warp_store(const AirHandQAr
 __device__ __forceinline__ u32 air_shard_odd(const AirHandQArgs &a, u32 m) { return ((a.row0 + m) >> (a.d.log_q - 1)) & 1u; }
 #endif
 
+// Decodes one instruction: every opcode but FOLD computes its value into v and returns false, for the caller to store in slot dst;
+// a FOLD returns true and is the caller's (the quotient accumulates it against an alpha power, the check tests it for zero).  The
+// one copy of each opcode's semantics.  Env supplies slot(s), local(c), next(c), pub(k) and, with EXT (opcodes 12-14), pre_local(c), pre_next(c) and
+// periodic(k); first / last / trans are the selectors' values at the row.
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <int F, bool EXT, class Env>
+__host__ __device__ __forceinline__ bool air_decode(Env &env, const AirInsn in, u32 first, u32 last, u32 trans, u32 &v) {
+    const u32 op = in.op_dst & 15u;
+    switch (op) {
+        case P3GPU_AIR_CONST: v = in.arg; break;
+        case P3GPU_AIR_MAIN_LOCAL: v = env.local(in.arg); break;
+        case P3GPU_AIR_MAIN_NEXT: v = env.next(in.arg); break;
+        case P3GPU_AIR_PUBLIC: v = env.pub(in.arg); break;
+        case P3GPU_AIR_IS_FIRST_ROW: v = first; break;
+        case P3GPU_AIR_IS_LAST_ROW: v = last; break;
+        case P3GPU_AIR_IS_TRANSITION: v = trans; break;
+        case P3GPU_AIR_ADD: v = fp_add<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+        case P3GPU_AIR_SUB: v = fp_sub<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+        case P3GPU_AIR_NEG: v = fp_neg<F>(env.slot(in.arg)); break;
+        case P3GPU_AIR_MUL: v = mont_mul<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
+        default:                                                    // AIR_OP_FOLD (and, with EXT, opcodes 12-14)
+            if constexpr (EXT) {
+                if (op != AIR_OP_FOLD) {
+                    v = op == AIR_OP_PRE_LOCAL ? env.pre_local(in.arg) : op == AIR_OP_PRE_NEXT ? env.pre_next(in.arg) : env.periodic(in.arg);
+                    break;
+                }
+            }
+            return true;
+    }
+    return false;
+}
+
 // Evaluates the program at natural index i.  Env supplies insn(pc), slot(s), local(c), next(c), pub(k), apow(k) (alpha^(K-1-k)),
 // the row loads for memory rows bitrev(i) / bitrev(i + 2^q), zh(i) = Z_H(x_i) and inv_zh(i).  EXT (a program that reads
 // preprocessed or periodic columns) compiles in opcodes 12-14: Env then also supplies set_ext_rows(m, m_next, periodic_row),
@@ -319,35 +374,44 @@ __host__ __device__ __forceinline__ uint4 air_row_quotient(Env &env, const AirDo
     u64 acc[4] = {0, 0, 0, 0};
     for (u32 pc = 0; pc < n_insns; pc++) {
         const AirInsn in = env.insn(pc);
-        const u32 op = in.op_dst & 15u, dst = in.op_dst >> 4;
+        const u32 dst = in.op_dst >> 4;
         u32 v;
-        switch (op) {
-            case P3GPU_AIR_CONST: v = in.arg; break;
-            case P3GPU_AIR_MAIN_LOCAL: v = env.local(in.arg); break;
-            case P3GPU_AIR_MAIN_NEXT: v = env.next(in.arg); break;
-            case P3GPU_AIR_PUBLIC: v = env.pub(in.arg); break;
-            case P3GPU_AIR_IS_FIRST_ROW: v = first; break;
-            case P3GPU_AIR_IS_LAST_ROW: v = last; break;
-            case P3GPU_AIR_IS_TRANSITION: v = trans; break;
-            case P3GPU_AIR_ADD: v = fp_add<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
-            case P3GPU_AIR_SUB: v = fp_sub<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
-            case P3GPU_AIR_NEG: v = fp_neg<F>(env.slot(in.arg)); break;
-            case P3GPU_AIR_MUL: v = mont_mul<F>(env.slot(in.arg & 0xffffu), env.slot(in.arg >> 16)); break;
-            default:                                                    // AIR_OP_FOLD (and, with EXT, opcodes 12-14)
-                if constexpr (EXT) {
-                    if (op != AIR_OP_FOLD) {
-                        v = op == AIR_OP_PRE_LOCAL ? env.pre_local(in.arg) : op == AIR_OP_PRE_NEXT ? env.pre_next(in.arg) : env.periodic(in.arg);
-                        break;
-                    }
-                }
-                air_qmac<F>(acc, env.slot(in.arg), env.apow(dst));
-                continue;
+        if (air_decode<F, EXT>(env, in, first, last, trans, v)) {
+            air_qmac<F>(acc, env.slot(in.arg), env.apow(dst));
+            continue;
         }
         env.slot(dst) = v;
     }
     const u32 z = env.inv_zh(i);
     return make_uint4(mont_mul<F>(mont_redc<F>(acc[0]), z), mont_mul<F>(mont_redc<F>(acc[1]), z), mont_mul<F>(mont_redc<F>(acc[2]), z),
                       mont_mul<F>(mont_redc<F>(acc[3]), z));
+}
+
+// Checks row i of a trace of `height` rows (any height >= 1) with the reference's debug semantics (air/src/check_constraints.rs):
+// the trace in natural row order, next row (i + 1) mod height for the main and the preprocessed trace, selectors [i = 0],
+// [i = height - 1] and [i != height - 1] as Montgomery 0 / 1, periodic row i mod periodic_rows.  Calls on_fail(k) for every
+// constraint k whose value is non-zero, in ascending k (the compiler emits the folds in assertion order).  Env supplies what
+// air_decode reads for the EXT instance, insn(pc), set_rows(i, i_next) and set_ext_rows(i, i_next, periodic_row).
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable
+#endif
+template <int F, class Env, class OnFail>
+__host__ __device__ __forceinline__ void air_row_check(Env &env, u32 n_insns, u32 i, u32 height, u32 periodic_rows, OnFail &on_fail) {
+    const bool is_last = i + 1 == height;
+    const u32 nxt = is_last ? 0u : i + 1;
+    env.set_rows(i, nxt);
+    env.set_ext_rows(i, nxt, periodic_rows > 1 ? i % periodic_rows : 0u);
+    const u32 first = i == 0 ? Fp<F>::ONE : 0u, last = is_last ? Fp<F>::ONE : 0u, trans = is_last ? 0u : Fp<F>::ONE;
+    for (u32 pc = 0; pc < n_insns; pc++) {
+        const AirInsn in = env.insn(pc);
+        const u32 dst = in.op_dst >> 4;
+        u32 v;
+        if (air_decode<F, true>(env, in, first, last, trans, v)) {
+            if (env.slot(in.arg) != 0u) on_fail(dst);
+            continue;
+        }
+        env.slot(dst) = v;
+    }
 }
 
 // Host-side launch constants + tables: Z_H(x_i) and 1/Z_H(x_i) depend on i mod 2^q only (x^N = g^N w_q^(iN), w_q^N of order 2^q).

@@ -628,6 +628,28 @@ int32_t p3gpu_air_quotient_layout_dev(p3gpu_ctx *ctx, const p3gpu_air_program *p
                                 log_quotient_size, log_trace_height, public_values, alpha, d_quotient, true);
 }
 
+int32_t p3gpu_air_check_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const uint32_t *constraints,
+                                       size_t n_constraints, const p3gpu_air_layout *layout, p3gpu_air_program **out) {
+    P3_ENTER(ctx);
+    P3_CHECK(out && layout, P3GPU_EINVAL, "null argument");
+    *out = nullptr;
+    return air_program_create(ctx, field, nodes, n_nodes, constraints, n_constraints, *layout, out, true);
+}
+int32_t p3gpu_air_check_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_trace, size_t height, const uint32_t *d_preprocessed,
+                            const uint32_t *d_periodic, size_t periodic_rows, const uint32_t *public_values, uint32_t *d_counts) {
+    P3_ENTER(ctx);
+    P3_CHECK(prog && d_trace && d_counts, P3GPU_EINVAL, "null argument");
+    return air_check(ctx, prog, d_trace, height, d_preprocessed, d_periodic, periodic_rows, public_values, d_counts, nullptr, 0, nullptr, nullptr);
+}
+int32_t p3gpu_air_check_rows_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const uint32_t *d_trace, size_t height,
+                                 const uint32_t *d_preprocessed, const uint32_t *d_periodic, size_t periodic_rows, const uint32_t *public_values,
+                                 const uint32_t *d_rows, size_t n_rows, const uint64_t *d_offsets, uint32_t *d_failed) {
+    P3_ENTER(ctx);
+    P3_CHECK(prog && d_trace && (n_rows == 0 || (d_rows && d_offsets && d_failed)), P3GPU_EINVAL, "null argument");
+    return air_check(ctx, prog, d_trace, height, d_preprocessed, d_periodic, periodic_rows, public_values, nullptr, d_rows, n_rows, d_offsets,
+                     d_failed);
+}
+
 // ---- transcript + query phase (prove driver) ---------------------------------------------------------
 int32_t p3gpu_challenger_new(p3gpu_ctx *ctx, int field, int width, int rate, p3gpu_challenger **out) {
     P3_ENTER(ctx);

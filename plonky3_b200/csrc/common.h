@@ -160,8 +160,9 @@ int32_t air_quotient_sharded(p3gpu_ctx *ctx, int field, int vec_len, unsigned wo
                              unsigned log_h, unsigned log_n, const u32 *alpha, u32 *d_q);
 
 // air_program.cu: any AIR as a constraint program (air_program.cuh)
+// check: a check program (air_check.cu), compiled under the check limits (air_program.cuh AIR_CHECK_LIMITS)
 int32_t air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const u32 *constraints, size_t n_constraints,
-                           const p3gpu_air_layout &layout, p3gpu_air_program **out);
+                           const p3gpu_air_layout &layout, p3gpu_air_program **out, bool check = false);
 void air_program_destroy(p3gpu_air_program *prog);
 int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t *n_slots, size_t *n_cons);
 // layout_entry: called through p3gpu_air_quotient_layout_dev (d_pre / d_periodic as the program's layout declares them); otherwise
@@ -169,6 +170,10 @@ int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t 
 int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const u32 *d_lde, unsigned log_lde, const u32 *d_pre,
                              unsigned log_pre, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n,
                              const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
+// air_check.cu: the debug constraint check of a check program over the trace domain; pass 1 writes d_counts (height words), pass 2
+// (d_counts null) the failing constraints of the n_rows listed rows at their offsets
+int32_t air_check(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_trace, size_t height, const u32 *d_pre, const u32 *d_periodic,
+                  size_t periodic_rows, const u32 *pubs, u32 *d_counts, const u32 *d_rows, size_t n_rows, const u64 *d_offsets, u32 *d_failed);
 // A hand-written AIR quotient kernel (AirHandQArgs, air_program.cuh) over the 2N points of GENERATOR * K from the first 2N rows of
 // the committed bit-reversed LDE: checks the field, the domain, the alignment and alpha (messages name the AIR), builds the domain
 // and the alpha^(K - 1 - k) table (scratch2), then launches `kern_<field>` on min(SMs, 2N lanes / (32 warps)) blocks of `warps`

@@ -507,6 +507,48 @@ class Gpu:
                                                    self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    # ------------------------------------------------------------------ the debug constraint check (air.check_constraints)
+    def air_check_program_create(self, field, nodes, constraints, layout):
+        """A check program (p3gpu_air_check_program_create) of the DAG: layout = (width, n_public, preprocessed_width, n_periodic)."""
+        nd = np.ascontiguousarray(nodes, dtype=np.uint32).reshape(-1, 4)
+        cs = np.ascontiguousarray(constraints, dtype=np.uint32).ravel()
+        lay = np.ascontiguousarray(layout, dtype=np.uint32)
+        assert lay.size == 4
+        h = C.c_void_p()
+        check(self.L.p3gpu_air_check_program_create(self.h, field, nd.ctypes.data, nd.shape[0], cs.ctypes.data, cs.size, lay.ctypes.data,
+                                                    C.byref(h)))
+        return AirProgramHandle(self.L, h)
+
+    def _check_args(self, trace_dev, pre_dev, periodic_dev, public_values):
+        m = self._dev(trace_dev); self._use_torch_stream()
+        pre = self._dev(pre_dev) if pre_dev is not None else None
+        per = self._dev(periodic_dev) if periodic_dev is not None else None
+        pv = np.ascontiguousarray(public_values, dtype=np.uint32).ravel()
+        return (m.data_ptr(), int(m.shape[0]), pre.data_ptr() if pre is not None else None, per.data_ptr() if per is not None else None,
+                int(per.shape[0]) if per is not None else 0), pv
+
+    def air_check_counts(self, prog, trace_dev, pre_dev, periodic_dev, public_values):
+        """Pass 1 of the check: (height,) int32, the number of constraints failing on each row of the (height, width) trace.
+        pre_dev: the preprocessed trace (height rows); periodic_dev: the periodic columns repeated to the largest period; None when
+        the AIR has none.  public_values: Montgomery words."""
+        args, pv = self._check_args(trace_dev, pre_dev, periodic_dev, public_values)
+        counts = self._empty((args[1],))
+        check(self.L.p3gpu_air_check_dev(self.h, prog.h, *args, pv.ctypes.data if pv.size else None, counts.data_ptr()))
+        return counts
+
+    def air_check_rows(self, prog, trace_dev, pre_dev, periodic_dev, public_values, rows_dev, offsets_dev, n_failed):
+        """Pass 2 of the check: (n_failed,) int32, the failing constraints of row rows_dev[j] (int32 CUDA) in ascending order from
+        offsets_dev[j] (int64 CUDA) on."""
+        import torch
+        assert rows_dev.is_cuda and rows_dev.dtype == torch.int32 and rows_dev.is_contiguous()
+        assert offsets_dev.is_cuda and offsets_dev.dtype == torch.int64 and offsets_dev.is_contiguous()
+        assert int(offsets_dev.numel()) == int(rows_dev.numel())
+        args, pv = self._check_args(trace_dev, pre_dev, periodic_dev, public_values)
+        failed = self._empty((int(n_failed),))
+        check(self.L.p3gpu_air_check_rows_dev(self.h, prog.h, *args, pv.ctypes.data if pv.size else None, rows_dev.data_ptr(),
+                                              int(rows_dev.numel()), offsets_dev.data_ptr(), failed.data_ptr()))
+        return failed
+
     def pcs_commit_host(self, field, hash_kind, evals_host, log_blowup, cap_height):
         """p3gpu_pcs_commit: TwoAdicFriPcs::commit with the trace in HOST memory (numpy uint32 array or pinned CPU int32 tensor);
         the LDE and the digest layers stay on the device, only the cap returns.  Returns (cap (n, 8) array, lde, layers)."""

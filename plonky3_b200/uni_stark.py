@@ -156,7 +156,8 @@ def verify(config, air, proof, public_values=(), *, preprocessed_vk: Optional[Pr
     return _verify(config, air, proof, public_values, preprocessed_vk=preprocessed_vk)
 
 
-def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None) -> Proof:
+def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Optional[PreprocessedProverData] = None,
+          check_constraints: bool = False) -> Proof:
     """uni-stark/src/prover.rs:87-442 (prove_with_preprocessed).  `config`: StarkConfig, KeccakStarkConfig or Sha256StarkConfig — every transcript
     call goes through the challenger it initialises.  `air`: an air.SymbolicAir, such as poseidon2_air.VectorizedPoseidon2Air,
     keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air or poseidon1_air.VectorizedPoseidon1Air.  `trace`: device
@@ -167,7 +168,13 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
     empty).  Periodic columns need nothing here: the AIR evaluates them on the quotient domain.
 
     `shard`: a distributed.ShardedTrace when the trace's columns are split over ranks; `trace` is then this rank's column block,
-    and every rank returns the proof of the whole trace."""
+    and every rank returns the proof of the whole trace.
+
+    `check_constraints`: run air.check_constraints on the trace before committing it, as the reference's debug builds do
+    (uni-stark/src/prover.rs:102-103), and raise air.ConstraintViolation naming the first failing row and its constraints.  Not
+    with `shard` (the check reads whole rows)."""
+    if check_constraints and shard is not None:
+        raise ValueError("check_constraints needs whole trace rows: it does not take a column-sharded trace")
     import torch
     from . import extension as X
     pcs, f, gpu = config.pcs, config.pcs.dft.field, config.pcs.dft.gpu
@@ -209,6 +216,9 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
                          f"{pcs.fri.log_blowup} < {log_num_quotient_chunks}")
     opens_next = len(air.main_next_row_columns()) > 0
     pre_next = pre_width > 0 and len(air.preprocessed_next_row_columns()) > 0
+    if check_constraints:
+        from .air import check_constraints as _check
+        _check(air, trace, public_values)
     challenger = config.initialise_challenger()
     trace_domain = pcs.natural_domain_for_degree(degree)
 

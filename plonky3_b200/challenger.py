@@ -14,16 +14,16 @@ from .gpu import _is_torch
 from .poseidon2 import Poseidon2
 
 
-class DuplexChallenger:
-    """DuplexChallenger<F, Poseidon2<width>, width, rate>: examples use (Perm24, 24, 16) (examples/src/types.rs:56-60)."""
+class _DeviceChallenger:
+    """The method surface both device transcripts share, behind one C handle; a subclass only creates the handle.  Values in and
+    out are Montgomery words, as everywhere else in the prover."""
 
-    def __init__(self, field: Field, perm: Poseidon2, rate: int, gpu):
-        assert perm.field is field or perm.field == field
-        self.field, self.perm, self.rate, self.gpu = field, perm, rate, gpu
-        perm.upload(gpu)
+    def _create(self, new):
+        """`new(out)`: a C call writing the new handle to `out`."""
+        self.h = None
         h = C.c_void_p()
-        gpu._use_torch_stream()
-        check(gpu.L.p3gpu_challenger_new(gpu.h, field.id, perm.width, rate, C.byref(h)))
+        self.gpu._use_torch_stream()
+        check(new(C.byref(h)))
         self.h = h
 
     def __del__(self):
@@ -35,102 +35,9 @@ class DuplexChallenger:
             pass
 
     def clone(self):
-        c = object.__new__(DuplexChallenger)
-        c.field, c.perm, c.rate, c.gpu = self.field, self.perm, self.rate, self.gpu
-        h = C.c_void_p()
-        self.gpu._use_torch_stream()
-        check(self.gpu.L.p3gpu_challenger_clone(self.gpu.h, self.h, C.byref(h)))
-        c.h = h
-        return c
-
-    # ---- CanObserve
-    def observe_slice(self, values):
-        """Montgomery words; a CUDA int32 tensor is absorbed on the device without a copy."""
-        self.gpu._use_torch_stream()
-        if _is_torch(values) and values.is_cuda:
-            v = values.contiguous()
-            check(self.gpu.L.p3gpu_challenger_observe_dev(self.gpu.h, self.h, v.data_ptr(), v.numel()))
-            self._keep = v
-            return
-        v = np.ascontiguousarray(values.cpu().numpy().view(np.uint32) if _is_torch(values) else values, dtype=np.uint32).ravel()
-        check(self.gpu.L.p3gpu_challenger_observe(self.gpu.h, self.h, v.ctypes.data, v.size))
-
-    def observe(self, value: int): self.observe_slice(np.array([value], dtype=np.uint32))
-    def observe_canonical(self, x: int): self.observe(self.field.to_monty(x))           # Val::from_u8 / from_usize
-    def observe_cap(self, cap): self.observe_slice(cap)                                # every digest, element by element
-    def observe_algebra_slice(self, ys): self.observe_slice(ys)                        # EF4 = 4 base coefficients in order
-
-    # ---- CanSample
-    def sample_many(self, n: int) -> np.ndarray:
-        out = np.empty(n, dtype=np.uint32)
-        self.gpu._use_torch_stream()
-        check(self.gpu.L.p3gpu_challenger_sample(self.gpu.h, self.h, out.ctypes.data, n))
-        return out
-
-    def sample(self) -> int: return int(self.sample_many(1)[0])
-    def sample_algebra_element(self) -> np.ndarray: return self.sample_many(4)
-
-    def sample_bits(self, bits: int) -> int:
-        """CanSampleBits (duplex_challenger.rs:270-283): canonical value of one sample, masked."""
-        assert (1 << bits) < self.field.P
-        return self.field.from_monty(self.sample()) & ((1 << bits) - 1)
-
-    # ---- GrindingChallenger
-    def grind(self, bits: int) -> int:
-        w = C.c_uint32()
-        self.gpu._use_torch_stream()
-        check(self.gpu.L.p3gpu_challenger_grind(self.gpu.h, self.h, bits, C.byref(w)))
-        return int(w.value)
-
-
-class SerializingChallenger32:
-    """SerializingChallenger32<F, HashChallenger<u8, H, 32>> (challenger/src/serializing_challenger.rs, hash_challenger.rs) with
-    H = Keccak256Hash, the transcript of the Keccak configuration (examples/src/types.rs:19-35), or H = Sha256, the transcript of
-    the SHA-256 configurations (keccak-air/examples/prove_baby_bear_sha256*.rs); `hasher` is "keccak256" (the default) or
-    "sha256".  Resident on the GPU like DuplexChallenger and with the same method surface.  Field elements are observed as the 4
-    little-endian bytes of their canonical values; a digest (8 words: [u64; 4] or [u8; 32]) as its 32 bytes; samples are
-    rejection-sampled from 4 bytes popped off the end of the hash's digest; `sample_bits` masks the raw u32; `grind` returns the
-    smallest witness.  Values in and out are Montgomery words, as everywhere else in the prover."""
-
-    HASHERS = ("keccak256", "sha256")
-
-    def __init__(self, field: Field, gpu, hasher: str = "keccak256"):
-        if hasher not in self.HASHERS:
-            raise ValueError(f"unknown transcript hash {hasher!r} (one of {', '.join(self.HASHERS)})")
-        self.field, self.gpu, self.hasher = field, gpu, hasher
-        h = C.c_void_p()
-        gpu._use_torch_stream()
-        new = gpu.L.p3gpu_challenger_new_sha256 if hasher == "sha256" else gpu.L.p3gpu_challenger_new_keccak256
-        check(new(gpu.h, field.id, C.byref(h)))
-        self.h = h
-
-    @classmethod
-    def from_hasher(cls, initial_state, field: Field, gpu, hasher: str = "keccak256"):
-        """from_hasher(initial_state, H): `initial_state` bytes become the start of the input buffer.  The transcript takes whole
-        32-bit words, so their number must be a multiple of 4."""
-        init = bytes(initial_state)
-        if len(init) % 4:
-            raise ValueError("the initial state must be a whole number of 32-bit words")
-        c = cls(field, gpu, hasher)
-        if init:
-            c._observe_digest(np.frombuffer(init, dtype="<u4").astype(np.uint32))
-        return c
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None) and self.gpu.h:
-                self.gpu.L.p3gpu_challenger_free(self.gpu.h, self.h)
-                self.h = None
-        except Exception:
-            pass
-
-    def clone(self):
-        c = object.__new__(SerializingChallenger32)
-        c.field, c.gpu, c.hasher = self.field, self.gpu, self.hasher
-        h = C.c_void_p()
-        self.gpu._use_torch_stream()
-        check(self.gpu.L.p3gpu_challenger_clone(self.gpu.h, self.h, C.byref(h)))
-        c.h = h
+        c = object.__new__(type(self))
+        c.__dict__.update(self.__dict__)
+        c._create(lambda out: self.gpu.L.p3gpu_challenger_clone(self.gpu.h, self.h, out))
         return c
 
     # ---- CanObserve
@@ -142,18 +49,19 @@ class SerializingChallenger32:
             check(self.gpu.L.p3gpu_challenger_observe_dev(self.gpu.h, self.h, v.data_ptr(), v.numel()))
             self._keep = v
             return
-        v = np.ascontiguousarray(values.cpu().numpy().view(np.uint32) if _is_torch(values) else values, dtype=np.uint32).ravel()
+        v = _host_words(values)
         check(self.gpu.L.p3gpu_challenger_observe(self.gpu.h, self.h, v.ctypes.data, v.size))
 
-    def _observe_digest(self, words):
-        v = np.ascontiguousarray(words.cpu().numpy().view(np.uint32) if _is_torch(words) else words, dtype=np.uint32).ravel()
+    def observe(self, value: int): self.observe_slice(np.array([value], dtype=np.uint32))
+    def observe_canonical(self, x: int): self.observe(self.field.to_monty(x))           # Val::from_u8 / from_usize
+    def observe_algebra_slice(self, ys): self.observe_slice(ys)                        # EF4 = 4 base coefficients in order
+
+    def observe_cap(self, cap):
+        """A Merkle cap's digests as the MMCS commits them: [F; 8] digests element by element (the duplex transcript); [u64; 4] or
+        [u8; 32] digests, held as 8 words, as their 32 bytes (the byte transcripts)."""
+        v = _host_words(cap)
         self.gpu._use_torch_stream()
         check(self.gpu.L.p3gpu_challenger_observe_digest(self.gpu.h, self.h, v.ctypes.data, v.size))
-
-    def observe(self, value: int): self.observe_slice(np.array([value], dtype=np.uint32))
-    def observe_canonical(self, x: int): self.observe(self.field.to_monty(x))
-    def observe_cap(self, cap): self._observe_digest(cap)                             # CanObserve<MerkleCap<F, [u64; 4] | [u8; 32]>>: the bytes
-    def observe_algebra_slice(self, ys): self.observe_slice(ys)
 
     # ---- CanSample
     def sample_many(self, n: int) -> np.ndarray:
@@ -166,7 +74,8 @@ class SerializingChallenger32:
     def sample_algebra_element(self) -> np.ndarray: return self.sample_many(4)
 
     def sample_bits(self, bits: int) -> int:
-        """CanSampleBits: the raw u32 of 4 popped bytes, masked (not a reduced field element)."""
+        """CanSampleBits: the duplex transcript masks the canonical value of one sample (duplex_challenger.rs:270-283), a byte
+        transcript the raw u32 of 4 popped bytes.  2^bits must be below the field order (P3GpuError EINVAL otherwise)."""
         out = np.empty(1, dtype=np.uint32)
         self.gpu._use_torch_stream()
         check(self.gpu.L.p3gpu_challenger_sample_bits(self.gpu.h, self.h, bits, 1, out.ctypes.data))
@@ -178,3 +87,47 @@ class SerializingChallenger32:
         self.gpu._use_torch_stream()
         check(self.gpu.L.p3gpu_challenger_grind(self.gpu.h, self.h, bits, C.byref(w)))
         return int(w.value)
+
+
+def _host_words(values) -> np.ndarray:
+    return np.ascontiguousarray(values.cpu().numpy().view(np.uint32) if _is_torch(values) else values, dtype=np.uint32).ravel()
+
+
+class DuplexChallenger(_DeviceChallenger):
+    """DuplexChallenger<F, Poseidon2<width>, width, rate>: examples use (Perm24, 24, 16) (examples/src/types.rs:56-60)."""
+
+    def __init__(self, field: Field, perm: Poseidon2, rate: int, gpu):
+        assert perm.field is field or perm.field == field
+        self.field, self.perm, self.rate, self.gpu = field, perm, rate, gpu
+        perm.upload(gpu)
+        self._create(lambda out: gpu.L.p3gpu_challenger_new(gpu.h, field.id, perm.width, rate, out))
+
+
+class SerializingChallenger32(_DeviceChallenger):
+    """SerializingChallenger32<F, HashChallenger<u8, H, 32>> (challenger/src/serializing_challenger.rs, hash_challenger.rs) with
+    H = Keccak256Hash, the transcript of the Keccak configuration (examples/src/types.rs:19-35), or H = Sha256, the transcript of
+    the SHA-256 configurations (keccak-air/examples/prove_baby_bear_sha256*.rs); `hasher` is "keccak256" (the default) or
+    "sha256".  Field elements are observed as the 4 little-endian bytes of their canonical values; a digest (8 words: [u64; 4] or
+    [u8; 32]) as its 32 bytes; samples are rejection-sampled from 4 bytes popped off the end of the hash's digest; `sample_bits`
+    masks the raw u32; `grind` returns the smallest witness."""
+
+    HASHERS = ("keccak256", "sha256")
+
+    def __init__(self, field: Field, gpu, hasher: str = "keccak256"):
+        if hasher not in self.HASHERS:
+            raise ValueError(f"unknown transcript hash {hasher!r} (one of {', '.join(self.HASHERS)})")
+        self.field, self.gpu, self.hasher = field, gpu, hasher
+        new = gpu.L.p3gpu_challenger_new_sha256 if hasher == "sha256" else gpu.L.p3gpu_challenger_new_keccak256
+        self._create(lambda out: new(gpu.h, field.id, out))
+
+    @classmethod
+    def from_hasher(cls, initial_state, field: Field, gpu, hasher: str = "keccak256"):
+        """from_hasher(initial_state, H): `initial_state` bytes become the start of the input buffer.  The transcript takes whole
+        32-bit words, so their number must be a multiple of 4."""
+        init = bytes(initial_state)
+        if len(init) % 4:
+            raise ValueError("the initial state must be a whole number of 32-bit words")
+        c = cls(field, gpu, hasher)
+        if init:
+            c.observe_cap(np.frombuffer(init, dtype="<u4").astype(np.uint32))
+        return c

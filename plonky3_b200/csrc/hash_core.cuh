@@ -1,7 +1,8 @@
 // The hash primitives of the hot path as device functions: Poseidon2 over the 31-bit Montgomery fields (width 16 / 24),
-// Keccak-f[1600] and the SHA-256 compression.  Kept apart from the kernels (hash.cu) so that the same source can also be compiled
-// as plain C++ and executed on the host against the CPU oracle (tests/cpp/hash_core_host.cpp, keccak256_host.cpp,
-// sha256_host.cpp): g++ ignores the CUDA attributes, and the intrinsics used here get host bodies there.
+// Keccak-f[1600] and the SHA-256 compression, and the byte transcript over Keccak-256 or SHA-256.  Kept apart from the kernels
+// (hash.cu, challenger.cu) so that the same source can also be compiled as plain C++ and executed on the host against the CPU
+// oracle (tests/cpp/hash_core_host.cpp, keccak256_host.cpp, sha256_host.cpp, transcript_host.cpp): g++ ignores the CUDA
+// attributes, and the intrinsics used here get host bodies there.
 #pragma once
 #include "field.cuh"
 #include "poseidon2_consts.h"
@@ -260,7 +261,14 @@ static __constant__ u32 SHA256_K[64] = {
     0xa2bfe8a1u, 0xa81a664bu, 0xc24b8b70u, 0xc76c51a3u, 0xd192e819u, 0xd6990624u, 0xf40e3585u, 0x106aa070u, 0x19a4c116u, 0x1e376c08u,
     0x2748774cu, 0x34b0bcb5u, 0x391c0cb3u, 0x4ed8aa4au, 0x5b9cca4fu, 0x682e6ff3u, 0x748f82eeu, 0x78a5636fu, 0x84c87814u, 0x8cc70208u,
     0x90befffau, 0xa4506cebu, 0xbef9a3f7u, 0xc67178f2u};
-static __constant__ u32 SHA256_IV[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+// The initial hash value; a function so that host code (the transcript's initial state) reads the same constants
+__host__ __device__ constexpr u32 sha256_iv_word(int i) {
+    constexpr u32 iv[8] = {0x6a09e667u, 0xbb67ae85u, 0x3c6ef372u, 0xa54ff53au, 0x510e527fu, 0x9b05688cu, 0x1f83d9abu, 0x5be0cd19u};
+    return iv[i];
+}
+// the copy the hash kernels read, as constant-bank operands
+static __constant__ u32 SHA256_IV[8] = {sha256_iv_word(0), sha256_iv_word(1), sha256_iv_word(2), sha256_iv_word(3),
+                                        sha256_iv_word(4), sha256_iv_word(5), sha256_iv_word(6), sha256_iv_word(7)};
 
 __device__ __forceinline__ u32 rotr32(u32 x, int r) { return __funnelshift_l(x, x, 32 - r); }
 __device__ __forceinline__ u32 bswap32(u32 x) {
@@ -331,6 +339,168 @@ __device__ inline void sha256(const unsigned char *msg, size_t len, unsigned cha
     }
     for (int k = 0; k < 8; k++)
         for (int j = 0; j < 4; j++) out[4 * k + j] = (unsigned char)(st[k] >> (24 - 8 * j));
+}
+
+// =================================================================================================
+// SerializingChallenger32<F, HashChallenger<u8, H, 32>> (challenger/src/serializing_challenger.rs, hash_challenger.rs)
+// =================================================================================================
+// The transcript of the Keccak and SHA-256 configurations.  The reference keeps every observed byte in an input buffer and hashes
+// all of it when a sample finds the output buffer empty; the digest then becomes both the new input buffer and the output buffer,
+// whose bytes are popped from the end.  Absorbing the input block by block as it fills gives the same digest, so the state is the
+// hash's running state over the full blocks plus the pending words of the partial block; every input is a whole number of 32-bit
+// words (4-byte field elements, 32-byte digests).  The state is an array of TR_WORDS words (device memory in challenger.cu, a host
+// array in tests/cpp/transcript_host.cpp):
+//     [0, 64)              the hash's running state, laid out by the policy
+//     [TR_PEND, +BLOCK)    the pending words, in the hash's block representation; [TR_NPEND] their number
+//     [TR_OUT, +8)         the output buffer: the digest as 8 big-endian words, so that the u32 of the 4 bytes popped off its end
+//                          (u32::from_le_bytes of bytes 4m+3, 4m+2, 4m+1, 4m) is word m itself; [TR_NOUT] how many words are left
+// A policy gives the block size in words, the running State (held in registers) with init / load / store over the state words,
+// absorb (one full block), finish (the pending words, an optional extra word and the padding: the digest as big-endian words) and
+// block_word (a word of 4 stream bytes in little-endian order, as it enters a block).  absorb and finish also see the state words,
+// for what a policy keeps there rather than in registers.
+constexpr int TR_PEND = 64, TR_NPEND = 98, TR_OUT = 100, TR_NOUT = 108, TR_WORDS = 128;
+
+// Keccak256Hash: the Keccak state as (lo[25], hi[25]) at [0, 50), zero initially; 34-word blocks of little-endian words
+struct Keccak256Policy {
+    static constexpr int BLOCK = KECCAK256_RATE_WORDS;
+    typedef KState State;
+    static __host__ __device__ void init(u32 *st) {
+        for (int i = 0; i < 50; i++) st[i] = 0;
+    }
+    static __device__ __forceinline__ void load(const u32 *st, State &s) {
+#pragma unroll
+        for (int i = 0; i < 25; i++) { s.lo[i] = st[i]; s.hi[i] = st[25 + i]; }
+    }
+    static __device__ __forceinline__ void store(u32 *st, const State &s) {
+#pragma unroll
+        for (int i = 0; i < 25; i++) { st[i] = s.lo[i]; st[25 + i] = s.hi[i]; }
+    }
+    static __device__ __forceinline__ u32 block_word(u32 x) { return x; }
+    static __device__ __forceinline__ void absorb(u32 *, State &s, const u32 (&w)[BLOCK]) { keccak256_absorb_block(s, w); }
+    // the n < BLOCK pending words, then `extra` if has_extra: one Keccak-f, or two when the extra word completes the block
+    static __device__ __forceinline__ void finish(State &s, const u32 *st, bool has_extra, u32 extra, u32 (&d)[8]) {
+        const u32 n = st[TR_NPEND], *pend = st + TR_PEND;
+        u32 w[BLOCK];
+#pragma unroll
+        for (int i = 0; i < BLOCK; i++) w[i] = (u32)i < n ? pend[i] : (has_extra && (u32)i == n ? extra : 0u);
+        u32 tail = n + (has_extra ? 1u : 0u);
+        if (tail == (u32)BLOCK) { keccak256_absorb_block(s, w); tail = 0; }
+        keccak256_final_block(s, w, tail);
+#pragma unroll
+        for (int k = 0; k < 8; k++) d[k] = bswap32(keccak256_digest_word(s, k));
+    }
+};
+
+// Sha256: the midstate at [0, 8) (the IV initially) and the number of full blocks at [8] (for the length in the padding);
+// 16-word blocks of big-endian words.  The block count stays in the state words, not in State: held in a register it made ptxas
+// schedule the single-thread observe kernel's compression 7 % slower (H100 80GB HBM3, 700 W); in memory the kernel is unchanged.
+struct Sha256Policy {
+    static constexpr int BLOCK = 16;
+    struct State { u32 h[8]; };
+    static __host__ __device__ void init(u32 *st) {
+        for (int i = 0; i < 8; i++) st[i] = sha256_iv_word(i);
+        st[8] = 0;
+    }
+    static __device__ __forceinline__ void load(const u32 *st, State &s) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) s.h[i] = st[i];
+    }
+    static __device__ __forceinline__ void store(u32 *st, const State &s) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) st[i] = s.h[i];
+    }
+    static __device__ __forceinline__ u32 block_word(u32 x) { return bswap32(x); }
+    static __device__ __forceinline__ void absorb(u32 *st, State &s, const u32 (&w)[BLOCK]) { sha256_compress(s.h, w); st[8]++; }
+    // the n < BLOCK pending words, then `extra` if has_extra, then the padding: one or two compressions through one inlined copy of
+    // the compression
+    static __device__ __forceinline__ void finish(State &s, const u32 *st, bool has_extra, u32 extra, u32 (&d)[8]) {
+        const u32 n = st[TR_NPEND], *pend = st + TR_PEND;
+        const u32 tail = n + (has_extra ? 1u : 0u);
+        const u64 nb = sha256_blocks(tail), bits = ((u64)st[8] * 16 + tail) * 32;
+#pragma unroll 1
+        for (u64 b = 0; b < nb; b++) {
+            u32 w[16];
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                const u64 j = 16 * b + i;
+                w[i] = j < n ? pend[i] : (j < tail ? extra : sha256_pad_word(j, tail, nb, bits));
+            }
+            sha256_compress(s.h, w);
+        }
+#pragma unroll
+        for (int k = 0; k < 8; k++) d[k] = s.h[k];
+    }
+};
+
+// CanObserve.  MONTY: Montgomery words, observed as the 4 little-endian bytes of their canonical values (CanObserve<F>); otherwise
+// words observed as their own bytes (a digest held as 8 words).  Any buffered output is invalidated.
+template <class H, int F, bool MONTY>
+__device__ void transcript_observe(u32 *st, const u32 *vals, size_t n) {
+    if (n == 0) return;
+    typename H::State s;
+    H::load(st, s);
+    st[TR_NOUT] = 0;
+    u32 m = st[TR_NPEND];
+    for (size_t j = 0; j < n; j++) {
+        st[TR_PEND + m] = H::block_word(MONTY ? from_monty<F>(vals[j]) : vals[j]);
+        if (++m == (u32)H::BLOCK) {
+            u32 w[H::BLOCK];
+#pragma unroll
+            for (int i = 0; i < H::BLOCK; i++) w[i] = st[TR_PEND + i];
+            H::absorb(st, s, w);
+            m = 0;
+        }
+    }
+    st[TR_NPEND] = m;
+    H::store(st, s);
+}
+
+// HashChallenger::flush: the digest of everything observed is the new input buffer (the running state back at its start) and the
+// output buffer
+template <class H>
+__device__ void transcript_flush(u32 *st) {
+    typename H::State s;
+    H::load(st, s);
+    u32 d[8];
+    H::finish(s, st, false, 0u, d);
+    H::init(st);
+#pragma unroll
+    for (int k = 0; k < 8; k++) { st[TR_PEND + k] = H::block_word(bswap32(d[k])); st[TR_OUT + k] = d[k]; }
+    st[TR_NPEND] = 8;
+    st[TR_NOUT] = 8;
+}
+
+// Four bytes popped from the END of the output buffer, as u32::from_le_bytes of the popped order: the last big-endian word left
+template <class H>
+__device__ __forceinline__ u32 transcript_pop_u32(u32 *st) {
+    if (st[TR_NOUT] == 0) transcript_flush<H>(st);
+    const u32 m = st[TR_NOUT] - 1;
+    st[TR_NOUT] = m;
+    return st[TR_OUT + m];
+}
+
+// raw = false: n field elements by rejection sampling of 31-bit values (CanSample<F>), as Montgomery words; raw = true: n u32s of
+// 4 popped bytes AND `mask` (CanSampleBits)
+template <class H, int F>
+__device__ void transcript_sample(u32 *st, u32 *out, size_t n, bool raw, u32 mask) {
+    for (size_t j = 0; j < n; j++) {
+        if (raw) { out[j] = transcript_pop_u32<H>(st) & mask; continue; }
+        u32 v;
+        do { v = transcript_pop_u32<H>(st) & 0x7fffffffu; } while (v >= Fp<F>::P);
+        out[j] = to_monty<F>(v);
+    }
+}
+
+// Whether the canonical value c is a proof-of-work witness: observe(c); sample_bits(bits) == 0 (mask = 2^bits - 1), read off
+// without changing the state.  The hash is finished from the running state with the pending words and c; the first sampled u32
+// is the last big-endian digest word.
+template <class H>
+__device__ __forceinline__ bool transcript_is_witness(const u32 *st, u32 c, u32 mask) {
+    typename H::State s;
+    H::load(st, s);
+    u32 d[8];
+    H::finish(s, st, true, H::block_word(c), d);
+    return (d[7] & mask) == 0;
 }
 
 }  // namespace p3

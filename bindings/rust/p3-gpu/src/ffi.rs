@@ -156,6 +156,9 @@ unsafe extern "C" {
                                                  log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
     pub fn p3gpu_p1air_quotient_sharded_dev(ctx: *mut P3GpuCtx, field: c_int, vector_len: c_int, grp: *const P3GpuPeerGroup, col_starts: *const usize,
                                             log_lde_height: c_uint, log_trace_height: c_uint, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
+    pub fn p3gpu_air_quotient_sharded_dev(ctx: *mut P3GpuCtx, prog: *const P3GpuAirProgram, grp: *const P3GpuPeerGroup, col_starts: *const usize,
+                                          d_periodic: *const u32, log_periodic_rows: c_uint, log_lde_height: c_uint, log_trace_height: c_uint,
+                                          public_values: *const u32, alpha: *const u32, d_quotient_slice: *mut u32) -> i32;
 
     // streams, counters
     pub fn p3gpu_ctx_set_stream(ctx: *mut P3GpuCtx, cuda_stream: *mut c_void) -> i32;

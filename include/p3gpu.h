@@ -553,6 +553,23 @@ int32_t p3gpu_p1air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_l
                                          unsigned log_lde_height, unsigned log_trace_height, const uint32_t alpha[4],
                                          uint32_t *d_quotient_slice);
 
+/* The same for any AIR given as a constraint program (p3gpu_air_quotient_dev / _layout_dev over the LDE domain: log_quotient_size =
+ * log_lde_height): the quotient values of MY row block after p3gpu_commit_sharded_dev with the same col_starts (col_starts[world] is
+ * the program's width), written to d_quotient_slice (R = 2^log_lde_height / world EF4 values) in BIT-REVERSED order as
+ * p3gpu_blake3_air_quotient_sharded_dev does.  Local columns are read in place from grp->rows[rank]; next-row columns from the row
+ * block of the single rank that holds every next row of mine, bitrev((bitrev(rank) + 2^q) mod world) with q = log_lde_height -
+ * log_trace_height (my own block when world <= 2^q).  d_periodic / log_periodic_rows: the whole periodic table, as for
+ * p3gpu_air_quotient_layout_dev.  P3GPU_EINVAL before any launch: a NULL argument, a bad peer group, a program created for the check
+ * (p3gpu_air_check_program_create), a non-canonical alpha or public value, public values missing, a periodic table given / missing
+ * against the program, a misaligned buffer (slice 16 bytes, row blocks and table 4 bytes), column blocks that do not cover the
+ * program's width or leave a segment bound that is neither a multiple of 8 columns nor the width; P3GPU_EUNSUPPORTED: fewer than
+ * 1024 rows per rank, a quotient domain other than the LDE domain (more than 8 extra bits over the trace), a program with
+ * preprocessed columns, more shared memory than a block has (slots x 512 B + constraints x 16 B + one 8-byte unit-table entry per
+ * 8 columns; the message gives the three). */
+int32_t p3gpu_air_quotient_sharded_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                       const uint32_t *d_periodic, unsigned log_periodic_rows, unsigned log_lde_height, unsigned log_trace_height,
+                                       const uint32_t *public_values, const uint32_t alpha[4], uint32_t *d_quotient_slice);
+
 #ifdef __cplusplus
 }
 #endif

@@ -44,6 +44,7 @@ EXPORTS = [
     "p3gpu_p1air_set_constants", "p3gpu_p1air_columns", "p3gpu_p1air_generate_trace_dev", "p3gpu_p1air_quotient_dev",
     "p3gpu_blake3_air_generate_trace_cols_dev", "p3gpu_sha256_air_generate_trace_cols_dev", "p3gpu_p1air_generate_trace_cols_dev",
     "p3gpu_blake3_air_quotient_sharded_dev", "p3gpu_sha256_air_quotient_sharded_dev", "p3gpu_p1air_quotient_sharded_dev",
+    "p3gpu_air_quotient_sharded_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -166,6 +167,7 @@ def load():
         "p3gpu_blake3_air_quotient_sharded_dev": (i32, [vp, ci, vp, vp, cu, cu, vp, vp]),
         "p3gpu_sha256_air_quotient_sharded_dev": (i32, [vp, ci, vp, vp, cu, cu, vp, vp]),
         "p3gpu_p1air_quotient_sharded_dev": (i32, [vp, ci, ci, vp, vp, cu, cu, vp, vp]),
+        "p3gpu_air_quotient_sharded_dev": (i32, [vp, vp, vp, vp, vp, cu, cu, cu, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

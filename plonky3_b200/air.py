@@ -367,6 +367,21 @@ class SymbolicAir:
         prog = self.program()
         return self.gpu.air_quotient_layout(prog, trace_lde_dev, preprocessed_on_quotient_domain, table, log_q, log_degree, pv, alpha)
 
+    def sharded_quotient_values(self, grp, log_lde_height: int, log_degree: int, alpha, public_values=()):
+        """The quotient values of `grp`'s row block after its sharded commit (distributed.PeerGroup.commit), over the LDE domain
+        (log_num_quotient_chunks == log_blowup): (R, 4), R = 2^log_lde_height / world, in bit-reversed order: entry m is natural
+        index bitrev(rank R + m).  Next-row columns are read from the row block of the one rank that holds them
+        (distributed.next_row_rank).  `grp`: anything with the commit's `struct` (_lib.PeerGroupStruct) and `col_starts`.
+        `public_values`: canonical.  No preprocessed columns."""
+        if len(public_values) != self.num_public_values():
+            raise ValueError(f"{len(public_values)} public values given, the AIR has {self.num_public_values()}")
+        if self.preprocessed_width() > 0:
+            raise ValueError(f"the AIR has {self.preprocessed_width()} preprocessed columns: no sharded quotient")
+        log_lde_height, log_degree = int(log_lde_height), int(log_degree)
+        pv = [self.field.to_monty(int(v) % self.field.P) for v in public_values]
+        table = self.periodic_table(log_degree, log_lde_height)
+        return self.gpu.air_quotient_sharded(self.program(), grp.struct, grp.col_starts, table, log_lde_height, log_degree, pv, alpha)
+
     # ---- verifier: the constraint folder on the same DAG
     def eval_folded_constraints(self, e, local, nxt, public_values, is_first_row, is_last_row, is_transition, alpha, *,
                                 preprocessed_local=None, preprocessed_next=None, periodic_values=None):
@@ -538,9 +553,12 @@ class KernelAir(SymbolicAir):
         """Whether the AIR has a quotient kernel for one rank's row block of the row-sharded commit."""
         return cls._kernel_quotient_sharded is not KernelAir._kernel_quotient_sharded
 
-    def sharded_quotient_values(self, grp, log_lde_height: int, log_degree: int, alpha):
+    def sharded_quotient_values(self, grp, log_lde_height: int, log_degree: int, alpha, public_values=()):
         """The quotient values of `grp`'s row block after its sharded commit (distributed.PeerGroup.commit, log_blowup 1): (R, 4), R =
-        2^log_lde_height / world, in bit-reversed order: entry m is natural index bitrev(rank R + m) of the quotient domain."""
+        2^log_lde_height / world, in bit-reversed order: entry m is natural index bitrev(rank R + m) of the quotient domain.  The AIR's
+        own sharded kernel, never the constraint program; it takes no public values."""
+        if len(public_values) != 0:
+            raise ValueError(f"{len(public_values)} public values given, the {self.air_name} AIR has none")
         self._need_gpu("quotient evaluation")
         return self._kernel_quotient_sharded(grp, int(log_lde_height), int(log_degree), alpha)
 

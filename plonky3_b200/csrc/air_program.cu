@@ -68,6 +68,56 @@ template <int F, bool EXT> __global__ void __launch_bounds__(AIR_BLOCK) air_prog
     reinterpret_cast<uint4 *>(a.q)[i] = air_row_quotient<F, EXT>(env, a.d, a.n_insns, i);
 }
 
+// Row-sharded instance (p3gpu_air_quotient_sharded_dev): one rank's row block of the row-sharded commit, whose quotient domain is
+// the LDE domain.  One thread per block row m: natural index i = bitrev(row0 + m), the same air_row_quotient as the dense kernel,
+// its value stored at q[m] (the block's bit-reversed slice).  Local columns are read in place from the rank's chunk-major block,
+// next-row columns from the chunk-major block of the one rank holding every next row of this block (air_shard_next_rank), at
+// local row bitrev(i + 2^q) mod R; both through the unit table (AirShardRow), which sits in shared memory behind the slots.
+// Periodic values as in the dense kernel (every rank holds the whole small table).  A program without AIR_USES_NEXT never reads
+// the peer's block.  The peer's rows are final before this kernel runs, because the sharded commit ends in a barrier, and stay
+// unchanged until every rank is done with them, because a row block is written only by the commit and the exchange after the
+// quotient (ShardedTrace.quotient_values) starts with a barrier.
+struct AirShardQArgs {
+    AirQArgs q;                 // the dense arguments: program, tables, output; q.lde / q.width unused
+    const u32 *own, *peer;      // my row block; the row block holding my points' next rows (my own when the program reads none)
+    const u64 *units;           // n_units entries, one per 8 columns (air_shard_units)
+    u32 n_units, n_slots, row0, rows;
+    unsigned log_rows;
+};
+
+template <int F> struct AirShardDevEnv : AirDevEnv<F> {
+    const AirShardQArgs *s;
+    const u64 *tab;             // the unit table in shared memory
+    AirShardRow cur, nxt;
+    __device__ __forceinline__ void set_rows(u32 m, u32 mn) {
+        cur = AirShardRow{s->own, tab, air_shard_locate(m, s->log_rows).row};
+        nxt = AirShardRow{s->peer, tab, air_shard_locate(mn, s->log_rows).row};
+    }
+    __device__ __forceinline__ void set_ext_rows(u32, u32, u32 pr) { this->per = this->a->periodic + (size_t)pr * this->a->n_periodic; }
+    __device__ __forceinline__ u32 local(u32 c) const { return cur.ld(c); }
+    __device__ __forceinline__ u32 next(u32 c) const { return nxt.ld(c); }
+    // the sharded entry refuses a program with preprocessed columns
+    __device__ __forceinline__ u32 pre_local(u32) const { return 0u; }
+    __device__ __forceinline__ u32 pre_next(u32) const { return 0u; }
+};
+
+template <int F, bool EXT> __global__ void __launch_bounds__(AIR_BLOCK) air_program_quotient_sharded_kernel(const AirShardQArgs a) {
+    extern __shared__ uint4 air_sm[];
+    for (u32 t = threadIdx.x; t < a.q.n_cons; t += AIR_BLOCK) air_sm[t] = __ldg(a.q.apow + t);
+    u64 *tab = reinterpret_cast<u64 *>(reinterpret_cast<u32 *>(air_sm + a.q.n_cons) + (size_t)a.n_slots * AIR_BLOCK);
+    for (u32 t = threadIdx.x; t < a.n_units; t += AIR_BLOCK) tab[t] = __ldg(a.units + t);
+    __syncthreads();
+    const u32 m = blockIdx.x * AIR_BLOCK + threadIdx.x;
+    if (m >= a.rows) return;
+    AirShardDevEnv<F> env;
+    env.a = &a.q;
+    env.ap = air_sm;
+    env.sl = reinterpret_cast<u32 *>(air_sm + a.q.n_cons) + threadIdx.x;
+    env.s = &a;
+    env.tab = tab;
+    reinterpret_cast<uint4 *>(a.q.q)[m] = air_row_quotient<F, EXT>(env, a.q.d, a.q.n_insns, air_bitrev(a.row0 + m, a.q.d.log_q));
+}
+
 int32_t air_program_create(p3gpu_ctx *ctx, int field, const p3gpu_air_node *nodes, size_t n_nodes, const u32 *constraints, size_t n_constraints,
                            const p3gpu_air_layout &layout, p3gpu_air_program **out, bool check) {
     std::string err;
@@ -104,25 +154,28 @@ int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t 
     return P3GPU_OK;
 }
 
+// The launch arguments of either instance: checks the public values and alpha, builds the domain and stages the tables in one
+// copy: alpha table | Z_H | 1/Z_H | public values | (8-byte aligned) `units`, the sharded instance's unit table (*d_units).
 template <int F>
-static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, const u32 *d_pre, const u32 *d_periodic,
-                                   unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs, const u32 *alpha, u32 *d_q) {
+static int32_t air_quotient_args(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, const u32 *d_pre, const u32 *d_periodic,
+                                 unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs, const u32 *alpha, u32 *d_q,
+                                 const std::vector<u64> &units, AirQArgs &qa, const u64 **d_units) {
     const AirProgram &p = pg->prog;
     for (u32 k = 0; k < p.n_public; k++) P3_CHECK(pubs[k] < Fp<F>::P, P3GPU_EINVAL, "public value %u is not a canonical Montgomery word", k);
     for (int d = 0; d < 4; d++) P3_CHECK(alpha[d] < Fp<F>::P, P3GPU_EINVAL, "alpha is not a canonical Montgomery element");
     std::vector<u32> zh, izh;
-    AirQArgs qa;
     qa.d = air_domain<F>(log_q, log_n, p.uses, zh, izh);
     qa.d.periodic_mask = (1u << log_periodic_rows) - 1u;
     const std::vector<uint4> ap = air_alpha_table<F>(alpha, p.n_constraints);
-    // one staging copy: alpha table | Z_H | 1/Z_H | public values
     const size_t nz = zh.size(), words = (size_t)p.n_constraints * 4 + 2 * nz + p.n_public;
-    std::vector<u32> host(std::max<size_t>(words, 1));
+    const size_t unit_at = (words + 1) & ~(size_t)1;
+    std::vector<u32> host(std::max<size_t>(units.empty() ? words : unit_at + 2 * units.size(), 1));
     if (!ap.empty()) memcpy(host.data(), ap.data(), ap.size() * 16);
     u32 *h = host.data() + (size_t)p.n_constraints * 4;
     std::copy(zh.begin(), zh.end(), h);
     std::copy(izh.begin(), izh.end(), h + nz);
     std::copy(pubs, pubs + p.n_public, h + 2 * nz);
+    if (!units.empty()) memcpy(host.data() + unit_at, units.data(), units.size() * 8);
     void *tab = nullptr;
     P3_TRY(ctx_scratch2(ctx, host.size() * 4, &tab));
     P3_CUDA(cudaMemcpyAsync(tab, host.data(), host.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -134,6 +187,16 @@ static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, 
     qa.q = d_q;
     qa.pre = d_pre; qa.pre_width = p.pre_width;
     qa.periodic = d_periodic; qa.n_periodic = p.n_periodic;
+    if (d_units) *d_units = reinterpret_cast<const u64 *>(dt + unit_at);
+    return P3GPU_OK;
+}
+
+template <int F>
+static int32_t air_quotient_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_lde, const u32 *d_pre, const u32 *d_periodic,
+                                   unsigned log_periodic_rows, unsigned log_q, unsigned log_n, const u32 *pubs, const u32 *alpha, u32 *d_q) {
+    const AirProgram &p = pg->prog;
+    AirQArgs qa;
+    P3_TRY(air_quotient_args<F>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q, {}, qa, nullptr));
     const size_t smem = air_smem_bytes(p.n_slots, p.n_constraints);
     auto kern = (p.uses & AIR_USES_EXT) ? air_program_quotient_kernel<F, true> : air_program_quotient_kernel<F, false>;
     if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -182,6 +245,71 @@ int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const 
     if (field == BABY_BEAR)
         return air_quotient_launch<BABY_BEAR>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q);
     return air_quotient_launch<KOALA_BEAR>(ctx, pg, d_lde, d_pre, d_periodic, log_periodic_rows, log_q, log_n, pubs, alpha, d_q);
+}
+
+template <int F>
+static int32_t air_quotient_sharded_launch(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *own, const u32 *peer, const std::vector<u64> &units,
+                                           size_t smem, u32 row0, unsigned log_rows, const u32 *d_periodic, unsigned log_periodic_rows,
+                                           unsigned log_lde, unsigned log_n, const u32 *pubs, const u32 *alpha, u32 *d_q) {
+    const AirProgram &p = pg->prog;
+    AirShardQArgs sa;
+    P3_TRY(air_quotient_args<F>(ctx, pg, nullptr, nullptr, d_periodic, log_periodic_rows, log_lde, log_n, pubs, alpha, d_q, units, sa.q, &sa.units));
+    sa.own = own; sa.peer = peer;
+    sa.n_units = (u32)units.size(); sa.n_slots = p.n_slots; sa.row0 = row0; sa.rows = 1u << log_rows; sa.log_rows = log_rows;
+    auto kern = (p.uses & AIR_USES_EXT) ? air_program_quotient_sharded_kernel<F, true> : air_program_quotient_sharded_kernel<F, false>;
+    if (smem > 48 * 1024) P3_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<sa.rows / AIR_BLOCK, AIR_BLOCK, smem, ctx->stream>>>(sa);
+    ctx->launches++;
+    P3_CUDA(cudaGetLastError());
+    return P3GPU_OK;
+}
+
+int32_t air_program_quotient_sharded(p3gpu_ctx *ctx, const p3gpu_air_program *pg, unsigned world, unsigned rank, u32 *const *rows,
+                                     const size_t *col_starts, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_lde, unsigned log_n,
+                                     const u32 *pubs, const u32 *alpha, u32 *d_q) {
+    P3_CHECK(pg->device == ctx->device, P3GPU_EINVAL, "AIR program was created on device %d, the context is on device %d", pg->device, ctx->device);
+    P3_CHECK(!pg->check, P3GPU_EINVAL,
+             "the AIR program was created with p3gpu_air_check_program_create: evaluate the quotient of a p3gpu_air_program_create program");
+    const AirProgram &p = pg->prog;
+    const int field = p.field;
+    P3_CHECK(p.pre_width == 0, P3GPU_EUNSUPPORTED, "sharded AIR quotient: the program has %u preprocessed columns (no sharded preprocessed trace)",
+             p.pre_width);
+    const unsigned two_adicity = field == BABY_BEAR ? Fp<BABY_BEAR>::TWO_ADICITY : Fp<KOALA_BEAR>::TWO_ADICITY;
+    P3_CHECK(log_n <= log_lde && log_lde <= two_adicity, P3GPU_EINVAL, "sharded AIR quotient: need log_trace_height %u <= log_lde_height %u <= %u",
+             log_n, log_lde, two_adicity);
+    // the quotient domain is the LDE domain: its 2^log_lde points are the LDE's rows, and rank g owns points bitrev(g R + m)
+    P3_CHECK(log_lde - log_n <= AIR_MAX_RATE_BITS, P3GPU_EUNSUPPORTED,
+             "sharded AIR quotient: the quotient domain is the LDE domain, 2^%u over a trace of 2^%u rows: at most %u extra bits", log_lde, log_n,
+             AIR_MAX_RATE_BITS);
+    const unsigned log_g = log2_floor(world);
+    P3_CHECK(log_lde >= log_g && log_lde - log_g >= 10, P3GPU_EUNSUPPORTED,
+             "sharded AIR quotient: 2^%u LDE rows over %u ranks (at least 1024 rows per rank, as the sharded commit)", log_lde, world);
+    const unsigned log_rows = log_lde - log_g;
+    P3_CHECK(p.n_public == 0 || pubs != nullptr, P3GPU_EINVAL, "the program reads %u public values, none given", p.n_public);
+    P3_CHECK(reinterpret_cast<uintptr_t>(d_q) % 16 == 0, P3GPU_EINVAL, "sharded AIR quotient: misaligned quotient slice");
+    for (unsigned g = 0; g < world; g++)
+        P3_CHECK(reinterpret_cast<uintptr_t>(rows[g]) % 4 == 0, P3GPU_EINVAL, "sharded AIR quotient: misaligned row block of rank %u", g);
+    P3_CHECK((p.n_periodic > 0) == (d_periodic != nullptr), P3GPU_EINVAL, "periodic table %s, the program has %u periodic columns",
+             d_periodic ? "given" : "missing", p.n_periodic);
+    if (d_periodic) {
+        P3_CHECK(log_periodic_rows <= log_lde, P3GPU_EINVAL, "periodic table of 2^%u rows over a quotient domain of 2^%u", log_periodic_rows, log_lde);
+        P3_CHECK(reinterpret_cast<uintptr_t>(d_periodic) % 4 == 0, P3GPU_EINVAL, "sharded AIR quotient: misaligned periodic table");
+    } else {
+        log_periodic_rows = 0;
+    }
+    std::vector<u64> units;
+    P3_TRY(air_shard_units(world, col_starts, (size_t)1 << log_rows, p.width, units));
+    const size_t base = air_smem_bytes(p.n_slots, p.n_constraints), smem = base + units.size() * 8;
+    P3_CHECK(smem <= 227 * 1024, P3GPU_EUNSUPPORTED,
+             "sharded AIR quotient needs %zu bytes of shared memory, a block has %d: %u slots x %u B + %u constraints x 16 B + %zu units x 8 B",
+             smem, 227 * 1024, p.n_slots, AIR_BLOCK * 4, p.n_constraints, units.size());
+    const u32 *peer = (p.uses & AIR_USES_NEXT) ? rows[air_shard_next_rank(rank, log_g, log_lde - log_n)] : rows[rank];
+    const u32 row0 = rank << log_rows;
+    if (field == BABY_BEAR)
+        return air_quotient_sharded_launch<BABY_BEAR>(ctx, pg, rows[rank], peer, units, smem, row0, log_rows, d_periodic, log_periodic_rows, log_lde,
+                                                      log_n, pubs, alpha, d_q);
+    return air_quotient_sharded_launch<KOALA_BEAR>(ctx, pg, rows[rank], peer, units, smem, row0, log_rows, d_periodic, log_periodic_rows, log_lde,
+                                                   log_n, pubs, alpha, d_q);
 }
 
 // ---- hand-written AIR quotient kernels (keccak_air.cu, blake3_air.cu, poseidon1_air.cu) -----------------------------------

@@ -4,8 +4,8 @@
 //
 // This header holds everything that is not a CUDA launch — the node validation, the compiler, the per-instruction semantics, the
 // per-row quotient evaluation and the per-row constraint check — so host C++ can include it (tests/cpp/air_program_check.cpp and,
-// for the EXT instance, tests/cpp/air_layout_check.cpp run the quotient against the oracle on the CPU, tests/cpp/air_check_host.cpp
-// the check) exactly as the kernels do.
+// for the EXT instance, tests/cpp/air_layout_check.cpp run the quotient against the oracle on the CPU, tests/cpp/air_shard_check.cpp
+// the row-sharded quotient over chunk-major row blocks, tests/cpp/air_check_host.cpp the check) exactly as the kernels do.
 //
 //   nodes        p3gpu_air_node {op, a, b, imm} in topological order (operands refer only to earlier nodes)
 //   compile      drop dead nodes; per constraint in assertion order emit its not yet emitted cone (post-order), then FOLD it;
@@ -271,18 +271,40 @@ inline u64 air_unit_entry(u64 base, u64 stride) { return base | (stride << 48); 
 __device__ __forceinline__ void air_shard_table_load(const AirHandQArgs &a, u64 *tab) {
     for (u32 t = threadIdx.x; t < a.n_units; t += blockDim.x) tab[t] = __ldg(a.units + t);
 }
-// block row m of a row block, read through the unit table in shared memory
+#endif
+// block row m of a row block, read through the unit table (shared memory on the device; host C++ runs the same arithmetic)
 struct AirShardRow {
     const u32 *blk;
     const u64 *tab;
     u32 m;
-    __device__ __forceinline__ const u32 *at(u32 c) const {
+    __host__ __device__ __forceinline__ const u32 *at(u32 c) const {
         const u64 e = tab[c / AIR_UNIT];
         return blk + (e & AIR_UNIT_BASE_MASK) + (size_t)m * (u32)(e >> 48) + c;
     }
-    __device__ __forceinline__ u32 ld(u32 c) const { return __ldg(at(c)); }
-};
+    __host__ __device__ __forceinline__ u32 ld(u32 c) const {
+#ifdef __CUDA_ARCH__
+        return __ldg(at(c));
+#else
+        return *at(c);
 #endif
+    }
+};
+
+// ---- where a point's rows live in the row-sharded commit ------------------------------------------------------------------
+// Rank g holds memory rows [g R, (g + 1) R) of the bit-reversed LDE, R = 2^log_rows: memory row M is local row M mod R of rank
+// M / R.  Point i = bitrev(M) reads its next row at natural index i + 2^q, memory row bitrev(i + 2^q).  The owner of a memory row
+// is its top log2(G) bits, i.e. the low log2(G) bits of the natural index; those are bitrev(g) for every point of rank g, and adding
+// 2^q changes them the same way for all of them (a carry only leaves upwards).  So every next row of rank g lies on ONE rank,
+// bitrev((bitrev(g) + 2^q) mod G), which is g itself when G <= 2^q.
+struct AirShardLoc { u32 rank, row; };
+__host__ __device__ __forceinline__ AirShardLoc air_shard_locate(u32 mem_row, unsigned log_rows) {
+    return AirShardLoc{mem_row >> log_rows, mem_row & ((1u << log_rows) - 1u)};
+}
+__host__ __device__ __forceinline__ u32 air_shard_next_rank(u32 rank, unsigned log_world, unsigned q) {
+    if (q >= log_world) return rank;
+    const u32 mask = (1u << log_world) - 1u;
+    return air_bitrev((air_bitrev(rank, log_world) + (1u << q)) & mask, log_world);
+}
 
 // selectors_on_coset (commit/src/domain.rs:321-361) at x_i = g * w_q^i, unnormalised: Z_H / (x - 1), Z_H / (x - w^-1), x - w^-1.
 // zh = Z_H(x_i).  Shared by the constraint-program kernel and the hand-written Keccak AIR kernel (keccak_air.cu).

@@ -858,6 +858,16 @@ int32_t p3gpu_p1air_quotient_sharded_dev(p3gpu_ctx *ctx, int field, int vector_l
     return p1air_quotient_sharded(ctx, field, vector_len, sh, grp->rows[grp->rank], log_lde_height, log_trace_height, alpha, d_quotient_slice);
 }
 
+int32_t p3gpu_air_quotient_sharded_dev(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const p3gpu_peer_group *grp, const size_t *col_starts,
+                                       const uint32_t *d_periodic, unsigned log_periodic_rows, unsigned log_lde_height, unsigned log_trace_height,
+                                       const uint32_t *public_values, const uint32_t alpha[4], uint32_t *d_quotient_slice) {
+    P3_ENTER(ctx);
+    P3_TRY(check_group(grp, true));
+    P3_CHECK(prog && col_starts && alpha && d_quotient_slice, P3GPU_EINVAL, "null argument");
+    return air_program_quotient_sharded(ctx, prog, grp->world, grp->rank, grp->rows, col_starts, d_periodic, log_periodic_rows, log_lde_height,
+                                        log_trace_height, public_values, alpha, d_quotient_slice);
+}
+
 // TwoAdicFriPcs::commit of ONE trace whose columns are sharded over the ranks, bit-identical to the single-GPU commitment.
 int32_t p3gpu_commit_sharded_dev(p3gpu_ctx *ctx, int field, int hash, const p3gpu_peer_group *grp, uint32_t *epoch, const uint32_t *d_evals_local,
                                  size_t h, const size_t *col_starts, unsigned log_blowup, unsigned cap_height,

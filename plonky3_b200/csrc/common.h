@@ -170,6 +170,11 @@ int32_t air_program_info(const p3gpu_air_program *prog, size_t *n_insns, size_t 
 int32_t air_program_quotient(p3gpu_ctx *ctx, const p3gpu_air_program *prog, const u32 *d_lde, unsigned log_lde, const u32 *d_pre,
                              unsigned log_pre, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_q, unsigned log_n,
                              const u32 *pubs, const u32 *alpha, u32 *d_q, bool layout_entry);
+// rank `rank`'s row block rows[rank] of the row-sharded commit with column blocks col_starts (p3gpu_air_quotient_sharded_dev);
+// rows: every rank's row block (the peer blocks are read for next-row columns)
+int32_t air_program_quotient_sharded(p3gpu_ctx *ctx, const p3gpu_air_program *prog, unsigned world, unsigned rank, u32 *const *rows,
+                                     const size_t *col_starts, const u32 *d_periodic, unsigned log_periodic_rows, unsigned log_lde, unsigned log_n,
+                                     const u32 *pubs, const u32 *alpha, u32 *d_q);
 // air_check.cu: the debug constraint check of a check program over the trace domain; pass 1 writes d_counts (height words), pass 2
 // (d_counts null) the failing constraints of the n_rows listed rows at their offsets
 int32_t air_check(p3gpu_ctx *ctx, const p3gpu_air_program *pg, const u32 *d_trace, size_t height, const u32 *d_pre, const u32 *d_periodic,

@@ -380,6 +380,29 @@ def block_view(world: int, rank: int, block):
     return st
 
 
+def blocks_view(world: int, rank: int, blocks):
+    """A _lib.PeerGroupStruct that names every rank's row block, `blocks[q]` (CUDA tensors in the layout of `chunk_major_block`,
+    all on this device), as rank `rank` of a `world`-rank commit sees them: for the sharded quotient entry points, which read the own
+    block and, for a constraint program that reads the next row, the block of `next_row_rank`.  The control pointers are set to the
+    blocks to pass the group's null checks; nothing that exchanges, synchronises or hashes may be given this view."""
+    st = _lib.PeerGroupStruct()
+    st.world, st.rank, st.timeout_s = world, rank, 1.0
+    for q in range(world):
+        st.ctrl[q] = st.rows[q] = blocks[q].data_ptr()
+    return st
+
+
+def next_row_rank(rank: int, world: int, q: int) -> int:
+    """The one rank holding the next rows of every point of `rank`'s row block (air_program.cuh air_shard_next_rank): point i =
+    bitrev(M) of memory row M reads natural index i + 2^q, and the owner of a row is the low log2(world) bits of its natural index,
+    bitrev(rank) for all of rank's points, so the owner is bitrev((bitrev(rank) + 2^q) mod world).  `rank` itself when world <= 2^q."""
+    log_g = world.bit_length() - 1
+    assert world == 1 << log_g and 0 <= rank < world, "world is a power of two, rank below it"
+    if (1 << q) >= world:
+        return rank
+    return int(_bitrev((int(_bitrev(rank, log_g)) + (1 << q)) % world, log_g))
+
+
 def query_owner(index: int, rows_per_rank: int):
     """(rank, local row) holding row `index` of the bit-reversed LDE after the row-sharded commit."""
     return index // rows_per_rank, index % rows_per_rank
@@ -403,7 +426,8 @@ class ShardedTrace:
     """The trace's prover data and its opener when the trace's columns are split over the ranks of a PeerGroup: rank g holds
     columns [col_starts[g], col_starts[g+1]), and after the sharded commit LDE rows [g R, (g+1) R), R = LDE height / world, with
     its sub-tree.  `uni_stark.prove(config, air, block, shard=ShardedTrace(grp, col_starts))` proves with it any air.KernelAir that
-    has a sharded quotient kernel (the Poseidon2 AIR over KoalaBear, the Blake3, SHA-256 and Poseidon1 AIRs), under either
+    has a sharded quotient kernel (the Poseidon2 AIR over KoalaBear, the Blake3, SHA-256 and Poseidon1 AIRs) and any
+    constraint-program SymbolicAir without preprocessed columns (its next rows come from one peer's row block), under any
     configuration: the commit, the exchanges and the openings carry 8-word digests, which is what the Poseidon2, the Keccak and the
     SHA-256 MMCS write ([F; 8], [u64; 4] and [u8; 32]).
 
@@ -443,12 +467,12 @@ class ShardedTrace:
         self.path_len = self.log_height - min(mmcs.cap_height, self.log_height)
         return cap, self
 
-    def quotient_values(self, air, quotient_domain, alpha):
+    def quotient_values(self, air, quotient_domain, alpha, public_values=()):
         """The AIR's quotient values in natural order over the quotient domain, which must be the LDE domain: the AIR's sharded
         kernel on my rows in place, the bit-reversed slices all-gathered and put back in natural order by one gather."""
         assert quotient_domain[1] == self.log_height, "the sharded quotient covers the LDE domain: log_num_quotient_chunks == log_blowup"
         H = self.shape[0]
-        q_slice = air.sharded_quotient_values(self.grp, self.log_height, self.log_degree, alpha)
+        q_slice = air.sharded_quotient_values(self.grp, self.log_height, self.log_degree, alpha, public_values)
         q_bitrev = self.grp.exchange(q_slice).reshape(H, 4)
         return q_bitrev[_bitrev(torch.arange(H, device=self.device, dtype=torch.int64), self.log_height)].contiguous()
 
@@ -528,17 +552,74 @@ class ShardedTrace:
         return [np.ascontiguousarray(ans[:, :W])], np.ascontiguousarray(ans[:, W:]).reshape(n, plen, 8)
 
 
-def sharded_air_error(config, air):
-    """None, or why prove_sharded cannot prove `air` under `config`: it needs a StarkConfig, KeccakStarkConfig or Sha256StarkConfig
-    and an air.KernelAir
-    with a sharded quotient kernel whose constraints read the local row only (a row's next row lies on another rank)."""
-    from .air import KernelAir
+def _split_error(width: int, col_starts):
+    """None, or why the sharded commit (p3gpu_commit_sharded_dev) and the sharded constraint-program quotient cannot take a trace of
+    `width` columns split at `col_starts` (None: one rank).  The device's rules, decided on the host from the arguments alone:
+      * ntt_coset_lde_sharded: every column block, its offset and the width are multiples of 4 columns;
+      * its column-block LDE runs on the tiled pipeline (lde_tiled_impl), which takes at least 8 columns: the whole width at world 1
+        (the single rank's fused LDE), every non-empty block otherwise;
+      * air_shard_units: every segment of the chunk-major row block (shard_col_segments) starts on a multiple of 8 columns and ends on
+        one or at the width, so no 8-column unit spans two segments."""
+    starts = [0, width] if col_starts is None else [int(x) for x in col_starts]
+    world = len(starts) - 1
+    if world < 1 or world > 16 or world & (world - 1):
+        return f"{world} ranks: a power of two up to 16"
+    if starts[0] != 0 or starts[-1] != width or any(b < a for a, b in zip(starts, starts[1:])):
+        return f"column blocks {starts} do not split the {width} columns in order"
+    if width % 4:
+        return "the sharded commit's LDE takes multiples of 4 columns"
+    for g in range(world):
+        a, b = starts[g], starts[g + 1]
+        if a % 4 or b % 4:
+            return f"rank {g}'s column block [{a}, {b}) does not start and end on a multiple of 4 columns, as the sharded commit's LDE needs"
+        if 0 < b - a < 8:
+            return (f"rank {g}'s column block [{a}, {b}) has {b - a} columns, fewer than the 8 the sharded commit's tiled LDE takes"
+                    if world > 1 else f"fewer than the 8 columns the sharded commit's tiled LDE takes")
+    try:
+        segments = column_segments(world, starts, 1)
+    except _lib.P3GpuError as e:
+        return f"column blocks {starts}: {e}"
+    for c0, c1, _ in segments:
+        if c0 % 8 or (c1 % 8 and c1 != width):
+            return (f"column blocks {starts} leave a row-block segment [{c0}, {c1}) that cuts an 8-column unit of the sharded quotient's "
+                    "unit table")
+    return None
+
+
+def _symbolic_sharded_error(config, air, col_starts):
+    """sharded_air_error for a constraint-program SymbolicAir: every decision from the arguments, before any device call, so every
+    rank reaches the same one."""
+    from .uni_stark import KeccakStarkConfig, Sha256StarkConfig, StarkConfig, get_log_num_quotient_chunks
+    head = f"prove_sharded: SymbolicAir is a constraint-program AIR of {air.width()} columns; "
+    if air.preprocessed_width() > 0:
+        return head + (f"it has {air.preprocessed_width()} preprocessed columns, which would need a sharded commit of the preprocessed "
+                       "trace")
+    err = _split_error(air.width(), col_starts)
+    if err:
+        return head + err
+    if not isinstance(config, (StarkConfig, KeccakStarkConfig, Sha256StarkConfig)):
+        return head + f"{type(config).__name__} is not a StarkConfig or KeccakStarkConfig, nor a Sha256StarkConfig"
+    chunks, log_blowup = get_log_num_quotient_chunks(air), config.pcs.fri.log_blowup
+    if chunks != log_blowup:
+        return head + (f"log_num_quotient_chunks {chunks} (constraint degree {air.max_constraint_degree()}) differs from log_blowup "
+                       f"{log_blowup}: the sharded quotient covers the LDE domain only")
+    return None
+
+
+def sharded_air_error(config, air, col_starts=None):
+    """None, or why prove_sharded cannot prove `air` under `config` with the column blocks `col_starts` (None: not yet known; the
+    rules that depend on them are checked at world 1): it needs a StarkConfig, KeccakStarkConfig or Sha256StarkConfig and either an
+    air.KernelAir with a sharded quotient kernel whose constraints read the local row only (a row's next row lies on another rank),
+    or a constraint-program SymbolicAir without preprocessed columns, whose quotient domain is the LDE domain and whose columns the
+    sharded commit can take split at `col_starts`."""
+    from .air import KernelAir, SymbolicAir
     from .field import KoalaBear
     from .poseidon2_air import VectorizedPoseidon2Air
     from .uni_stark import KeccakStarkConfig, Sha256StarkConfig, StarkConfig
+    if not isinstance(air, SymbolicAir):
+        return f"prove_sharded: {type(air).__name__} is not an air.SymbolicAir"
     if not isinstance(air, KernelAir):
-        return (f"prove_sharded: {type(air).__name__} is a constraint-program AIR; only AIRs with hand-written kernels have a sharded "
-                "quotient")
+        return _symbolic_sharded_error(config, air, col_starts)
     name = air.air_name or type(air).__name__
     if air.main_next_row_columns():
         return f"prove_sharded: the {name} AIR reads the next row, which lies on another rank"
@@ -555,18 +636,21 @@ def sharded_air_error(config, air):
 def prove_sharded(config, air, grp: "PeerGroup", trace_block, col_starts, public_values=()):
     """uni_stark.prove with the trace sharded by column block over the ranks of `grp` (rank g holds columns [col_starts[g],
     col_starts[g+1]) of the 2^n-row trace), through ShardedTrace.  `config`: StarkConfig, KeccakStarkConfig or Sha256StarkConfig; `air`: the Poseidon2
-    AIR over KoalaBear, or the Blake3, SHA-256 or Poseidon1 AIR over either field (sharded_air_error says why another is refused,
-    before any device work).  Every rank returns the same Proof, byte for byte the one `uni_stark.prove` writes for the whole trace on
-    one GPU; its timings_ms are each span's maximum over the ranks."""
+    AIR over KoalaBear, the Blake3, SHA-256 or Poseidon1 AIR over either field, or a constraint-program SymbolicAir (next-row reads,
+    public values and periodic columns included; sharded_air_error says why another is refused, before any device work).  Every rank
+    returns the same Proof, byte for byte the one `uni_stark.prove` writes for the whole trace on one GPU; its timings_ms are each
+    span's maximum over the ranks."""
+    from .air import KernelAir
     from .uni_stark import get_log_num_quotient_chunks, prove
-    err = sharded_air_error(config, air)
+    err = sharded_air_error(config, air, col_starts)
     if err:
         raise ValueError(err)
     pcs = config.pcs
     assert grp.gpu is pcs.dft.gpu, "the PeerGroup and the config must share one GPU context"
-    assert len(public_values) == 0, f"the {air.air_name} AIR has no public values"
+    if isinstance(air, KernelAir):
+        assert len(public_values) == 0, f"the {air.air_name} AIR has no public values"
     assert get_log_num_quotient_chunks(air) == pcs.fri.log_blowup, "quotient domain must equal the LDE domain (fast path of get_evaluations_on_domain)"
-    proof = prove(config, air, trace_block, shard=ShardedTrace(grp, col_starts))
+    proof = prove(config, air, trace_block, public_values, shard=ShardedTrace(grp, col_starts))
     if grp.world > 1 and dist.is_initialized():
         every = [None] * grp.world
         dist.all_gather_object(every, proof.timings_ms, group=grp.group)

@@ -507,6 +507,24 @@ class Gpu:
                                                    self._ef(alpha).ctypes.data, q.data_ptr()))
         return q
 
+    def air_quotient_sharded(self, prog, group, col_starts, periodic_dev, log_lde_height, log_trace_height, public_values, alpha):
+        """p3gpu_air_quotient_sharded_dev: my row block's quotient values after the row-sharded commit, over the LDE domain: (R, 4),
+        R = 2^log_lde_height / world, the bit-reversed slice `rank`.  `group`: the _lib.PeerGroupStruct of the commit (every rank's row
+        block: mine is read in place, the one holding my next rows too), `col_starts`: the commit's world + 1 column offsets,
+        `periodic_dev`: the periodic table (None without periodic columns), public_values: Montgomery words."""
+        self._use_torch_stream()
+        per = self._dev(periodic_dev) if periodic_dev is not None else None
+        if per is not None and int(per.shape[0]) & (int(per.shape[0]) - 1):
+            raise _lib.P3GpuError(f"periodic table height {int(per.shape[0])} is not a power of two", _lib.EINVAL)
+        cs = (C.c_size_t * len(col_starts))(*[int(x) for x in col_starts])
+        pv = np.ascontiguousarray(public_values, dtype=np.uint32).ravel()
+        q = self._empty(((1 << log_lde_height) // int(group.world), 4))
+        check(self.L.p3gpu_air_quotient_sharded_dev(self.h, prog.h, C.byref(group), cs, per.data_ptr() if per is not None else None,
+                                                    int(per.shape[0]).bit_length() - 1 if per is not None else 0, log_lde_height,
+                                                    log_trace_height, pv.ctypes.data if pv.size else None, self._ef(alpha).ctypes.data,
+                                                    q.data_ptr()))
+        return q
+
     # ------------------------------------------------------------------ the debug constraint check (air.check_constraints)
     def air_check_program_create(self, field, nodes, constraints, layout):
         """A check program (p3gpu_air_check_program_create) of the DAG: layout = (width, n_public, preprocessed_width, n_periodic)."""

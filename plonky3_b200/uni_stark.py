@@ -9,9 +9,9 @@ p3gpu_air_quotient_layout_dev); poseidon2_air.VectorizedPoseidon2Air, the config
 koala-bear --objective poseidon-2-permutations --log-trace-length L -d radix-2-dit-parallel -m poseidon-2`),
 keccak_air.KeccakAir, blake3_air.Blake3Air, sha256_air.Sha256Air and poseidon1_air.VectorizedPoseidon1Air through their
 hand-written kernels.  With
-`shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 (KoalaBear), Blake3, SHA-256 and Poseidon1 AIRs with the
-trace's columns split over several GPUs, the shard standing in for the trace commit, the quotient values and the trace's row reads of
-the opening.
+`shard=distributed.ShardedTrace(...)` the same lines prove the Poseidon2 (KoalaBear), Blake3, SHA-256 and Poseidon1 AIRs and any
+constraint-program AIR without preprocessed columns with the trace's columns split over several GPUs, the shard standing in for the
+trace commit, the quotient values and the trace's row reads of the opening.
 
     trace (device)  --pcs.commit-->  trace cap ............................... p3gpu_coset_lde_batch_dev + p3gpu_merkle_commit_dev
     alpha <- transcript;  quotient values on GENERATOR * K ................... air.quotient_values (p3gpu_p2air_quotient_dev, ...)
@@ -208,8 +208,8 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
         err = periodic_column_error(periodic, degree)
         if err:
             raise ValueError(err)
-    if shard is not None and (pre_width or periodic):
-        raise ValueError("the row-sharded prove does not take preprocessed or periodic columns")
+    if shard is not None and pre_width:
+        raise ValueError("the row-sharded prove does not take preprocessed columns (it does take periodic columns)")
     if log_num_quotient_chunks > pcs.fri.log_blowup:
         # the quotient domain must lie inside the committed LDE (fast path of get_evaluations_on_domain); the reference asserts too
         raise ValueError(f"constraint degree {air.max_constraint_degree()} needs {num_quotient_chunks} quotient chunks: log_blowup "
@@ -248,7 +248,7 @@ def prove(config, air, trace, public_values=(), *, shard=None, preprocessed: Opt
         quotient_flat = air.quotient_values(trace_on_quotient_domain, log_degree, alpha, public_values,   # natural order = flatten_to_base
                                             preprocessed_on_quotient_domain=pre_q)
     else:
-        quotient_flat = shard.quotient_values(air, quotient_domain, alpha)
+        quotient_flat = shard.quotient_values(air, quotient_domain, alpha, public_values)
     span("compute quotient polynomial", t0)
 
     t0 = time.perf_counter()

@@ -36,6 +36,11 @@ int32_t ctx_scratch2(p3gpu_ctx *ctx, size_t bytes, void **out) {
     *out = ctx->scratch2;
     return P3GPU_OK;
 }
+int32_t ctx_lde_tiles(p3gpu_ctx *ctx, size_t bytes, void **out) {
+    P3_TRY(grow(&ctx->lde_tiles, &ctx->lde_tiles_bytes, bytes, ctx->stream));
+    *out = ctx->lde_tiles;
+    return P3GPU_OK;
+}
 
 int32_t ctx_pool(p3gpu_ctx *ctx, int slot, size_t bytes, void **out) {
     P3_TRY(grow(&ctx->pool[slot], &ctx->pool_bytes[slot], bytes ? bytes : 1, ctx->stream));
@@ -108,6 +113,7 @@ void p3gpu_ctx_destroy(p3gpu_ctx *ctx) {
     for (int f = 0; f < 2; f++) if (ctx->fold_table[f]) cudaFree(ctx->fold_table[f]);
     if (ctx->scratch) cudaFree(ctx->scratch);
     if (ctx->scratch2) cudaFree(ctx->scratch2);
+    if (ctx->lde_tiles) cudaFree(ctx->lde_tiles);
     if (ctx->p1_consts) cudaFree(ctx->p1_consts);
     for (int i = 0; i < 4; i++) if (ctx->pool[i]) cudaFree(ctx->pool[i]);
     if (ctx->xchg_stream) cudaStreamDestroy(ctx->xchg_stream);

@@ -97,6 +97,7 @@ struct p3gpu_ctx {
     // grow-only scratch
     void *scratch = nullptr; size_t scratch_bytes = 0;
     void *scratch2 = nullptr; size_t scratch2_bytes = 0;
+    void *lde_tiles = nullptr; size_t lde_tiles_bytes = 0;   // coset LDE: the fused pass's tile-major output (ntt.cu), used by nothing else
     void *pool[4] = {nullptr, nullptr, nullptr, nullptr}; size_t pool_bytes[4] = {0, 0, 0, 0};  // host-pointer wrappers / commit phase
     // Poseidon2 constants: [field][0: width 16, 1: width 24], host copy + device copy
     p3::Poseidon2Consts p2_host[2][2];
@@ -113,6 +114,7 @@ namespace p3 {
 
 int32_t ctx_scratch(p3gpu_ctx *ctx, size_t bytes, void **out);
 int32_t ctx_scratch2(p3gpu_ctx *ctx, size_t bytes, void **out);
+int32_t ctx_lde_tiles(p3gpu_ctx *ctx, size_t bytes, void **out);
 int32_t ctx_pool(p3gpu_ctx *ctx, int slot, size_t bytes, void **out);
 int32_t ctx_leaf_table(p3gpu_ctx *ctx, size_t bytes, void **out);  // grow-only cached device buffers (no malloc/free per call)
 

@@ -32,7 +32,10 @@
 // and forward pass 2, so the coefficients are written and read once.  Forward pass 2 runs on whole-row bands in 8-CTA clusters
 // (ntt_band_pass_kernel: one bulk copy per eighth of a band in and out, the three cross-CTA layers over distributed shared
 // memory, overlapped with another band's local layers) where an eighth fits its ring slot; matrices of up to 48 columns keep
-// 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  Inverse pass 1 runs on the same kernel where a part fits
+// 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  On the 8-CTA kernel with whole column tiles, the fused pass
+// stores each tile as one dense block of a tile-major scratch and forward pass 2 gathers its rows from those blocks
+// (make_tile_major_tensor_maps): the corner turn between the two passes is done by tensor loads, not by short strided stores.
+// Inverse pass 1 runs on the same kernel where a part fits
 // (100 columns at 2^20 rows, 100-200 at 2^18), its "bands" being the strided units of rows 2^10 apart, each part moved by one 3-D
 // tensor copy.
 // Every other LDE runs the four passes as separate launches.
@@ -90,6 +93,7 @@ struct PassArgs {
     u32 in_tiled, out_tiled;   // pipelined kernel: intermediate buffers in column-tile-major layout (see lde_tiled_impl)
     u32 in_blocks;             // pipelined kernel, tiled input: 2^log_n-row blocks per column tile (cosets)
     u32 n_items, csplit, tpi;  // pipelined kernel: work items = (row tile, coset) units x csplit column chunks of tpi tiles
+    u32 tile_major;            // fused LDE pass: store each finished tile as one dense block of the tile-major scratch (launch_lde_mid)
     unsigned long long *prof;  // profiling build only: per CTA/tile phase timestamps (P3GPU_NTT_PROFBUF)
     int log_n, l0, l1;
     const uint2 *tw;  // heap-ordered twiddles of coset 0
@@ -609,6 +613,13 @@ __device__ __forceinline__ void tma_store_part(const CUtensorMap *map, const voi
                  ::"l"(reinterpret_cast<unsigned long long>(map)), "r"((u32)__cvta_generic_to_shared(smem)), "r"(0), "r"(unit), "r"(row0) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// a band's part gathered from the tile-major scratch through a 5-D tensor map (column, column tile, block row, tile row, coset): see
+// make_tile_major_tensor_maps
+__device__ __forceinline__ void tma_load_gather(const CUtensorMap *map, void *smem, u32 T, u32 l0, u32 coset, u32 bar) {
+    asm volatile("cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
+                 ::"r"((u32)__cvta_generic_to_shared(smem)), "l"(reinterpret_cast<unsigned long long>(map)), "r"(0), "r"(0), "r"(T), "r"(l0),
+                   "r"(coset), "r"(bar) : "memory");
+}
 
 // The band's layers as both band kernels split them: LX cross-CTA layers (step X), then QA (step A) and QB (step B) local layers
 // on each CTA's part of RQ rows.
@@ -713,9 +724,13 @@ __device__ __forceinline__ void band_store_part(const PassArgs &a, const u32 *pa
 // loaded once with slot 0's first load.  The network is linear, so the scale by a.scale is applied where the values leave step B, on
 // the 14 local warps: in step X it made the 6 exchange warps the ones that set the period (DESIGN 4.1).  The ring has a fourth slot,
 // which the one twiddle table leaves room for.
-template <int F, int R_LOG, int CL, bool STRIDED>
+// GATHER: the last pass of the LDE reading the fused pass's tile-major scratch a.in (launch_lde_mid) instead of a dense block: CTA q's
+// part of band T, rows L in [q*RQ, (q+1)*RQ), is block row T of the blocks of tiles L, and comes in as ONE 5-D tensor copy (imap,
+// make_tile_major_tensor_maps) whose box lands as the same row-major part.  Everything else is the contiguous band's.
+template <int F, int R_LOG, int CL, bool GATHER, bool STRIDED>
 __global__ void __launch_bounds__(BAND_THREADS, 1)
 ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap) {
+    static_assert(!(GATHER && STRIDED), "the gather mode is the last pass's");
     constexpr u32 RQ = BandShape<R_LOG, CL>::RQ, R = 1u << R_LOG;
     constexpr u32 NX = 32 * BAND_XWARPS, NL = 32 * BAND_LWARPS;    // threads [0, NX) exchange, [NX, NX + NL) local, then the copy warp
     constexpr u32 NS = STRIDED ? 4 : 3;                            // ring slots
@@ -745,6 +760,14 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
             mbar_expect_tx(bar, (load ? qwords * 4 : 0) + (tw ? 8 * (R - 2) : 0));
             if (load) tma_load_part(&imap, data0 + s * qwords, T, q * RQ, bar);
             if (tw) load_tile_twiddles(tws0, a.tw, 0, 0, R_LOG, bar);
+        } else if constexpr (GATHER) {
+            const uint2 *tw = a.tw + (size_t)coset * a.tw_stride;
+            uint2 *tws = tws0 + s * R;
+            const bool load = !P3_SKIP(a.skip_load);
+            tws[1] = tw[((size_t)1 << a.l0) + T];
+            mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
+            if (load) tma_load_gather(&imap, data0 + s * qwords, T, q * RQ, coset, bar);
+            load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
         } else {
             band_load_part<R_LOG, CL>(a, data0 + s * qwords, tws0 + s * R, coset, T, q, bar);
         }
@@ -869,8 +892,8 @@ __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_k
 //     gf + j*E1, gf = bitrev_Q1(g)), so the coefficients stay in that thread's registers for all cosets;
 //   * per coset: forward step 1 in registers, stored to the tile buffer in forward layout, then forward step 2 (Q1 layers) on
 //     consecutive local rows, in place; ONE tensor copy (omap) stores the tile to that coset's output block, where the
-//     four-launch path's forward pass 1 stores it; the next coset rewrites the buffer once the copy has read it out, and the
-//     HBM writes drain while the CTA computes;
+//     four-launch path's forward pass 1 stores it (a.tile_major: as one dense block of the tile-major scratch instead); the next
+//     coset rewrites the buffer once the copy has read it out, and the HBM writes drain while the CTA computes;
 //   * work items go in forward-tile order (L, column tile), T = bitrev_r(L): the CTAs resident at once store neighbouring
 //     output rows (runs of ~26 rows per 2^r-row group at 132 SMs) instead of rows 2^r / 32 apart, while each tile's
 //     reads stay one contiguous block of 2^r rows.
@@ -975,8 +998,10 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                         unsigned long long w0_, w1_;
                         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
 #endif
-                        // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
-                        tma_store_tile_keep(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
+                        // tensor coordinates (column, 0, 0, L, coset), tile-major (0, 0, 0, tile, coset): see launch_lde_mid
+                        // (tile-major blocks are written in whole lines: no L2 hint, which measured the same or slower there)
+                        if (a.tile_major) tma_store_tile(&omap, data0 + b * buf_words, 0, (int)tt, (int)cs);
+                        else tma_store_tile_keep(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
                         bulk_wait_read();   // the copy has read the buffer out: the next coset (or tile) may rewrite it
 #ifdef P3GPU_NTT_PROFILE
                         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
@@ -1110,8 +1135,11 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             } else if (!P3_SKIP(a.skip_store)) {
                 fence_proxy_async_smem();
                 __syncthreads();
-                // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
-                if (threadIdx.x == 0) tma_store_tile(&omap, data, (int)col, (int)L, (int)cs);
+                // tensor coordinates (column, 0, 0, L, coset), tile-major (0, 0, 0, tile, coset): see launch_lde_mid
+                if (threadIdx.x == 0) {
+                    if (a.tile_major) tma_store_tile(&omap, data, 0, (int)t, (int)cs);
+                    else tma_store_tile(&omap, data, (int)col, (int)L, (int)cs);
+                }
             }
         }
 #ifdef P3GPU_NTT_PROFILE
@@ -1550,22 +1578,28 @@ static bool band_pass_eligible(const PassArgs &a) {
 // 0.28 ms at 4, 0.41 against 0.50 at 48), the 8-CTA kernel from 64 (0.56 against 0.65 ms) and at every wider shape (DESIGN 4.1).
 constexpr u32 BAND_NARROW_W = 48;
 static int32_t make_unit_tensor_map(const u32 *base, u32 w, int log_n, int r, u32 rows, CUtensorMap *tm);
-template <int F, int R_LOG, bool NARROW, bool STRIDED = false>
-static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
+// GATHER: a.in is the fused pass's tile-major scratch, read through gmap (make_tile_major_tensor_maps)
+template <int F, int R_LOG, bool NARROW, bool STRIDED = false, bool GATHER = false>
+static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a, const CUtensorMap *gmap = nullptr) {
     static_assert(!(NARROW && STRIDED), "the strided first pass runs in 8-CTA clusters only");
+    static_assert(!(NARROW && GATHER), "the gather mode runs in 8-CTA clusters only");
     constexpr int CL = NARROW ? 4 : BAND_CL, SLOTS = NARROW ? 2 : 3;
     const size_t qbytes = (((size_t)a.w * 4) << R_LOG) / CL;
     const size_t tw_bytes = ((size_t)1 << R_LOG) * sizeof(uint2);
     const size_t smem = STRIDED ? 4 * (qbytes + 8) + tw_bytes : SLOTS * (qbytes + tw_bytes + 8);
     constexpr auto kern = [] {
         if constexpr (NARROW) return ntt_band_pass_narrow_kernel<F, R_LOG, CL>;
-        else return ntt_band_pass_kernel<F, R_LOG, CL, STRIDED>;
+        else return ntt_band_pass_kernel<F, R_LOG, CL, GATHER, STRIDED>;
     }();
     CUtensorMap imap, omap;
     memset(&imap, 0, sizeof imap); memset(&omap, 0, sizeof omap);
     if constexpr (STRIDED) {
         P3_TRY(make_unit_tensor_map(a.in, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &imap));
         P3_TRY(make_unit_tensor_map(a.out, a.w, a.log_n, R_LOG, (1u << R_LOG) / CL, &omap));
+    }
+    if constexpr (GATHER) {
+        P3_CHECK(gmap != nullptr, P3GPU_EINVAL, "ntt: the gather band pass needs its tensor map");
+        imap = *gmap;
     }
     // per instantiation and device: the number of clusters that fit at once, for the size set_smem_limit last saw
     static int clusters[64] = {0};
@@ -1592,12 +1626,22 @@ static int32_t launch_band_r(p3gpu_ctx *ctx, PassArgs a) {
     ctx->launches++;
     return P3GPU_OK;
 }
+// gmap != nullptr: the gather mode over the fused pass's tile-major scratch a.in (w > BAND_NARROW_W, see coset_lde_impl)
 template <int F>
-static int32_t launch_band(p3gpu_ctx *ctx, PassArgs a) {
+static int32_t launch_band(p3gpu_ctx *ctx, PassArgs a, const CUtensorMap *gmap = nullptr) {
     // profiling build only: NOLOAD / NOSTORE skip the part's bulk copies, NOBFLY bit 0 steps A and B, bit 1 the exchange
     a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0);
     a.skip_load = env_int("P3GPU_NTT_NOLOAD", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
     const bool narrow = a.w <= BAND_NARROW_W;
+    if (gmap) {
+        P3_CHECK(!narrow, P3GPU_EINVAL, "ntt: the gather band pass needs more than %u columns", BAND_NARROW_W);
+        switch (a.l1 - a.l0) {
+            case 7: return launch_band_r<F, 7, false, false, true>(ctx, a, gmap);
+            case 8: return launch_band_r<F, 8, false, false, true>(ctx, a, gmap);
+            case 9: return launch_band_r<F, 9, false, false, true>(ctx, a, gmap);
+            default: return launch_band_r<F, 10, false, false, true>(ctx, a, gmap);
+        }
+    }
     switch (a.l1 - a.l0) {
         case 7: return narrow ? launch_band_r<F, 7, true>(ctx, a) : launch_band_r<F, 7, false>(ctx, a);
         case 8: return narrow ? launch_band_r<F, 8, true>(ctx, a) : launch_band_r<F, 8, false>(ctx, a);
@@ -1731,6 +1775,42 @@ static int32_t make_unit_tensor_map(const u32 *base, u32 w, int log_n, int r, u3
     return P3GPU_OK;
 }
 
+// The tile-major scratch between the fused LDE pass and the gathering last pass (2^2r rows of w = n_ct * ct columns, n_cosets
+// cosets).  Coset cs's forward tile L and column tile c make tile tt = L * n_ct + c, whose result is ONE dense block of 2^r rows x ct
+// words at word offset ((cs * 2^r + L) * n_ct + c) * 2^r * ct.  Block row i = j * 2^Q1 + b (forward step 2's local row) holds what
+// goes to row L + 2^r * i of the coset block, so row L of band i is block row i of tiles L * n_ct .. L * n_ct + n_ct - 1.
+// The fused pass stores a block as 2^Q2 runs of 2^Q1 * ct contiguous words, where the dense layout writes 2^r row segments of ct
+// words 2^r rows apart; the last pass then gathers each row of its part from n_ct blocks instead of reading one contiguous run.
+//   store map (ntt_lde_mid_kernel): (column, b, j, tile tt, coset), box (ct, 2^Q1 + 1, 2^Q2, 1, 1) = the padded forward layout, whose
+//     pad row per group the store skips;
+//   gather map (ntt_band_pass_kernel<..., GATHER>): (column, column tile, block row i, tile row L, coset), box (ct, n_ct, 1, rows, 1):
+//     rows L .. L + rows - 1 of band i, w words each, land row-major as one part.
+static int32_t encode_tile_major(TensorMapEncodeFn enc, const u32 *base, const cuuint64_t *dims, const cuuint64_t *strides, const cuuint32_t *box,
+                                 CUtensorMap *tm) {
+    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+    const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
+    return P3GPU_OK;
+}
+static int32_t make_tile_major_tensor_maps(const u32 *base, u32 ct, u32 n_ct, int r, u32 n_cosets, u32 rows, CUtensorMap *store_map,
+                                           CUtensorMap *gather_map) {
+    TensorMapEncodeFn enc = tensor_map_encoder();
+    P3_CHECK(enc != nullptr, P3GPU_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
+    const int q1 = r / 2;
+    const cuuint64_t seg = (cuuint64_t)ct * 4, blk = seg << r, tile_row = blk * n_ct, coset = tile_row << r;
+    {
+        const cuuint64_t dims[5] = {ct, 1ull << q1, 1ull << (r - q1), (cuuint64_t)n_ct << r, n_cosets};
+        const cuuint64_t strides[4] = {seg, seg << q1, blk, coset};
+        const cuuint32_t box[5] = {ct, (1u << q1) + 1, 1u << (r - q1), 1, 1};
+        P3_TRY(encode_tile_major(enc, base, dims, strides, box, store_map));
+    }
+    const cuuint64_t dims[5] = {ct, n_ct, 1ull << r, 1ull << r, n_cosets};
+    const cuuint64_t strides[4] = {blk, seg, tile_row, coset};
+    const cuuint32_t box[5] = {ct, n_ct, 1, rows, 1};
+    return encode_tile_major(enc, base, dims, strides, box, gather_map);
+}
+
 // P3GPU_NTT_PIPE (read per call: the tests switch between the kernel families): 1 = TMA pipeline for every eligible pass and
 // the tiled LDE for every eligible LDE, 0 = never, unset (-1) = the H100 choice: dense passes of 10 layers on the cp.async
 // kernel, everything else eligible on the pipeline.  Measured on H100 (400 W), ms, cp.async kernel (512 threads) vs pipeline
@@ -1826,19 +1906,22 @@ static u32 lde_mid_tile_width(u32 w) {
 
 // a: the inverse network's second pass (l0 = r, l1 = 2r) over the coefficient buffer, writing the forward networks' first-pass
 // results of a.n_cosets cosets to a.out (blocks a.out_stride apart); tw_fwd: the cosets' forward heaps, a.tw_stride apart.
+// tile_map != nullptr: the results go to the tile-major scratch instead (make_tile_major_tensor_map), one dense block per tile.
 template <int F>
-static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd) {
+static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd, const CUtensorMap *tile_map = nullptr) {
     a.ct = lde_mid_tile_width(a.w);
     a.n_ctiles = (a.w + a.ct - 1) / a.ct;
     a.prof = prof_window();
     a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
+    a.tile_major = tile_map != nullptr;
     // output = the forward networks' first pass (layers [0, r)) over the cosets' blocks: tile L, local row j*2^Q1 + b at row
     // L + 2^r * (j*2^Q1 + b), i.e. the pass map with groups of 2^Q1 rows (the forward layout gs2 = (2^Q1 + 1) * ct words)
     const int r = a.l1 - a.l0;
     PassArgs o = a;
     o.l0 = 0; o.l1 = r;
     CUtensorMap omap, imap;
-    P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
+    if (tile_map) omap = *tile_map;
+    else P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
     // input (producer-warp form): inverse tile T = coefficient rows T * 2^r + rho in the inverse layout, groups of 2^ceil(r/2) rows
     P3_TRY(make_pass_tensor_map(a, a.in, false, 0, a.ct, false, (r + 1) / 2, &imap));
     switch (r) {
@@ -2114,18 +2197,35 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
         a.tw = tw_inv; a.in = d_in; a.out = (u32 *)coef; a.has_scale = 1; a.scale = inv_height_scale<F>(h);
         if (band_first_pass_eligible(a)) P3_TRY(launch_band_first<F>(ctx, a));
         else P3_TRY(launch_pass<F>(ctx, a, 1, 4));
-        memset(&a, 0, sizeof a);
-        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
-        a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;
-        P3_TRY(launch_lde_mid<F>(ctx, a, tw));
-        memset(&a, 0, sizeof a);
-        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
-        a.tw = tw; a.tw_stride = h; a.in = d_out; a.in_stride = h * w; a.out = d_out; a.out_stride = h * w; a.final_reduce = 1;
         // forward pass 2 reads and writes contiguous bands of 2^r rows: eighths of bands as single bulk copies in 8-CTA clusters
         // (ntt_band_pass_kernel; up to 48 columns ntt_band_pass_narrow_kernel) where an eighth fits a ring slot; P3GPU_NTT_BAND=0
         // keeps the tile kernel
-        if (band_pass_eligible(a)) return launch_band<F>(ctx, a);
-        return launch_pass<F>(ctx, a, (unsigned)n_cosets, 4);
+        PassArgs b;
+        memset(&b, 0, sizeof b);
+        b.w = (u32)w; b.log_n = log_n; b.l0 = r; b.l1 = log_n; b.n_cosets = (u32)n_cosets;
+        b.tw = tw; b.tw_stride = h; b.in = d_out; b.in_stride = h * w; b.out = d_out; b.out_stride = h * w; b.final_reduce = 1;
+        const bool band = band_pass_eligible(b);
+        // Tile-major plan (make_tile_major_tensor_maps): the fused pass stores each tile as one dense block of its own scratch, and
+        // the 8-CTA band pass gathers each part's rows from those blocks with one tensor copy, so that the corner turn between the
+        // two happens in the loads, which take short segments far better than stores do (DESIGN 4.1).  Only for whole column tiles,
+        // at least two of them; P3GPU_NTT_GATHER=0 keeps the dense layout.  The scratch holds every coset: band i's output rows
+        // hold tile i's blocks, which every band reads.
+        const u32 ct = lde_mid_tile_width((u32)w), n_ct = (u32)w / ct;
+        CUtensorMap store_map, gather_map;
+        bool gather = band && w > BAND_NARROW_W && w % ct == 0 && n_ct >= 2 && env_int("P3GPU_NTT_GATHER", 1) != 0;
+        if (gather) {
+            void *tiles = nullptr;
+            P3_TRY(ctx_lde_tiles(ctx, n_cosets * h * w * 4, &tiles));
+            gather = make_tile_major_tensor_maps((const u32 *)tiles, ct, n_ct, r, (u32)n_cosets, (1u << r) / BAND_CL, &store_map,
+                                                 &gather_map) == P3GPU_OK;
+            if (gather) b.in = (const u32 *)tiles;
+        }
+        memset(&a, 0, sizeof a);
+        a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
+        a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;
+        P3_TRY(launch_lde_mid<F>(ctx, a, tw, gather ? &store_map : nullptr));
+        if (band) return launch_band<F>(ctx, b, gather ? &gather_map : nullptr);
+        return launch_pass<F>(ctx, b, (unsigned)n_cosets, 4);
     }
     P3_TRY(run_network<F>(ctx, log_n, w, tw_inv, 0, 1, d_in, 0, 0, (u32 *)coef, 0, 0, 0, 0, nullptr, true, inv_height_scale<F>(h), false));
     if (bitrev_rows) {

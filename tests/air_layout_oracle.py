@@ -11,6 +11,7 @@ The new leaves become main-trace columns of an extended LDE prefix that tests/ai
                                      or, for a stand-in device, row i mod (table height) of a given table
 """
 import numpy as np
+import torch
 
 import air_oracle as A
 
@@ -23,16 +24,16 @@ def periodic_values(fid, column, log_q, log_n):
     p = A._PRIMES[fid]
     col = np.asarray(column, dtype=np.int64) % p
     per = col.size
-    x = A._GEN[fid] * A._powers(A._root(fid, log_q), 1 << log_q, p) % p
+    x = (A._GEN[fid] * A._powers(A._root(fid, log_q), 1 << log_q, p, "cpu") % p).numpy()
     if per == 1:
         return np.full(x.shape, int(col[0]), dtype=np.int64)
     w_inv = pow(A._root(fid, per.bit_length() - 1), p - 2, p)
     n_inv = pow(per, p - 2, p)
     coeffs = []
     for k in range(per):                                               # c_k = (1/p) sum_j v_j w^(-jk)
-        wk = A._powers(pow(w_inv, k, p), per, p)
+        wk = A._powers(pow(w_inv, k, p), per, p, "cpu").tolist()
         coeffs.append(int(sum(int(v) * int(t) % p for v, t in zip(col, wk)) % p * n_inv % p))
-    y = A._vpow(x, (1 << log_n) // per, p)
+    y = A._vpow(torch.from_numpy(x), (1 << log_n) // per, p).numpy()
     acc = np.zeros_like(x)
     for c in reversed(coeffs):
         acc = (acc * y + c) % p
@@ -54,7 +55,7 @@ def air_quotient(fid, nodes, constraints, lde_bitrev, log_q, log_n, public_value
         pre = np.asarray(pre_lde_bitrev, dtype=np.uint32)[:size]
         pre_width = pre.shape[1]
         blocks.append(pre)
-    rows = A._bitrev(log_q)
+    rows = A._bitrev(torch.arange(size, dtype=torch.int64), log_q).numpy()
     if periodic_table is not None:
         t = np.asarray(periodic_table, dtype=np.uint32)
         nat = t[np.arange(size) % t.shape[0]]

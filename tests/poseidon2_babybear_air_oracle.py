@@ -12,6 +12,7 @@ on canonical int64, written from the reference independently of `poseidon2_eval`
 The internal diagonal is the C oracle's Poseidon2BabyBear<16> diagonal (O.poseidon2_diag), not the one `poseidon2_eval` spells out.
 """
 import numpy as np
+import torch
 
 import air_oracle as A
 from oracle import p3_oracle as O
@@ -157,7 +158,7 @@ def quotient(c: RoundConstants, lde_bitrev, log_n, alpha_monty, vector_len=8):
     lde = np.asarray(lde_bitrev, dtype=np.uint32)
     H = lde.shape[0]
     log_h = H.bit_length() - 1
-    vals = constraint_values(c, lde[A._bitrev(log_h)], vector_len)              # natural order
+    vals = constraint_values(c, lde[A._bitrev(torch.arange(H), log_h).numpy()], vector_len)      # natural order
     K = vals.shape[1]
     alpha = [F.from_monty(int(v)) for v in alpha_monty]
     apow = [[1, 0, 0, 0]]
@@ -168,7 +169,7 @@ def quotient(c: RoundConstants, lde_bitrev, log_n, alpha_monty, vector_len=8):
     lo, hi = coef & 0xFFFF, coef >> 16                                          # 31 x 16-bit products: 2^47 each, sums < 2^59
     for d in range(4):
         acc[:, d] = ((vals @ lo[:, d]) % P + (vals @ hi[:, d]) % P * (1 << 16)) % P
-    x = F.GENERATOR * A._powers(A._root(F.id, log_h), H, P) % P
+    x = F.GENERATOR * A._powers(A._root(F.id, log_h), H, P, "cpu") % P
     zh = (A._vpow(x, 1 << log_n, P) - 1) % P
-    out = acc * A._vpow(zh, P - 2, P)[:, None] % P
+    out = acc * A._vpow(zh, P - 2, P).numpy()[:, None] % P
     return ((out << 32) % P).astype(np.uint32)

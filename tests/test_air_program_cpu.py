@@ -148,6 +148,8 @@ def test_random_dags_match_oracle(checker, f, seed, shape):
     exp = A.air_quotient(f.id, nodes, cons, lde, log_n + q, log_n, pubs, alpha)
     bad = np.flatnonzero((got != exp).any(axis=1))
     assert bad.size == 0, f"first differing row {bad[:1]}"
+    # the oracle in chunks of 3 natural indices (each gathering its own rows, next rows and selectors) gives the same words
+    assert np.array_equal(A.air_quotient(f.id, nodes, cons, lde, log_n + q, log_n, pubs, alpha, chunk_points=3), exp)
     reachable = n_insn - len(cons)                                    # every emitted compute instruction is one live node
     assert slots == live <= reachable
 

@@ -33,14 +33,14 @@
 // (ntt_band_pass_kernel: one bulk copy per eighth of a band in and out, the three cross-CTA layers over distributed shared
 // memory, overlapped with another band's local layers) where an eighth fits its ring slot; matrices of up to 48 columns keep
 // 4-CTA clusters without the overlap (ntt_band_pass_narrow_kernel).  On the 8-CTA kernel with whole column tiles, the fused pass
-// stores each tile as one dense block of a tile-major scratch and forward pass 2 gathers its rows from those blocks
+// stores each tile from registers as one dense block of a tile-major scratch and forward pass 2 gathers its rows from those blocks
 // (make_tile_major_tensor_maps): the corner turn between the two passes is done by tensor loads, not by short strided stores.
 // Inverse pass 1 runs on the same kernel where a part fits
 // (100 columns at 2^20 rows, 100-200 at 2^18), its "bands" being the strided units of rows 2^10 apart, each part moved by one 3-D
 // tensor copy.
 // Every other LDE runs the four passes as separate launches.
 // The fused pass runs warp-specialised where its registers allow (all instances but the runtime-width one at r = 10): a producer
-// lane loads each tile with one tensor copy and owns the tile stores and their read-out waits (DESIGN 4.1).
+// lane loads each tile with one tensor copy and, on the dense plan, owns the tile stores and their read-out waits (DESIGN 4.1).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -93,7 +93,6 @@ struct PassArgs {
     u32 in_tiled, out_tiled;   // pipelined kernel: intermediate buffers in column-tile-major layout (see lde_tiled_impl)
     u32 in_blocks;             // pipelined kernel, tiled input: 2^log_n-row blocks per column tile (cosets)
     u32 n_items, csplit, tpi;  // pipelined kernel: work items = (row tile, coset) units x csplit column chunks of tpi tiles
-    u32 tile_major;            // fused LDE pass: store each finished tile as one dense block of the tile-major scratch (launch_lde_mid)
     unsigned long long *prof;  // profiling build only: per CTA/tile phase timestamps (P3GPU_NTT_PROFBUF)
     int log_n, l0, l1;
     const uint2 *tw;  // heap-ordered twiddles of coset 0
@@ -613,6 +612,19 @@ __device__ __forceinline__ void tma_store_part(const CUtensorMap *map, const voi
                  ::"l"(reinterpret_cast<unsigned long long>(map)), "r"((u32)__cvta_generic_to_shared(smem)), "r"(0), "r"(unit), "r"(row0) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// Block row of forward row i = j * 2^Q1 + b (j < 2^Q2, b < 2^Q1: forward step 2's item j, register b, with Q1 and Q2 as
+// ntt_lde_mid_kernel splits r) in a tile-major block: b * 2^Q2 + j, so that register b of consecutive items is one contiguous run.
+// The map moves bit fields, so it splits over them: tile_block_row(j * 2^Q1 + b) = tile_block_row(j * 2^Q1) + tile_block_row(b).
+template <int R_LOG> __host__ __device__ constexpr u32 tile_block_row(u32 i) {
+    constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
+    return ((i & ((1u << Q1) - 1u)) << Q2) + (i >> Q1);
+}
+// its inverse: the forward row i that block row p holds
+template <int R_LOG> __host__ __device__ constexpr u32 tile_block_row_inv(u32 p) {
+    constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
+    return ((p & ((1u << Q2) - 1u)) << Q1) + (p >> Q2);
+}
+static_assert(tile_block_row_inv<7>(tile_block_row<7>(37)) == 37 && tile_block_row<7>(37) == 5 * 16 + 4, "tile-major block rows");
 // a band's part gathered from the tile-major scratch through a 5-D tensor map (column, column tile, block row, tile row, coset): see
 // make_tile_major_tensor_maps
 __device__ __forceinline__ void tma_load_gather(const CUtensorMap *map, void *smem, u32 T, u32 l0, u32 coset, u32 bar) {
@@ -725,8 +737,9 @@ __device__ __forceinline__ void band_store_part(const PassArgs &a, const u32 *pa
 // the 14 local warps: in step X it made the 6 exchange warps the ones that set the period (DESIGN 4.1).  The ring has a fourth slot,
 // which the one twiddle table leaves room for.
 // GATHER: the last pass of the LDE reading the fused pass's tile-major scratch a.in (launch_lde_mid) instead of a dense block: CTA q's
-// part of band T, rows L in [q*RQ, (q+1)*RQ), is block row T of the blocks of tiles L, and comes in as ONE 5-D tensor copy (imap,
-// make_tile_major_tensor_maps) whose box lands as the same row-major part.  Everything else is the contiguous band's.
+// part of band T, rows L in [q*RQ, (q+1)*RQ), is block row tile_block_row(T) of the blocks of tiles L, and comes in as ONE 5-D tensor copy (imap,
+// make_tile_major_tensor_maps) whose box lands as the same row-major part.  A cluster's bands go in block-row order (out_of).
+// Everything else is the contiguous band's.
 template <int F, int R_LOG, int CL, bool GATHER, bool STRIDED>
 __global__ void __launch_bounds__(BAND_THREADS, 1)
 ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__ CUtensorMap imap, const __grid_constant__ CUtensorMap omap) {
@@ -748,7 +761,13 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
     const u32 total = a.n_cosets << band_log;
     const int n = (int)((total - 1 - cid) / n_clusters) + 1;      // this cluster's bands: cid + k * n_clusters, k < n (grid <= bands)
 
-    auto out_of = [&](u32 k, u32 &coset, u32 &T) { const u32 t = cid + k * n_clusters; coset = t >> band_log; T = t & ((1u << band_log) - 1u); };
+    // GATHER: the bands in block-row order, so that the clusters at work at once gather neighbouring block rows, which share lines
+    auto out_of = [&](u32 k, u32 &coset, u32 &T) {
+        const u32 t = cid + k * n_clusters;
+        coset = t >> band_log;
+        T = t & ((1u << band_log) - 1u);
+        if constexpr (GATHER) T = tile_block_row_inv<R_LOG>(T);
+    };
     auto issue = [&](u32 k) {   // copy lane: band k's part and twiddles into ring slot k % NS
         u32 coset, T;
         out_of(k, coset, T);
@@ -766,7 +785,7 @@ ntt_band_pass_kernel(const __grid_constant__ PassArgs a, const __grid_constant__
             const bool load = !P3_SKIP(a.skip_load);
             tws[1] = tw[((size_t)1 << a.l0) + T];
             mbar_expect_tx(bar, (load ? qwords * 4 : 0) + 8 * (R - 2));
-            if (load) tma_load_gather(&imap, data0 + s * qwords, T, q * RQ, coset, bar);
+            if (load) tma_load_gather(&imap, data0 + s * qwords, tile_block_row<R_LOG>(T), q * RQ, coset, bar);
             load_tile_twiddles(tws, tw, a.l0, T, R_LOG, bar);
         } else {
             band_load_part<R_LOG, CL>(a, data0 + s * qwords, tws0 + s * R, coset, T, q, bar);
@@ -892,8 +911,12 @@ __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_k
 //     gf + j*E1, gf = bitrev_Q1(g)), so the coefficients stay in that thread's registers for all cosets;
 //   * per coset: forward step 1 in registers, stored to the tile buffer in forward layout, then forward step 2 (Q1 layers) on
 //     consecutive local rows, in place; ONE tensor copy (omap) stores the tile to that coset's output block, where the
-//     four-launch path's forward pass 1 stores it (a.tile_major: as one dense block of the tile-major scratch instead); the next
-//     coset rewrites the buffer once the copy has read it out, and the HBM writes drain while the CTA computes;
+//     four-launch path's forward pass 1 stores it; the next coset rewrites the buffer once the copy has read it out, and the HBM
+//     writes drain while the CTA computes;
+//   * TILES (the tile-major plan, make_tile_major_tensor_maps): forward step 2 stores its results from registers to the tile's
+//     dense block of the scratch a.out instead, in the block-row order of tile_block_row, in which each warp's store of one
+//     register is one whole 128-byte line.  No write-back, fence or read-out wait: the next coset's forward step 1 rewrites the
+//     buffer once every warp's step 2 has read it (one consumer barrier);
 //   * work items go in forward-tile order (L, column tile), T = bitrev_r(L): the CTAs resident at once store neighbouring
 //     output rows (runs of ~26 rows per 2^r-row group at 132 SMs) instead of rows 2^r / 32 apart, while each tile's
 //     reads stay one contiguous block of 2^r rows.
@@ -904,10 +927,13 @@ __global__ void __launch_bounds__(BAND_NARROW_THREADS, 1) ntt_band_pass_narrow_k
 // stores: the consumers write a coset's forward step 2 back, fence and arrive on ready[b]; the producer stores the tile, waits
 // until the copy has read the buffer out (the thread that commits a bulk group is the one that can wait for it) and arrives on
 // `freed`, which the consumers wait on before the next coset's forward step 1 rewrites the buffer.  After a tile's last coset
-// the producer refills the buffer with tile k + 2 instead: the consumers' only other wait is full[b].
+// the producer refills the buffer with tile k + 2 instead: the consumers' only other wait is full[b].  TILES: the producer stores
+// nothing; the consumers arrive on ready[b] once per tile, after the last coset's step 2 has read the buffer, and the producer
+// then refills it.
+// (TILES precedes CT_T so that no instance's name ends in "true, false>", the band pass's gather instance: tests match on it.)
 template <int R_LOG, int CT_T> __host__ __device__ constexpr int lde_mid_threads() { return (1 << (R_LOG / 2)) * (CT_T ? CT_T : 12); }
 
-template <int F, int R_LOG, int CT_T, bool PROD>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
+template <int F, int R_LOG, bool TILES, int CT_T, bool PROD>   // CT_T: compile-time tile width (16/20) or 0 = runtime a.ct (4/8/12)
 __global__ void __launch_bounds__(lde_mid_threads<R_LOG, CT_T>() + (PROD ? 32 : 0), 1)
 ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, const __grid_constant__ CUtensorMap omap,
                    const __grid_constant__ CUtensorMap imap) {
@@ -957,7 +983,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
     if constexpr (PROD) {
         if (threadIdx.x == 0) {
             for (u32 b = 0; b < 2; b++) { mbar_init(full_bar(b), 1); mbar_init(ready_bar(b), THREADS); }
-            mbar_init(freed_bar, 1);
+            if constexpr (!TILES) mbar_init(freed_bar, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncthreads();
@@ -986,36 +1012,39 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             if (n_mine > 1) load(1);
             for (u32 k = 0; k < n_mine; k++) {
                 const u32 b = k & 1u, tt = blockIdx.x + k * gridDim.x;
-                const u32 col = (tt % a.n_ctiles) * CT, L = tt / a.n_ctiles;
+                if constexpr (TILES) {
+                    // ready[b] completes once per tile in buffer b, when its last coset's step 2 has read the buffer
+                    mbar_wait(ready_bar(b), (k >> 1) & 1u);
+                } else {
+                    const u32 col = (tt % a.n_ctiles) * CT, L = tt / a.n_ctiles;
 #ifdef P3GPU_NTT_PROFILE
-                unsigned long long read_wait = 0;
+                    unsigned long long read_wait = 0;
 #endif
-                for (u32 cs = 0; cs < a.n_cosets; cs++) {
-                    // ready[b] completes once per coset of every tile in buffer b
-                    mbar_wait(ready_bar(b), ((k >> 1) * a.n_cosets + cs) & 1u);
-                    if (!P3_SKIP(a.skip_store)) {
+                    for (u32 cs = 0; cs < a.n_cosets; cs++) {
+                        // ready[b] completes once per coset of every tile in buffer b
+                        mbar_wait(ready_bar(b), ((k >> 1) * a.n_cosets + cs) & 1u);
+                        if (!P3_SKIP(a.skip_store)) {
 #ifdef P3GPU_NTT_PROFILE
-                        unsigned long long w0_, w1_;
-                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
+                            unsigned long long w0_, w1_;
+                            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
 #endif
-                        // tensor coordinates (column, 0, 0, L, coset), tile-major (0, 0, 0, tile, coset): see launch_lde_mid
-                        // (tile-major blocks are written in whole lines: no L2 hint, which measured the same or slower there)
-                        if (a.tile_major) tma_store_tile(&omap, data0 + b * buf_words, 0, (int)tt, (int)cs);
-                        else tma_store_tile_keep(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
-                        bulk_wait_read();   // the copy has read the buffer out: the next coset (or tile) may rewrite it
+                            // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
+                            tma_store_tile_keep(&omap, data0 + b * buf_words, (int)col, (int)L, (int)cs);
+                            bulk_wait_read();   // the copy has read the buffer out: the next coset (or tile) may rewrite it
 #ifdef P3GPU_NTT_PROFILE
-                        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
-                        read_wait += w1_ - w0_;
+                            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w1_));
+                            read_wait += w1_ - w0_;
 #endif
+                        }
+                        if (cs + 1 < a.n_cosets) mbar_arrive(freed_bar);
                     }
-                    if (cs + 1 < a.n_cosets) mbar_arrive(freed_bar);
-                }
 #ifdef P3GPU_NTT_PROFILE
-                P3_PSTAMP(k, 6, read_wait);
+                    P3_PSTAMP(k, 6, read_wait);
 #endif
+                }
                 if (k + 2 < n_mine) load(k + 2);
             }
-            bulk_wait_all();
+            if constexpr (!TILES) bulk_wait_all();
             return;
         }
     } else {
@@ -1032,7 +1061,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             P3_STAMP(1);
             mbar_wait(full_bar(buf), (k >> 1) & 1u);   // every consumer thread waits for every tile, in order
         } else {
-            if (threadIdx.x == 0) bulk_wait_read();   // the previous tile's last store has left the buffer refilled next
+            if (!TILES && threadIdx.x == 0) bulk_wait_read();   // the previous tile's last store has left the buffer refilled next
             __syncthreads();   // every warp is done with the buffer that is refilled next
 #ifdef P3GPU_NTT_PROFILE
             if (a.prof && threadIdx.x == 0 && k < 16) { u32 sm_; asm volatile("mov.u32 %0, %%smid;" : "=r"(sm_)); a.prof[((size_t)blockIdx.x * 16 + k) * 8] = sm_; }
@@ -1078,7 +1107,8 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q2>(coef, twi, E1 + g);
         }
 #ifdef P3GPU_NTT_PROFILE
-        // slot 6 (PROD: 7): time thread 0 waits for the previous coset's store to leave the buffer (PROD: for the producer's `freed`)
+        // slot 6 (PROD: 7): time thread 0 waits for the previous coset's store to leave the buffer (PROD: for the producer's `freed`;
+        // TILES: for the barrier before forward step 1)
         unsigned long long store_wait = 0;
 #endif
         for (u32 cs = 0; cs < a.n_cosets; cs++) {
@@ -1088,7 +1118,9 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             unsigned long long w0_ = 0, w1_ = 0;
             if (cs > 0) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(w0_));
 #endif
-            if (PROD && cs > 0) {
+            if constexpr (TILES) {
+                consumer_sync<PROD, THREADS>();   // every warp's step 2 of the previous coset (cs = 0: inverse step 2) has read the buffer
+            } else if (PROD && cs > 0) {
                 // the producer has seen the previous coset's store leave the buffer: `freed` completes n_cosets - 1 times per tile.
                 // coef[] is live here: at r = 10, ct = 20 a phase counter or the watchdog's registers would spill.
                 mbar_wait_plain(freed_bar, (k * (a.n_cosets - 1u) + cs - 1u) & 1u);
@@ -1110,8 +1142,27 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                 for (u32 j = 0; j < E2; j++) sp[j * gs2] = y[j];
             }
             consumer_sync<PROD, THREADS>();
-            // ---- forward step 2 (in place): item (j, c2) holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
-            {
+            // ---- forward step 2 (in place; TILES: to the tile's block of coset cs, see make_tile_major_tensor_maps): item (j, c2)
+            // holds forward local rows j*E1 + b, network rows L + (j*E1 + b) * 2^r
+            if constexpr (TILES) {
+                // cw = CT: item it = j*CT + c2 stores register b to block word tile_block_row(j*E1 + b)*CT + c2 = b*E2*CT + it, so a
+                // warp's 32 consecutive items write one whole 128-byte line per register.  (32-bit word offsets: the scratch holds
+                // fewer than 2^32 words, see coset_lde_impl.)
+                const u32 blk = (cs * total + t) * R * CT;
+                for (u32 it = threadIdx.x; it < E2 * CT; it += THREADS) {
+                    const u32 j = it / CT, c2 = it - j * CT;
+                    const u32 *sp = data + j * gs2 + c2;
+                    u32 x[E1];
+#pragma unroll
+                    for (u32 b = 0; b < E1; b++) x[b] = sp[b * CT];
+                    if (!P3_SKIP(a.skip_bfly)) reg_network<F, Q1>(x, tf, E2 + j);
+                    if (!P3_SKIP(a.skip_store)) {
+                        u32 *dst = a.out + blk + tile_block_row<R_LOG>(j * E1) * CT + c2;
+#pragma unroll
+                        for (u32 b = 0; b < E1; b++) dst[tile_block_row<R_LOG>(b) * CT] = x[b];
+                    }
+                }
+            } else {
                 u32 j = threadIdx.x / cw, c2 = threadIdx.x - j * cw;
                 for (; j < E2; ) {
                     u32 *sp = data + j * gs2 + c2;
@@ -1127,7 +1178,14 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
                     if (c2 >= cw) { c2 -= cw; j++; }
                 }
             }
-            if constexpr (PROD) {
+            if constexpr (TILES) {
+                if (PROD && cs + 1 == a.n_cosets) {
+                    // this thread's shared-memory writes are ordered before the producer's next load into this buffer; then the
+                    // producer may refill it
+                    fence_proxy_async_smem();
+                    mbar_arrive(ready_bar(buf));
+                }
+            } else if constexpr (PROD) {
                 // this thread's shared-memory writes are ordered before the producer's tensor copies (the store of this coset, and
                 // after the last coset the next load into this buffer); then the producer may take the buffer
                 fence_proxy_async_smem();
@@ -1135,11 +1193,8 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
             } else if (!P3_SKIP(a.skip_store)) {
                 fence_proxy_async_smem();
                 __syncthreads();
-                // tensor coordinates (column, 0, 0, L, coset), tile-major (0, 0, 0, tile, coset): see launch_lde_mid
-                if (threadIdx.x == 0) {
-                    if (a.tile_major) tma_store_tile(&omap, data, 0, (int)t, (int)cs);
-                    else tma_store_tile(&omap, data, (int)col, (int)L, (int)cs);
-                }
+                // tensor coordinates (column, 0, 0, L, coset): see launch_lde_mid
+                if (threadIdx.x == 0) tma_store_tile(&omap, data, (int)col, (int)L, (int)cs);
             }
         }
 #ifdef P3GPU_NTT_PROFILE
@@ -1147,7 +1202,7 @@ ntt_lde_mid_kernel(const __grid_constant__ PassArgs a, const uint2 *tw_fwd, cons
 #endif
         P3_STAMP(5);
     }
-    if (!PROD && threadIdx.x == 0) bulk_wait_all();
+    if (!PROD && !TILES && threadIdx.x == 0) bulk_wait_all();
 }
 
 // ---- pipelined path: TMA tile loads + warp-specialised consumer groups -------------------------------------------
@@ -1678,7 +1733,7 @@ static int32_t launch_band_first(p3gpu_ctx *ctx, PassArgs a) {
 // consumer threads need 168 registers against the 152 that 416 threads leave them.
 template <int R_LOG, int CT_T> constexpr bool lde_mid_producer() { return R_LOG < 10 || CT_T != 0; }
 
-template <int F, int R_LOG, int CT_T, bool PROD>
+template <int F, int R_LOG, bool TILES, int CT_T, bool PROD>
 static int32_t launch_lde_mid_rcp(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
     constexpr int Q2 = (R_LOG + 1) / 2, Q1 = R_LOG - Q2;
     constexpr int THREADS = lde_mid_threads<R_LOG, CT_T>(), BLOCK = THREADS + (PROD ? 32 : 0);
@@ -1688,7 +1743,7 @@ static int32_t launch_lde_mid_rcp(p3gpu_ctx *ctx, const PassArgs &a, const uint2
     const size_t smem = 2 * buf_words * 4 + (2 + a.n_cosets) * ((size_t)1 << R_LOG) * sizeof(uint2) + (PROD ? 5 * 8 : 0);
     P3_CHECK(smem <= 227 * 1024, P3GPU_EINVAL, "ntt: fused LDE tile does not fit shared memory");
     P3_CHECK(gs2 == (e1 + 1) * ct && gs1 == (e2 + 1) * ct, P3GPU_EINVAL, "ntt: fused LDE tile layout is no TMA box");
-    constexpr auto kern = ntt_lde_mid_kernel<F, R_LOG, CT_T, PROD>;
+    constexpr auto kern = ntt_lde_mid_kernel<F, R_LOG, TILES, CT_T, PROD>;
     P3_TRY(set_smem_limit<kern>(ctx, smem));
     const size_t tiles = ((size_t)1 << (a.log_n - R_LOG)) * a.n_ctiles;
     // persistent grid: as many CTAs per SM as threads, registers and shared memory allow (one at 2^20 rows)
@@ -1699,18 +1754,23 @@ static int32_t launch_lde_mid_rcp(p3gpu_ctx *ctx, const PassArgs &a, const uint2
     P3_CUDA(cudaGetLastError());
     return P3GPU_OK;
 }
-template <int F, int R_LOG, int CT_T>
+template <int F, int R_LOG, bool TILES, int CT_T>
 static int32_t launch_lde_mid_rc(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
-    if constexpr (lde_mid_producer<R_LOG, CT_T>()) return launch_lde_mid_rcp<F, R_LOG, CT_T, true>(ctx, a, tw_fwd, omap, imap);
-    else return launch_lde_mid_rcp<F, R_LOG, CT_T, false>(ctx, a, tw_fwd, omap, imap);
+    if constexpr (lde_mid_producer<R_LOG, CT_T>()) return launch_lde_mid_rcp<F, R_LOG, TILES, CT_T, true>(ctx, a, tw_fwd, omap, imap);
+    else return launch_lde_mid_rcp<F, R_LOG, TILES, CT_T, false>(ctx, a, tw_fwd, omap, imap);
+}
+template <int F, int R_LOG, bool TILES>
+static int32_t launch_lde_mid_rt(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
+    switch (a.ct) {
+        case 16: return launch_lde_mid_rc<F, R_LOG, TILES, 16>(ctx, a, tw_fwd, omap, imap);
+        case 20: return launch_lde_mid_rc<F, R_LOG, TILES, 20>(ctx, a, tw_fwd, omap, imap);
+        default: return launch_lde_mid_rc<F, R_LOG, TILES, 0>(ctx, a, tw_fwd, omap, imap);
+    }
 }
 template <int F, int R_LOG>
-static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, const uint2 *tw_fwd, const CUtensorMap &omap, const CUtensorMap &imap) {
-    switch (a.ct) {
-        case 16: return launch_lde_mid_rc<F, R_LOG, 16>(ctx, a, tw_fwd, omap, imap);
-        case 20: return launch_lde_mid_rc<F, R_LOG, 20>(ctx, a, tw_fwd, omap, imap);
-        default: return launch_lde_mid_rc<F, R_LOG, 0>(ctx, a, tw_fwd, omap, imap);
-    }
+static int32_t launch_lde_mid_r(p3gpu_ctx *ctx, const PassArgs &a, bool tiles, const uint2 *tw_fwd, const CUtensorMap &omap,
+                                const CUtensorMap &imap) {
+    return tiles ? launch_lde_mid_rt<F, R_LOG, true>(ctx, a, tw_fwd, omap, imap) : launch_lde_mid_rt<F, R_LOG, false>(ctx, a, tw_fwd, omap, imap);
 }
 
 // ---- pipelined kernel: host side -------------------------------------------------------------------------------
@@ -1777,38 +1837,25 @@ static int32_t make_unit_tensor_map(const u32 *base, u32 w, int log_n, int r, u3
 
 // The tile-major scratch between the fused LDE pass and the gathering last pass (2^2r rows of w = n_ct * ct columns, n_cosets
 // cosets).  Coset cs's forward tile L and column tile c make tile tt = L * n_ct + c, whose result is ONE dense block of 2^r rows x ct
-// words at word offset ((cs * 2^r + L) * n_ct + c) * 2^r * ct.  Block row i = j * 2^Q1 + b (forward step 2's local row) holds what
-// goes to row L + 2^r * i of the coset block, so row L of band i is block row i of tiles L * n_ct .. L * n_ct + n_ct - 1.
-// The fused pass stores a block as 2^Q2 runs of 2^Q1 * ct contiguous words, where the dense layout writes 2^r row segments of ct
-// words 2^r rows apart; the last pass then gathers each row of its part from n_ct blocks instead of reading one contiguous run.
-//   store map (ntt_lde_mid_kernel): (column, b, j, tile tt, coset), box (ct, 2^Q1 + 1, 2^Q2, 1, 1) = the padded forward layout, whose
-//     pad row per group the store skips;
-//   gather map (ntt_band_pass_kernel<..., GATHER>): (column, column tile, block row i, tile row L, coset), box (ct, n_ct, 1, rows, 1):
-//     rows L .. L + rows - 1 of band i, w words each, land row-major as one part.
-static int32_t encode_tile_major(TensorMapEncodeFn enc, const u32 *base, const cuuint64_t *dims, const cuuint64_t *strides, const cuuint32_t *box,
-                                 CUtensorMap *tm) {
-    const cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    const CUresult rc = enc(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
-    return P3GPU_OK;
-}
-static int32_t make_tile_major_tensor_maps(const u32 *base, u32 ct, u32 n_ct, int r, u32 n_cosets, u32 rows, CUtensorMap *store_map,
-                                           CUtensorMap *gather_map) {
+// words at word offset ((cs * 2^r + L) * n_ct + c) * 2^r * ct.  Forward step 2's local row i = j * 2^Q1 + b holds what goes to row
+// L + 2^r * i of the coset block, and is block row tile_block_row(i) = b * 2^Q2 + j: the order in which ntt_lde_mid_kernel<..., TILES,
+// ...> stores each warp's register b as one whole 128-byte line (ct % 4 == 0, so 2^Q2 * ct words are a multiple of 32).  Row L of
+// band i is block row tile_block_row(i) of tiles L * n_ct .. L * n_ct + n_ct - 1, so the last pass gathers each row of its part from
+// n_ct blocks instead of reading one contiguous run.  The gather map (ntt_band_pass_kernel<..., GATHER>) is (column, column tile,
+// block row, tile row L, coset) with box (ct, n_ct, 1, rows, 1): rows L .. L + rows - 1 of band i, w words each, land row-major as
+// one part.
+static int32_t make_tile_major_tensor_maps(const u32 *base, u32 ct, u32 n_ct, int r, u32 n_cosets, u32 rows, CUtensorMap *gather_map) {
     TensorMapEncodeFn enc = tensor_map_encoder();
     P3_CHECK(enc != nullptr, P3GPU_ECUDA, "cuTensorMapEncodeTiled is not available from this driver");
-    const int q1 = r / 2;
     const cuuint64_t seg = (cuuint64_t)ct * 4, blk = seg << r, tile_row = blk * n_ct, coset = tile_row << r;
-    {
-        const cuuint64_t dims[5] = {ct, 1ull << q1, 1ull << (r - q1), (cuuint64_t)n_ct << r, n_cosets};
-        const cuuint64_t strides[4] = {seg, seg << q1, blk, coset};
-        const cuuint32_t box[5] = {ct, (1u << q1) + 1, 1u << (r - q1), 1, 1};
-        P3_TRY(encode_tile_major(enc, base, dims, strides, box, store_map));
-    }
     const cuuint64_t dims[5] = {ct, n_ct, 1ull << r, 1ull << r, n_cosets};
     const cuuint64_t strides[4] = {blk, seg, tile_row, coset};
-    const cuuint32_t box[5] = {ct, n_ct, 1, rows, 1};
-    return encode_tile_major(enc, base, dims, strides, box, gather_map);
+    const cuuint32_t box[5] = {ct, n_ct, 1, rows, 1}, es[5] = {1, 1, 1, 1, 1};
+    const CUresult rc = enc(gather_map, CU_TENSOR_MAP_DATA_TYPE_UINT32, 5, const_cast<u32 *>(base), dims, strides, box, es,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    P3_CHECK(rc == CUDA_SUCCESS, P3GPU_ECUDA, "cuTensorMapEncodeTiled failed (%d)", (int)rc);
+    return P3GPU_OK;
 }
 
 // P3GPU_NTT_PIPE (read per call: the tests switch between the kernel families): 1 = TMA pipeline for every eligible pass and
@@ -1906,29 +1953,28 @@ static u32 lde_mid_tile_width(u32 w) {
 
 // a: the inverse network's second pass (l0 = r, l1 = 2r) over the coefficient buffer, writing the forward networks' first-pass
 // results of a.n_cosets cosets to a.out (blocks a.out_stride apart); tw_fwd: the cosets' forward heaps, a.tw_stride apart.
-// tile_map != nullptr: the results go to the tile-major scratch instead (make_tile_major_tensor_map), one dense block per tile.
+// tiles: a.out is the tile-major scratch instead (make_tile_major_tensor_maps), one dense block per tile, stored from registers.
 template <int F>
-static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd, const CUtensorMap *tile_map = nullptr) {
+static int32_t launch_lde_mid(p3gpu_ctx *ctx, PassArgs a, const uint2 *tw_fwd, bool tiles = false) {
     a.ct = lde_mid_tile_width(a.w);
     a.n_ctiles = (a.w + a.ct - 1) / a.ct;
     a.prof = prof_window();
     a.skip_bfly = env_int("P3GPU_NTT_NOBFLY", 0); a.skip_store = env_int("P3GPU_NTT_NOSTORE", 0);
-    a.tile_major = tile_map != nullptr;
     // output = the forward networks' first pass (layers [0, r)) over the cosets' blocks: tile L, local row j*2^Q1 + b at row
     // L + 2^r * (j*2^Q1 + b), i.e. the pass map with groups of 2^Q1 rows (the forward layout gs2 = (2^Q1 + 1) * ct words)
     const int r = a.l1 - a.l0;
     PassArgs o = a;
     o.l0 = 0; o.l1 = r;
     CUtensorMap omap, imap;
-    if (tile_map) omap = *tile_map;
-    else P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
+    memset(&omap, 0, sizeof omap);
+    if (!tiles) P3_TRY(make_pass_tensor_map(o, a.out, false, a.out_stride, a.ct, false, r / 2, &omap));
     // input (producer-warp form): inverse tile T = coefficient rows T * 2^r + rho in the inverse layout, groups of 2^ceil(r/2) rows
     P3_TRY(make_pass_tensor_map(a, a.in, false, 0, a.ct, false, (r + 1) / 2, &imap));
     switch (r) {
-        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tw_fwd, omap, imap);
-        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tw_fwd, omap, imap);
-        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tw_fwd, omap, imap);
-        default: return launch_lde_mid_r<F, 10>(ctx, a, tw_fwd, omap, imap);
+        case 7: return launch_lde_mid_r<F, 7>(ctx, a, tiles, tw_fwd, omap, imap);
+        case 8: return launch_lde_mid_r<F, 8>(ctx, a, tiles, tw_fwd, omap, imap);
+        case 9: return launch_lde_mid_r<F, 9>(ctx, a, tiles, tw_fwd, omap, imap);
+        default: return launch_lde_mid_r<F, 10>(ctx, a, tiles, tw_fwd, omap, imap);
     }
 }
 
@@ -2211,19 +2257,20 @@ static int32_t coset_lde_impl(p3gpu_ctx *ctx, const u32 *d_in, size_t h, size_t 
         // at least two of them; P3GPU_NTT_GATHER=0 keeps the dense layout.  The scratch holds every coset: band i's output rows
         // hold tile i's blocks, which every band reads.
         const u32 ct = lde_mid_tile_width((u32)w), n_ct = (u32)w / ct;
-        CUtensorMap store_map, gather_map;
-        bool gather = band && w > BAND_NARROW_W && w % ct == 0 && n_ct >= 2 && env_int("P3GPU_NTT_GATHER", 1) != 0;
+        CUtensorMap gather_map;
+        void *tiles = nullptr;
+        // (The band pass's slot bounds w << r, which keeps the scratch below the 2^32 words the fused pass's offsets can address.)
+        bool gather = band && w > BAND_NARROW_W && w % ct == 0 && n_ct >= 2 && n_cosets * h * w < (1ull << 32) &&
+                      env_int("P3GPU_NTT_GATHER", 1) != 0;
         if (gather) {
-            void *tiles = nullptr;
             P3_TRY(ctx_lde_tiles(ctx, n_cosets * h * w * 4, &tiles));
-            gather = make_tile_major_tensor_maps((const u32 *)tiles, ct, n_ct, r, (u32)n_cosets, (1u << r) / BAND_CL, &store_map,
-                                                 &gather_map) == P3GPU_OK;
+            gather = make_tile_major_tensor_maps((const u32 *)tiles, ct, n_ct, r, (u32)n_cosets, (1u << r) / BAND_CL, &gather_map) == P3GPU_OK;
             if (gather) b.in = (const u32 *)tiles;
         }
         memset(&a, 0, sizeof a);
         a.w = (u32)w; a.log_n = log_n; a.l0 = r; a.l1 = log_n; a.n_cosets = (u32)n_cosets;
-        a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = d_out; a.out_stride = h * w;
-        P3_TRY(launch_lde_mid<F>(ctx, a, tw, gather ? &store_map : nullptr));
+        a.tw = tw_inv; a.tw_stride = h; a.in = (const u32 *)coef; a.out = gather ? (u32 *)tiles : d_out; a.out_stride = h * w;
+        P3_TRY(launch_lde_mid<F>(ctx, a, tw, gather));
         if (band) return launch_band<F>(ctx, b, gather ? &gather_map : nullptr);
         return launch_pass<F>(ctx, b, (unsigned)n_cosets, 4);
     }

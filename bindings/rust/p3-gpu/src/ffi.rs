@@ -94,6 +94,9 @@ unsafe extern "C" {
                                  out: *mut u32, bitrev_rows: c_int) -> i32;
     pub fn p3gpu_coset_lde_batch_dev(ctx: *mut P3GpuCtx, field: c_int, d_in: *const u32, h: usize, w: usize, added_bits: c_uint, shift: u32,
                                      d_out: *mut u32, bitrev_rows: c_int) -> i32;
+    pub fn p3gpu_lde_coefficients_dev(ctx: *mut P3GpuCtx, field: c_int, d_trace: *mut u32, h: usize, w: usize) -> i32;
+    pub fn p3gpu_lde_coset_block_dev(ctx: *mut P3GpuCtx, field: c_int, d_coeffs: *const u32, h: usize, w: usize, added_bits: c_uint,
+                                     shift: u32, coset: usize, d_out: *mut u32) -> i32;
 
     // Poseidon2 constants (drawn by Rust: Poseidon2::new / new_from_rng), Mmcs::commit
     pub fn p3gpu_poseidon2_set_constants(ctx: *mut P3GpuCtx, field: c_int, width: c_int, rc_initial: *const u32, rc_terminal: *const u32,

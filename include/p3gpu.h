@@ -113,6 +113,16 @@ int32_t p3gpu_coset_lde_batch_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_i
 int32_t p3gpu_coset_lde_batch(p3gpu_ctx *ctx, int field, const uint32_t *h_in, size_t h, size_t w,
                               unsigned added_bits, uint32_t shift, uint32_t *h_out, int bitrev_rows);
 
+/* The LDE as coefficients plus one coset at a time, for a trace whose whole LDE does not fit beside it.
+ * p3gpu_lde_coefficients_dev: the h x w trace (natural rows) becomes, in its own storage, the coefficient form that
+ *   p3gpu_lde_coset_block_dev reads (network order, scaled by 1/h).  The trace is consumed; no trace-sized scratch is used.
+ * p3gpu_lde_coset_block_dev: memory rows [coset h, (coset + 1) h) of what p3gpu_coset_lde_batch_dev(.., added_bits, shift, ..,
+ *   bitrev_rows = 1) writes for that trace, word for word, into the h x w d_out (coset < 2^added_bits; d_out must not alias
+ *   d_coeffs).  Those rows are the evaluations on shift * w_K^bitrev(coset) * H in bit-reversed order. */
+int32_t p3gpu_lde_coefficients_dev(p3gpu_ctx *ctx, int field, uint32_t *d_trace, size_t h, size_t w);
+int32_t p3gpu_lde_coset_block_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_coeffs, size_t h, size_t w, unsigned added_bits,
+                                  uint32_t shift, size_t coset, uint32_t *d_out);
+
 /* ---- Poseidon2 / hashing ---------------------------------------------------------------------- */
 /* Poseidon2::new (poseidon2/src/lib.rs:50-87): round constants cross the boundary in Montgomery form.
  * width 16 or 24; rc_initial / rc_terminal: 4 x width; rc_internal: rounds_p scalars. */

@@ -45,6 +45,7 @@ EXPORTS = [
     "p3gpu_blake3_air_generate_trace_cols_dev", "p3gpu_sha256_air_generate_trace_cols_dev", "p3gpu_p1air_generate_trace_cols_dev",
     "p3gpu_blake3_air_quotient_sharded_dev", "p3gpu_sha256_air_quotient_sharded_dev", "p3gpu_p1air_quotient_sharded_dev",
     "p3gpu_air_quotient_sharded_dev",
+    "p3gpu_lde_coefficients_dev", "p3gpu_lde_coset_block_dev",
 ]
 
 PEER_CTRL_BYTES, PEER_CTRL_USER = 65536, 256
@@ -168,6 +169,8 @@ def load():
         "p3gpu_sha256_air_quotient_sharded_dev": (i32, [vp, ci, vp, vp, cu, cu, vp, vp]),
         "p3gpu_p1air_quotient_sharded_dev": (i32, [vp, ci, ci, vp, vp, cu, cu, vp, vp]),
         "p3gpu_air_quotient_sharded_dev": (i32, [vp, vp, vp, vp, vp, cu, cu, cu, vp, vp, vp]),
+        "p3gpu_lde_coefficients_dev": (i32, [vp, ci, vp, sz, sz]),
+        "p3gpu_lde_coset_block_dev": (i32, [vp, ci, vp, sz, sz, cu, u32, sz, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)

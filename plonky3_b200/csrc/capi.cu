@@ -208,6 +208,17 @@ int32_t p3gpu_coset_lde_batch_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_i
     P3_CHECK(d_in && d_out, P3GPU_EINVAL, "null argument");
     return ntt_coset_lde(ctx, field, d_in, h, w, added_bits, shift, d_out, bitrev_rows);
 }
+int32_t p3gpu_lde_coefficients_dev(p3gpu_ctx *ctx, int field, uint32_t *d_trace, size_t h, size_t w) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_trace, P3GPU_EINVAL, "null argument");
+    return ntt_lde_coefficients(ctx, field, d_trace, h, w);
+}
+int32_t p3gpu_lde_coset_block_dev(p3gpu_ctx *ctx, int field, const uint32_t *d_coeffs, size_t h, size_t w, unsigned added_bits,
+                                  uint32_t shift, size_t coset, uint32_t *d_out) {
+    P3_ENTER(ctx);
+    P3_CHECK(d_coeffs && d_out, P3GPU_EINVAL, "null argument");
+    return ntt_lde_coset_block(ctx, field, d_coeffs, h, w, added_bits, shift, coset, d_out);
+}
 // ---- host-pointer pipeline ------------------------------------------------------------------------
 // A host-pointer call is PCIe-bound (config 2: 419 MB in and 839 MB out over PCIe against milliseconds of compute).  The matrix
 // is cut into column chunks (every column is an independent polynomial) and the three stages run on three streams:

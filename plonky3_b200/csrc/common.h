@@ -122,6 +122,9 @@ int32_t ctx_leaf_table(p3gpu_ctx *ctx, size_t bytes, void **out);  // grow-only 
 int32_t ntt_dft_batch(p3gpu_ctx *ctx, int field, int kind, const u32 *d_in, u32 *d_out, size_t h, size_t w, u32 shift);
 int32_t ntt_coset_lde(p3gpu_ctx *ctx, int field, const u32 *d_in, size_t h, size_t w, unsigned added_bits, u32 shift,
                       u32 *d_out, int bitrev_rows, size_t in_pitch = 0, size_t out_pitch = 0);
+int32_t ntt_lde_coefficients(p3gpu_ctx *ctx, int field, u32 *d_trace, size_t h, size_t w);
+int32_t ntt_lde_coset_block(p3gpu_ctx *ctx, int field, const u32 *d_coef, size_t h, size_t w, unsigned added_bits, u32 shift, size_t coset,
+                            u32 *d_out);
 // hash.cu
 int32_t hash_poseidon2_permute(p3gpu_ctx *ctx, int field, int width, u32 *d_states, size_t n);
 int32_t hash_keccak_f(p3gpu_ctx *ctx, u64 *d_states, size_t n);

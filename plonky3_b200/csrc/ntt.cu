@@ -2320,6 +2320,66 @@ int32_t ntt_coset_lde(p3gpu_ctx *ctx, int field, const u32 *d_in, size_t h, size
                               : coset_lde_impl<KOALA_BEAR>(ctx, d_in, h, w, added_bits, shift, d_out, bitrev_rows, in_pitch, out_pitch);
 }
 
+// The LDE kept as coefficients plus one coset at a time, for traces whose whole LDE does not fit beside them.
+// Coefficients: the inverse network of coset_lde_impl's generic path (network order, scaled by 1/h, lazy range) run on the trace
+// itself.  Without an output remap every pass, the first one included, writes exactly the rows of its tile that it read, so the
+// passes run in place and need no scratch.
+template <int F>
+static int32_t lde_coefficients_impl(p3gpu_ctx *ctx, u32 *d_trace, size_t h, size_t w) {
+    const int log_n = (int)log2_floor(h);
+    if (log_n == 0) return P3GPU_OK;   // a constant polynomial: its one coefficient is its value
+    const uint2 *tw_inv = nullptr;
+    P3_TRY(get_twiddles<F>(ctx, log_n, 0, Fp<F>::ONE, 1, &tw_inv));
+    return run_network<F>(ctx, log_n, w, tw_inv, 0, 1, d_trace, 0, 0, d_trace, 0, 0, 0, 0, nullptr, true, inv_height_scale<F>(h), false);
+}
+
+// Memory block `coset` of the bit-reversed LDE (rows [coset h, (coset + 1) h)) from lde_coefficients_impl's coefficients: the
+// forward network of that one coset with its twiddle heap, as the LDE runs it for every coset — the first pass permutes the
+// coefficients (PERM pass), the last runs on the band kernel where it is eligible, as forward pass 2 of the LDE does.
+template <int F>
+static int32_t lde_coset_block_impl(p3gpu_ctx *ctx, const u32 *d_coef, size_t h, size_t w, unsigned added_bits, u32 shift, size_t coset,
+                                    u32 *d_out) {
+    const int log_n = (int)log2_floor(h);
+    if (log_n == 0) {   // every evaluation of a constant is the constant
+        P3_CUDA(cudaMemcpyAsync(d_out, d_coef, w * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+        return P3GPU_OK;
+    }
+    const uint2 *tw = nullptr;
+    P3_TRY(get_twiddles<F>(ctx, log_n, (int)added_bits, shift, 0, &tw));
+    const uint2 *tw_c = tw + coset * h;
+    const NetworkPlan plan = plan_passes(log_n, network_max_r());
+    if (plan.n_passes == 2) {
+        PassArgs b;
+        memset(&b, 0, sizeof b);
+        b.w = (u32)w; b.log_n = log_n; b.l0 = plan.bounds[1]; b.l1 = log_n; b.n_cosets = 1;
+        b.tw = tw_c; b.in = d_out; b.in_stride = h * w; b.out = d_out; b.out_stride = h * w; b.final_reduce = 1;
+        if (band_pass_eligible(b)) {
+            PassArgs a;
+            memset(&a, 0, sizeof a);
+            a.w = (u32)w; a.log_n = log_n; a.l0 = 0; a.l1 = plan.bounds[1];
+            a.tw = tw_c; a.in = d_coef; a.in_bitrev = 1; a.out = d_out;
+            P3_TRY(launch_pass<F>(ctx, a, 1, 4));
+            return launch_band<F>(ctx, b);
+        }
+    }
+    return run_network<F>(ctx, log_n, w, tw_c, 0, 1, d_coef, 0, 1, d_out, 0, 0, 0, 0, nullptr, false, make_uint2(0, 0), true);
+}
+
+int32_t ntt_lde_coefficients(p3gpu_ctx *ctx, int field, u32 *d_trace, size_t h, size_t w) {
+    P3_TRY(check_shape(field, h, w, 0));
+    return field == BABY_BEAR ? lde_coefficients_impl<BABY_BEAR>(ctx, d_trace, h, w) : lde_coefficients_impl<KOALA_BEAR>(ctx, d_trace, h, w);
+}
+
+int32_t ntt_lde_coset_block(p3gpu_ctx *ctx, int field, const u32 *d_coef, size_t h, size_t w, unsigned added_bits, u32 shift, size_t coset,
+                            u32 *d_out) {
+    P3_CHECK(added_bits <= 8, P3GPU_EINVAL, "added_bits %u too large", added_bits);
+    P3_TRY(check_shape(field, h, w, added_bits));
+    P3_CHECK(coset < ((size_t)1 << added_bits), P3GPU_EINVAL, "coset %zu of an LDE with %zu cosets", coset, (size_t)1 << added_bits);
+    P3_CHECK(d_coef != d_out, P3GPU_EINVAL, "the coset block cannot overwrite the coefficients");
+    return field == BABY_BEAR ? lde_coset_block_impl<BABY_BEAR>(ctx, d_coef, h, w, added_bits, shift, coset, d_out)
+                              : lde_coset_block_impl<KOALA_BEAR>(ctx, d_coef, h, w, added_bits, shift, coset, d_out);
+}
+
 // Column-sharded coset LDE whose result lands row-sharded on all ranks (SURVEY 8e: column blocks -> all-to-all -> row blocks).
 // Column chunks a rank's block of w_local columns is exchanged in (boundaries multiples of 8 columns; P3GPU_SHARD_CHUNK, default
 // 64).  Every rank computes the same list for every source rank: the chunk-major row-block layout depends on it.

@@ -414,6 +414,48 @@ def quotient_slice_natural_indices(rank: int, rows_per_rank: int, log_height: in
     return _bitrev(m, log_height)
 
 
+def natural_order(q_bitrev, log_height: int):
+    """The quotient values of the whole domain in natural order from their 2^log_height bit-reversed entries (the row blocks' slices
+    in block order): one gather."""
+    H = 1 << log_height
+    return q_bitrev[_bitrev(torch.arange(H, device=q_bitrev.device, dtype=torch.int64), log_height)].contiguous()
+
+
+def segments_rowwise_dot(gpu, f, segments, rows: int, alpha):
+    """Mred(x) = sum_c alpha^c M[x][c] for every row of a row block held as column segments [(c0, c1, (rows, c1 - c0) tensor)]:
+    rowwise_dot per segment times alpha^c0, summed.  Returns (rows, 4)."""
+    r = torch.zeros((rows, 4), dtype=torch.int32, device=segments[0][2].device)
+    for c0, c1, block in segments:
+        gpu.ef_axpy(f.id, r, gpu.rowwise_dot(f.id, block, alpha), X.ef_pow(f, alpha, c0))
+    return r
+
+
+def block_openings(gpu, segments, rows: int, sub_layers, top_layers, block: int, local, width: int, path_len: int):
+    """Mmcs::open_multi_batch answers for queries at rows `local` of row block `block` of a tree whose row blocks are sub-trees: a
+    (k, width + path_len * 8) tensor of each query's row and path.  The row is gathered from the block's column segments [(c0, c1,
+    (rows, c1 - c0) tensor)], the path's levels inside the sub-tree come from the block's digest layers `sub_layers`, the levels above
+    it from `top_layers` (host arrays: level l holds the 2^(log2(blocks) - l) digests over the sub-tree roots)."""
+    li = np.ascontiguousarray(local, dtype=np.uint32)
+    k = int(li.size)
+    sub_len = min(rows.bit_length() - 1, path_len)
+    out = torch.zeros((k, width + path_len * 8), dtype=torch.int32, device=segments[0][2].device)
+    gpu._use_torch_stream()
+    for c0, c1, blk in segments:
+        piece = gpu._empty((k, c1 - c0))
+        check(gpu.L.p3gpu_gather_rows_dev(gpu.h, blk.data_ptr(), rows, c1 - c0, li.ctypes.data, k, 0, piece.data_ptr()))
+        out[:, c0:c1] = piece
+    if sub_len:
+        lens = (C.c_size_t * len(sub_layers))(*[int(l.shape[0]) for l in sub_layers])
+        paths = gpu._empty((k, sub_len, 8))
+        check(gpu.L.p3gpu_merkle_paths_dev(gpu.h, sub_layers[0].data_ptr(), lens, len(sub_layers), sub_len, li.ctypes.data, k, 0,
+                                           paths.data_ptr()))
+        out[:, width:width + sub_len * 8] = paths.reshape(k, -1)
+    for lvl in range(path_len - sub_len):              # levels above the sub-tree roots: the same siblings for all the block's queries
+        sib = np.ascontiguousarray(top_layers[lvl][(block >> lvl) ^ 1], dtype=np.uint32)
+        out[:, width + (sub_len + lvl) * 8: width + (sub_len + lvl + 1) * 8] = torch.from_numpy(sib.view(np.int32)).to(out.device)
+    return out
+
+
 def _bitrev(x, bits: int):
     """Bit reversal of `bits`-bit indices: numpy int64 arrays or CUDA int64 tensors."""
     r = x * 0
@@ -473,8 +515,7 @@ class ShardedTrace:
         assert quotient_domain[1] == self.log_height, "the sharded quotient covers the LDE domain: log_num_quotient_chunks == log_blowup"
         H = self.shape[0]
         q_slice = air.sharded_quotient_values(self.grp, self.log_height, self.log_degree, alpha, public_values)
-        q_bitrev = self.grp.exchange(q_slice).reshape(H, 4)
-        return q_bitrev[_bitrev(torch.arange(H, device=self.device, dtype=torch.int64), self.log_height)].contiguous()
+        return natural_order(self.grp.exchange(q_slice).reshape(H, 4), self.log_height)
 
     def get_matrices(self, _data):
         return [self]
@@ -504,9 +545,7 @@ class ShardedTrace:
         grp, gpu, f = self.grp, self.gpu, self.field
         R = grp.rows_per_rank
         mine = slice(grp.rank * R, (grp.rank + 1) * R)
-        r = torch.zeros((R, 4), dtype=torch.int32, device=self.device)
-        for c0, c1, block in self.segments:
-            gpu.ef_axpy(f.id, r, gpu.rowwise_dot(f.id, block, alpha), X.ef_pow(f, alpha, c0))
+        r = segments_rowwise_dot(gpu, f, self.segments, R, alpha)
         for inv_denoms, offset, ys in terms:
             gpu.open_reduce(f.id, acc[mine], r, inv_denoms[mine], *coeff_and_yred(offset, ys))
         acc.copy_(grp.exchange(acc[mine]).reshape(acc.shape))
@@ -521,32 +560,15 @@ class ShardedTrace:
         the tree over the sub-tree roots that the commit left in the control block."""
         grp, gpu = self.grp, self.gpu
         R, W, rank = grp.rows_per_rank, grp.w_total, grp.rank
-        log_r = R.bit_length() - 1
         idx = np.asarray(indices, dtype=np.int64)
         n, plen = int(idx.size), self.path_len
-        sub_len = min(log_r, plen)
         owner, local = idx // R, idx % R
         mine = np.nonzero(owner == rank)[0]
         rec = W + plen * 8
         table = torch.zeros((n, rec), dtype=torch.int32, device=self.device)
         if mine.size:
-            li = np.ascontiguousarray(local[mine], dtype=np.uint32)
-            mine = torch.from_numpy(mine).to(table.device)
-            k = int(li.size)
-            gpu._use_torch_stream()
-            for c0, c1, block in self.segments:
-                piece = gpu._empty((k, c1 - c0))
-                check(gpu.L.p3gpu_gather_rows_dev(gpu.h, block.data_ptr(), R, c1 - c0, li.ctypes.data, k, 0, piece.data_ptr()))
-                table[mine, c0:c1] = piece
-            if sub_len:
-                lay = self.sub_layers
-                lens = (C.c_size_t * len(lay))(*[int(l.shape[0]) for l in lay])
-                paths = gpu._empty((k, sub_len, 8))
-                check(gpu.L.p3gpu_merkle_paths_dev(gpu.h, lay[0].data_ptr(), lens, len(lay), sub_len, li.ctypes.data, k, 0, paths.data_ptr()))
-                table[mine, W:W + sub_len * 8] = paths.reshape(k, -1)
-            for lvl in range(plen - sub_len):          # levels above the sub-tree roots: the same siblings for all my queries
-                sib = self.top_layers[lvl][(rank >> lvl) ^ 1]
-                table[mine, W + (sub_len + lvl) * 8: W + (sub_len + lvl + 1) * 8] = torch.from_numpy(sib.view(np.int32)).to(table.device)
+            table[torch.from_numpy(mine).to(table.device)] = block_openings(gpu, self.segments, R, self.sub_layers, self.top_layers, rank,
+                                                                             local[mine], W, plen)
         got = grp.exchange(table.reshape(-1)).reshape(grp.world, n, rec)
         ans = got[torch.from_numpy(owner).to(table.device), torch.arange(n, device=table.device)].cpu().numpy().view(np.uint32)
         return [np.ascontiguousarray(ans[:, :W])], np.ascontiguousarray(ans[:, W:]).reshape(n, plen, 8)

@@ -93,6 +93,22 @@ class Gpu:
                                            out.ctypes.data, int(bitrev_rows)))
         return out
 
+    def lde_coefficients(self, field, trace_dev):
+        """p3gpu_lde_coefficients_dev: the device trace (h, w) becomes, in place, the coefficient form `lde_coset_block` reads.
+        Returns the same tensor; its trace values are gone."""
+        m = self._dev(trace_dev); self._use_torch_stream()
+        check(self.L.p3gpu_lde_coefficients_dev(self.h, field, m.data_ptr(), m.shape[0], m.shape[1]))
+        return m
+
+    def lde_coset_block(self, field, coeffs_dev, added_bits, shift, coset, out=None):
+        """p3gpu_lde_coset_block_dev: rows [coset h, (coset + 1) h) of coset_lde_batch(trace, added_bits, shift) from the trace's
+        `lde_coefficients`, into `out` (a contiguous (h, w) CUDA int32 tensor, new if None).  Returns it."""
+        m = self._dev(coeffs_dev); self._use_torch_stream()
+        o = self._empty(tuple(m.shape)) if out is None else self._dev(out)
+        assert tuple(o.shape) == tuple(m.shape), "the coset block has the trace's shape"
+        check(self.L.p3gpu_lde_coset_block_dev(self.h, field, m.data_ptr(), m.shape[0], m.shape[1], added_bits, shift, coset, o.data_ptr()))
+        return o
+
     # ------------------------------------------------------------------ hashing
     def poseidon2_set_constants(self, field, width, rc_initial, rc_terminal, rc_internal):
         a = np.ascontiguousarray(rc_initial, dtype=np.uint32).ravel()
